@@ -153,7 +153,9 @@ lv_status lv_map_add_device(lv_handle h, const float* d_xyz, int64_t n, int down
  * LiDAR frame (device memory) and is transformed by the filter's current state, i.e. the result of the lv_correct /
  * lv_correct_device that precedes the call, without that state ever visiting the host.  lv_map_add_last_sweep reuses
  * the sweep of that update (it is still resident), so one tick is lv_correct(...); lv_map_add_last_sweep(h, 1).
- * On an empty map both build it un-downsampled (Mapper.cpp:26).  Asynchronous.                                  */
+ * On an empty map both build it un-downsampled (Mapper.cpp:26).  That is how a sequence starts: the first tick's
+ * lv_correct returns LV_EMPTY_MAP but keeps the sweep, and lv_map_add_last_sweep builds the map from it at the
+ * current (propagated) state.  Asynchronous.                                                                      */
 lv_status lv_map_add_sweep_device(lv_handle h, const float* d_xyz_lidar, int64_t n, int downsample);
 lv_status lv_map_add_last_sweep(lv_handle h, int downsample);
 
@@ -197,11 +199,14 @@ lv_status lv_predict_host(const lv_params* p, const double acc[3], const double 
                           double* x, double* P);
 /* Localizator::correct(points, time) (Localizator.cpp:23-27): the whole iterated update.
  * xyz_lidar: HOST buffer of n deskewed points in the LiDAR frame.  logs (capacity
- * LV_MAX_EVALS) / n_evals / x_out / P_out may be NULL.                                       */
+ * LV_MAX_EVALS) / n_evals / x_out / P_out may be NULL.
+ * On an empty map it returns LV_EMPTY_MAP and leaves the state, the time and x_out / P_out untouched (Localizator.cpp:24),
+ * but the sweep is still uploaded and becomes the one lv_map_add_last_sweep adds: the first tick builds the map.  */
 lv_status lv_correct(lv_handle h, const float* xyz_lidar, int64_t n, double time,
                      lv_iter_log* logs, int32_t* n_evals, double* x_out, double* P_out);
 /* same, but the points are already resident in HBM (DEVICE pointer) and nothing is copied
- * back except through lv_get_state / lv_last_logs.                                           */
+ * back except through lv_get_state / lv_last_logs.  On an empty map it returns LV_EMPTY_MAP
+ * and records the sweep for lv_map_add_last_sweep, like lv_correct.                          */
 lv_status lv_correct_device(lv_handle h, const float* d_xyz_lidar, int64_t n, double time);
 lv_status lv_last_logs(lv_handle h, lv_iter_log* logs, int32_t* n_evals);
 double lv_last_time_updated(lv_handle h);                     /* Localizator::last_time_updated */

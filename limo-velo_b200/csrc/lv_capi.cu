@@ -681,13 +681,14 @@ lv_status lv_correct(lv_handle h, const float* xyz, int64_t n, double time, lv_i
                      double* x_out, double* P_out) {
     if (!h || !xyz || n <= 0) return LV_ERR_ARG;
     if (n_evals) *n_evals = 0;
-    if (h->map.empty) return LV_EMPTY_MAP;                       /* Localizator.cpp:24 */
     if (n > h->prm.max_points) { set_error("sweep capacity exceeded"); return LV_ERR_CAPACITY; }
     LV_CUDA(cudaSetDevice(h->prm.device));
+    /* the sweep is uploaded and recorded even on an empty map: the first tick's lv_map_add_last_sweep builds the map from it */
     LV_CUDA(cudaMemcpyAsync(h->d_sweep, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
+    h->last_sweep = h->d_sweep; h->last_sweep_n = n;
+    if (h->map.empty) return LV_EMPTY_MAP;                       /* Localizator.cpp:24: the state is left as it is */
     lv_status s = enqueue_update(h, h->d_sweep, n);
     if (s != LV_OK) return s;
-    h->last_sweep = h->d_sweep; h->last_sweep_n = n;
     s = fetch_results(h);
     h->last_time_updated = time;                                  /* Localizator.cpp:26 */
     if (logs) memcpy(logs, h->logs, sizeof(lv_iter_log) * (size_t)h->n_evals);
@@ -699,10 +700,10 @@ lv_status lv_correct(lv_handle h, const float* xyz, int64_t n, double time, lv_i
 
 lv_status lv_correct_device(lv_handle h, const float* d_xyz, int64_t n, double time) {
     if (!h || !d_xyz || n <= 0) return LV_ERR_ARG;
+    h->last_sweep = d_xyz; h->last_sweep_n = n;                   /* recorded on an empty map too (see lv_correct) */
     if (h->map.empty) return LV_EMPTY_MAP;
     LV_CUDA(cudaSetDevice(h->prm.device));
     lv_status s = enqueue_update(h, d_xyz, n);
-    h->last_sweep = d_xyz; h->last_sweep_n = n;
     h->last_time_updated = time;
     h->pending_fetch = true;
     return s;

@@ -703,9 +703,12 @@ struct lvo_map {
 namespace {
 const float kDownsampleSize = 0.2f;  // KD_TREE<Point>(0.3, 0.6, 0.2) (Mapper.cpp:65)
 
+/* 21 bits per axis, wrapped: cells 2^21 apart (419 km) share a bucket, which the exact box test of lvo_map_add filters out;
+ * unmasked, a coordinate beyond +-209 km spilled into the next field and one point could be found through two keys */
 inline uint64_t vox_key(int ix, int iy, int iz) {
-    return ((uint64_t)(uint32_t)(ix + (1 << 20)) << 42) | ((uint64_t)(uint32_t)(iy + (1 << 20)) << 21) |
-           (uint64_t)(uint32_t)(iz + (1 << 20));
+    const uint64_t m = 0x1FFFFF;
+    return (((uint64_t)(uint32_t)(ix + (1 << 20)) & m) << 42) | (((uint64_t)(uint32_t)(iy + (1 << 20)) & m) << 21) |
+           ((uint64_t)(uint32_t)(iz + (1 << 20)) & m);
 }
 inline int vox_idx(float v) { return (int)std::floor(v / kDownsampleSize); }
 

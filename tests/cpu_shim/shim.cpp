@@ -66,20 +66,21 @@ static void shim_add_impl(ShimMap* sm, const float* xyz, int64_t n, int downsamp
     sm->n_inserted += (uint32_t)n;
 }
 
-ShimMap* shim_map_create(const float* xyz, int64_t m, float cell, double max_dist) {
-    (void)max_dist;
+/* cap: map points the tables are sized for (at least m): 8 table slots and 64 arena entries per point */
+ShimMap* shim_map_create_cap(const float* xyz, int64_t m, int64_t cap, float cell) {
     ShimMap* sm = new ShimMap();
     const float ds = 0.2f;
     int k = (int)floor((double)cell / (double)ds + 0.5);
     k = k < 1 ? 1 : (k > kMaxCellsPerVoxel ? kMaxCellsPerVoxel : k);
+    if (cap < m) cap = m;
     uint32_t slots = 1u << 14;
-    while (slots < 8 * (uint64_t)(m + 65536)) slots <<= 1;
+    while (slots < 8 * (uint64_t)(cap + 65536)) slots <<= 1;
     uint4 empty; empty.x = empty.y = 0xFFFFFFFFu; empty.z = empty.w = 0;
     uint4 zero; zero.x = zero.y = zero.z = zero.w = 0;
     sm->table.assign(2 * (size_t)slots, zero);
     for (uint32_t s = 0; s < slots; ++s) sm->table[2 * (size_t)s] = empty;
     sm->btable.assign(slots / 4, empty);
-    sm->arena.resize((size_t)64 * (size_t)(m + 65536) + (1u << 20));
+    sm->arena.resize((size_t)64 * (size_t)(cap + 65536) + (1u << 20));
     sm->counters.assign(kMapCounters, 0u);
     sm->counters[kCtrArenaTop] = 16u;
     sm->touched.resize(slots);
@@ -92,6 +93,10 @@ ShimMap* shim_map_create(const float* xyz, int64_t m, float cell, double max_dis
     sm->view = map_view_of(r);
     if (m > 0) shim_add_impl(sm, xyz, m, 0);
     return sm;
+}
+ShimMap* shim_map_create(const float* xyz, int64_t m, float cell, double max_dist) {
+    (void)max_dist;
+    return shim_map_create_cap(xyz, m, m, cell);
 }
 /* Mapper::add on an existing map (KD_TREE::Add_Points) */
 void shim_map_add(ShimMap* sm, const float* xyz, int64_t n, int downsample) { shim_add_impl(sm, xyz, n, downsample); }

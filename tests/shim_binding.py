@@ -31,6 +31,8 @@ def lib():
         L = C.CDLL(os.path.join(_DIR, "liblv_cpushim.so"))
         L.shim_map_create.restype = C.c_void_p
         L.shim_map_create.argtypes = [C.POINTER(C.c_float), C.c_int64, C.c_float, C.c_double]
+        L.shim_map_create_cap.restype = C.c_void_p
+        L.shim_map_create_cap.argtypes = [C.POINTER(C.c_float), C.c_int64, C.c_int64, C.c_float]
         L.shim_map_destroy.argtypes = [C.c_void_p]
         L.shim_map_add.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_int64, C.c_int]
         L.shim_map_size.argtypes = [C.c_void_p]
@@ -69,10 +71,11 @@ def make_params(oprm, voxel_size=0.5):
 
 
 class ShimMap:
-    def __init__(self, xyz, cell=0.5, max_dist=2.0):
+    def __init__(self, xyz, cell=0.5, max_dist=2.0, capacity=0):
+        """capacity: map points to size the tables for (default: the build); isolated points need 27 table slots each"""
         self.L = lib()
         xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
-        self.h = self.L.shim_map_create(_f(xyz), xyz.shape[0], C.c_float(cell), C.c_double(max_dist))
+        self.h = self.L.shim_map_create_cap(_f(xyz), xyz.shape[0], int(capacity), C.c_float(cell))
 
     def __del__(self):
         try:
@@ -113,6 +116,15 @@ class ShimMap:
                               out["valid"].ctypes.data_as(C.c_void_p), out["nn_idx"].ctypes.data_as(C.c_void_p),
                               _f(out["nn_sqd"]), _f(out["plane"]), _f(out["dist"]), _f(out["g"]), _d(out["rows"]))
         return out
+
+    def query_stats(self, x, xyz, max_dist=2.0):
+        """per query: level (0 settled at level 0, 1 home bucket but not certified, 2 no level-0 slot) and home bucket size"""
+        xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+        n = xyz.shape[0]
+        level, scanned = np.zeros(n, np.int32), np.zeros(n, np.int32)
+        self.L.shim_query_stats(C.c_void_p(self.h), _d(np.ascontiguousarray(x, np.float64)), _f(xyz), C.c_int64(n),
+                                C.c_double(max_dist), level.ctypes.data_as(C.c_void_p), scanned.ctypes.data_as(C.c_void_p))
+        return level, scanned
 
     def reuse_check(self, x0, x1, xyz, max_dist=2.0):
         xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)

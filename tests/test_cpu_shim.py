@@ -250,3 +250,90 @@ def test_block_cube_mask_matches_the_per_bit_test():
                         if -r <= dx <= r and -r <= dy <= r and -r <= dz <= r:
                             want |= 1 << c
                     assert L.shim_block_cube_mask(cbx, cby, cbz, r) == want, (cbx, cby, cbz, r)
+
+
+# ---- map geometries the surface scenes never produce (tests/geometry.py) -------------------------------------------------
+import geometry as geo  # noqa: E402
+
+# Floors on the share of queries that take each scene's path, at each voxel size it runs at: about half the share measured on
+# these seeded scenes.  "uncert" = level 0 does not settle the query (ring search), "blind" = no level-0 slot while five map
+# points lie inside the gate, "big" = the home halo bucket holds more than LV_STAGE_PTS (2560) points.
+SCENE_FLOORS = {
+    "sweep_built": ("uncert", {0.2: 0.18, 0.4: 0.06, 0.6: 0.035}),
+    "sparse": ("uncert", {0.2: 0.5, 0.4: 0.38, 0.6: 0.025}),
+    "blind": ("blind", {0.2: 0.35, 0.4: 0.26, 0.6: 0.085}),
+    "cavity": ("blind", {0.4: 0.5}),
+    "cluster": ("big", {0.4: 0.17}),
+    "tiny1": ("fewer", {0.2: 0.5, 0.4: 0.5, 0.6: 0.5}),
+    "tiny4": ("fewer", {0.2: 0.5, 0.4: 0.5, 0.6: 0.5}),
+    "tiny5": ("uncert", {0.2: 0.5, 0.4: 0.4, 0.6: 0.4}),
+    "tiny6": ("uncert", {0.2: 0.5, 0.4: 0.45, 0.6: 0.25}),
+}
+FAR_FLOOR = ("uncert", {0.2: 0.5, 0.4: 0.45, 0.6: 0.43})
+
+
+@pytest.fixture(scope="module")
+def geo_scenes(lv):
+    return {sc.name: sc for sc in geo.all_scenes(lv)}
+
+
+def _geo_cases():
+    out = []
+    for name in ["sweep_built", "sparse", "blind", "cavity", "cluster", "tiny1", "tiny4", "tiny5", "tiny6"]:
+        out += [(name, v) for v in sorted(SCENE_FLOORS[name][1])]
+    for o in geo.FAR_OFFSETS:
+        for kind in ("sweep_built", "sparse"):
+            out += [("%s@%g,%g,%g" % ((kind,) + o), v) for v in (0.2, 0.4, 0.6)]
+    return out
+
+
+def _path_share(kind, level, bucket, five):
+    return {"uncert": level >= 1, "blind": (level == 2) & five, "big": bucket > 2560, "fewer": ~five}[kind].mean()
+
+
+@pytest.mark.parametrize("name,voxel", _geo_cases())
+def test_geometry_scene_takes_its_path_and_matches_the_oracle(O, geo_scenes, name, voxel):
+    """every scene proves it exercises its path (share of queries above a floor), then the shim's search, plane fit and rows
+    equal the oracle's bit for bit.  Where the map was grown with the 0.2 m rule, the content is checked against the oracle's
+    rule (and the reference ikd-Tree's) and the search against a kd-tree over the shim's own points."""
+    sc = geo_scenes[name]
+    oprm = O.make_params()
+    sm = sc.shim_map(S, voxel)
+    assert sm.check() == 0 or geo.clamps(sc.build, voxel).any()       # clamped keys break check()'s own neighbour walk
+    assert sm.error() == 0 and sm.size() > 0
+    pts = sm.points()
+    if sc.adds:
+        backends = [O.KNN_KDTREE] + ([O.KNN_REF_IKDTREE] if O.ref_available() else [])
+        got = set(map(tuple, pts.tolist()))
+        for be in backends:
+            ref = set(map(tuple, sc.oracle_map(O, be).points().tolist()))
+            assert len(got ^ ref) <= 1e-4 * len(ref), (be, len(got ^ ref), len(ref))
+    else:
+        assert (pts == sc.build).all()
+    om = O.Map(O.KNN_KDTREE)
+    om.build(pts)
+    ref = om.match_all(sc.x, oprm, sc.queries)
+    got = sm.match_all(sc.x, S.make_params(oprm, voxel), sc.queries)
+    # the path
+    level, bucket = sm.query_stats(sc.x, sc.queries)
+    five = np.isfinite(ref["nn_sqd"][:, 4]) & (ref["nn_sqd"][:, 4].astype(np.float64) < geo.GATE ** 2)
+    kind, floors = SCENE_FLOORS.get(name, FAR_FLOOR)
+    share = _path_share(kind, level, bucket, five)
+    assert share >= floors[voxel], (kind, share)
+    if name == "cavity":             # blind with more than kRingCands occupied voxels in the r = 5 cube of every query
+        assert (np.floor(sc.queries / 0.4) == np.floor(geo.CAVITY_CENTRE / 0.4)).all()
+        assert geo.cube_occupancy(pts, geo.CAVITY_CENTRE, 0.4, 5) > 1024
+    if name in ("sweep_built", "cluster") and voxel >= 0.4:             # own extents beyond kCellCache: uncached merge
+        assert geo.max_voxel_count(sc.build, voxel) > 48
+    if "@" in name and voxel == 0.2:
+        assert geo.clamps(sc.build, voxel).mean() > 0.9
+    # the answers
+    assert (got["g"] == ref["g"]).all()
+    inside = np.isfinite(got["nn_sqd"][:, 4])
+    assert not (ref["nn_sqd"][~inside, 4].astype(np.float64) < geo.GATE ** 2).any()
+    assert (got["nn_sqd"][inside] == ref["nn_sqd"][inside]).all()
+    assert (got["valid"] == ref["valid"]).all()
+    assert (got["plane"] == ref["plane"]).all() and (got["dist"] == ref["dist"]).all()
+    st, hx, h = om.measure(sc.x, oprm, sc.queries)
+    rows = got["rows"][got["valid"] == 1]
+    assert (rows[:, :12] == hx).all() and (rows[:, 12] == h).all()

@@ -48,7 +48,9 @@ def _check_update(loc, om, oprm, x_prop, P0, sweep, O, min_matches):
     return x, logs
 
 
-def _check_points(loc, om, oprm, x_prop, sweep):
+def _check_points(loc, om, oprm, x_prop, sweep, max_ties=4):
+    """max_ties: at most this many tied queries (None: any number, each of them a tie — maps with repeated points);
+    got["ties"] counts them"""
     got = loc.match_all(x_prop, sweep)
     ref = om.match_all(x_prop, oprm, sweep)
     inside = np.isfinite(got["nn_sqd"][:, 4])
@@ -59,7 +61,9 @@ def _check_points(loc, om, oprm, x_prop, sweep):
     differ = np.nonzero((got["valid"] != ref["valid"]) | (got["plane"] != ref["plane"]).any(1) | (got["dist"] != ref["dist"]))[0]
     if len(differ):
         from test_gpu_fullsize import boundary_ties
-        assert len(differ) <= 4 and len(boundary_ties(om, ref["g"][differ])) == len(differ), differ
+        assert max_ties is None or len(differ) <= max_ties, differ
+        assert len(boundary_ties(om, ref["g"][differ])) == len(differ), differ
+    got["ties"] = len(differ)
     return got
 
 

@@ -1,9 +1,9 @@
 """The measurement path over a sweep of voxel sizes x all eight bench sweeps, under a timeout (VERDICT r1 item 1).
 
 Round 1 left a hang open: lv_search_kernel<4> (4 lanes per query) never finished on bench sweeps 5 and 7 at
-voxel_size 0.35 (deterministic in isolation, tools/k1_isolate.py; the 1- and 8-lane instantiations of the same source
-were fine).  The per-query kernel now exists with 1 and 8 lanes only, the default path searches from shared memory,
-and this test pins the whole family: every voxel size the grid can take (k = 1, 2, 3 downsample cells per edge; 0.3,
+voxel_size 0.35 (deterministic in isolation; the 1- and 8-lane instantiations of the same source were fine).  The per-query
+kernel exists with 1, 4 and 8 lanes (lv_search_kernel<4> is the default for launches of 40 000 queries or more; every
+shape runs on the maps of test_gpu_geometry.py), and this test pins the whole family: every voxel size the grid can take (k = 1, 2, 3 downsample cells per edge; 0.3,
 0.35 and 0.5 round to a neighbour), every bench sweep, both query orders, bit-exact against the oracle.
 A kernel that does not terminate fails the test through pytest-timeout (thread method: the process is ended)."""
 import numpy as np
