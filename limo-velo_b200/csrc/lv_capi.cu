@@ -66,6 +66,10 @@ struct lv_context {
     size_t bin_tmp_bytes = 0;
     double* d_imu = nullptr;           /* kImuBatch x 7: lv_propagate_device */
     double* h_imu = nullptr;           /* pinned */
+    /* recorded after the last H2D copy out of h_imu / h_ctrl: the calls return before those copies run (they queue behind
+     * the update), so the next refill of the pinned buffer waits for this event, not for the whole stream */
+    cudaEvent_t imu_copied = nullptr;
+    cudaEvent_t ctrl_copied = nullptr;
     int64_t last_sweep_n = 0;          /* points of the sweep d_sweep holds (lv_correct / lv_measure*), for lv_map_add_last_sweep */
     const float* last_sweep = nullptr; /* device pointer of the sweep of the last update */
     bool use_reuse = true;
@@ -294,6 +298,8 @@ lv_status lv_create(const lv_params* p, lv_handle* out) {
     LV_CREATE_CUDA(cudaMalloc(&h->d_ctrl, sizeof(UpdateCtrl)));
     LV_CREATE_CUDA(cudaMemset(h->d_ctrl, 0, sizeof(UpdateCtrl)));
     LV_CREATE_CUDA(cudaMallocHost(&h->h_ctrl, sizeof(UpdateCtrl)));
+    LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->imu_copied, cudaEventDisableTiming));
+    LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->ctrl_copied, cudaEventDisableTiming));
     LV_CREATE_CUDA(cudaMalloc(&h->d_partials, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
     LV_CREATE_CUDA(cudaMemset(h->d_partials, 0, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
     LV_CREATE_CUDA(cudaMalloc(&h->d_group_rows, sizeof(double) * kPartialStride * 32));
@@ -319,6 +325,8 @@ void lv_destroy(lv_handle h) {
     for (auto& e : h->pending) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     for (auto& e : h->pool) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     for (auto& u : h->graphs) { cudaGraphExecDestroy(u.exec); cudaGraphDestroy(u.graph); }
+    if (h->imu_copied) cudaEventDestroy(h->imu_copied);
+    if (h->ctrl_copied) cudaEventDestroy(h->ctrl_copied);
     cudaFree(h->d_job); cudaFree(h->d_ref); cudaFree(h->d_redo); cudaFree(h->d_imu); cudaFreeHost(h->h_imu);
     cudaFree(h->d_bin_key); cudaFree(h->d_bin_val); cudaFree(h->d_bin_key_in); cudaFree(h->d_bin_val_in); cudaFree(h->d_redo_flag); cudaFree(h->d_bin_tmp);
     cudaFree(h->d_path); cudaFreeHost(h->h_path); cudaFree(h->d_times); cudaFree(h->d_deskew_in); cudaFree(h->d_bad); cudaFreeHost(h->h_bad);
@@ -508,12 +516,15 @@ lv_status lv_propagate_device(lv_handle h, const double* acc, const double* gyro
                                 h->prm.covariance_bias_acceleration};
     for (int32_t s0 = 0; s0 < k; s0 += kImuBatch) {
         const int32_t kb = k - s0 < kImuBatch ? k - s0 : kImuBatch;
-        if (s0 > 0) LV_CUDA(cudaStreamSynchronize(h->stream));    /* the pinned staging buffer is reused */
+        /* the pinned staging buffer is reused: the previous copy out of it (an earlier batch, or an earlier call still
+         * queued behind an update) must have run before it is refilled */
+        LV_CUDA(cudaEventSynchronize(h->imu_copied));
         for (int32_t i = 0; i < kb; ++i) {
             for (int a = 0; a < 3; ++a) { h->h_imu[7 * i + a] = acc[3 * (s0 + i) + a]; h->h_imu[7 * i + 3 + a] = gyro[3 * (s0 + i) + a]; }
             h->h_imu[7 * i + 6] = dt[s0 + i];
         }
         LV_CUDA(cudaMemcpyAsync(h->d_imu, h->h_imu, sizeof(double) * 7 * kb, cudaMemcpyHostToDevice, h->stream));
+        LV_CUDA(cudaEventRecord(h->imu_copied, h->stream));
         LV_CUDA(launch_predict(h->d_ctrl, noise, h->d_imu, kb, h->stream));
         h->prof.total_launches += 1;
     }
@@ -523,13 +534,16 @@ lv_status lv_propagate_device(lv_handle h, const double* acc, const double* gyro
 double lv_last_time_updated(lv_handle h) { return h ? h->last_time_updated : -1; }
 
 static lv_status upload_state(lv_context* h, const double* x, const double* P) {
-    /* x, P are staged through the pinned mirror so the copy is truly asynchronous */
+    /* x, P are staged through the pinned mirror so the copy is truly asynchronous; an earlier upload may still be queued
+     * behind an update (lv_correct_device, lv_propagate_device return without synchronising) */
+    LV_CUDA(cudaEventSynchronize(h->ctrl_copied));
     memcpy(h->h_ctrl->x, x, sizeof(double) * kStateLen);
     if (P) memcpy(h->h_ctrl->P, P, sizeof(double) * kN * kN);
     /* x and P are adjacent in UpdateCtrl: one copy (each small copy costs several microseconds of latency) */
     static_assert(offsetof(UpdateCtrl, P) == offsetof(UpdateCtrl, x) + sizeof(double) * kStateLen, "x, P adjacent");
     LV_CUDA(cudaMemcpyAsync(h->d_ctrl->x, h->h_ctrl->x, sizeof(double) * (kStateLen + (P ? kN * kN : 0)),
                             cudaMemcpyHostToDevice, h->stream));
+    LV_CUDA(cudaEventRecord(h->ctrl_copied, h->stream));
     return LV_OK;
 }
 

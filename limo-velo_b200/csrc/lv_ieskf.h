@@ -364,8 +364,10 @@ LV_HD_NOINLINE void sym_eig6(const double* Ain, double* ev, double* V) {
     for (int i = 0; i < 36; ++i) V[i] = Vs[i];
 }
 
-/* dnd[0:6] = V^-1 * sel * dx_[0:6]  (esekfom.hpp:1736-1744), executed by one thread */
-LV_HD_NOINLINE void degenerate_mask(const double* HTH, double D, const double* dxs, double* dnd) {
+/* dnd[0:6] = V^-1 * sel * dx_[0:6]  (esekfom.hpp:1736-1744), executed by one thread.  Returns 1 when an eigenvalue lies
+ * below D (the reference's test, VAPs(vapi) < D): the Cholesky pre-test all_eigs_above() also sends an eigenvalue of exactly
+ * D here, which masks nothing. */
+LV_HD_NOINLINE int degenerate_mask(const double* HTH, double D, const double* dxs, double* dnd) {
     double A6[36], ev[6], V[36], sel[36];
     for (int i = 0; i < 6; ++i)
         for (int j = 0; j < 6; ++j) A6[i * 6 + j] = HTH[i * 12 + j];
@@ -375,9 +377,12 @@ LV_HD_NOINLINE void degenerate_mask(const double* HTH, double D, const double* d
     if (prod < 1e-20)
         for (int i = 0; i < 36; ++i) V[i] = (i % 7 == 0) ? 1.0 : 0.0;
     for (int i = 0; i < 36; ++i) sel[i] = V[i];
+    int masked = 0;
     for (int j = 0; j < 6; ++j)
-        if (ev[j] < D)
+        if (ev[j] < D) {
+            masked = 1;
             for (int c = 0; c < 6; ++c) sel[j * 6 + c] = 0;
+        }
     double t[6];
     for (int i = 0; i < 6; ++i) {
         double s = 0;
@@ -405,6 +410,7 @@ LV_HD_NOINLINE void degenerate_mask(const double* HTH, double D, const double* d
         }
     }
     for (int i = 0; i < 6; ++i) dnd[i] = M[i * 7 + 6];
+    return masked;
 }
 
 /* true iff every eigenvalue of HTH[0:6,0:6] exceeds D: Cholesky of (A - D I) succeeds */
@@ -522,8 +528,8 @@ LV_HD_NOINLINE void ieskf_step(Ex& ex, const IeskfParams& prm, UpdateCtrl* c, Ie
      * lemma gives  P_inv[:, :12] = S[:, :12] (I12 + Q S11)^-1  exactly, also for singular Q
      * (estimate_extrinsics = false).  So one 12x12 system with 13 right-hand sides replaces both
      * inverses:  Y = (I + Q S11)^-1 [Q | HTh],  K_x[:, :12] = S[:, :12] Y[:, :12],  K_h = S[:, :12] Y[:, 12].
-     * Against exact arithmetic this is at least as accurate as the reference's formulation
-     * (DESIGN.md, "gain formulation").                                                              */
+     * Against 50-digit arithmetic both forms stay within cond * 2^-53 (tests/test_gpu_filter.py, DESIGN.md section 2
+     * "Gain"); neither is uniformly the more accurate.                                               */
     const double invR = 1.0 / prm.R;
     LV_PAR(it, 12 * 25) {
         const int i = it / 25, j = it - i * 25;
@@ -604,14 +610,14 @@ LV_HD_NOINLINE void ieskf_step(Ex& ex, const IeskfParams& prm, UpdateCtrl* c, Ie
     ex.sync();
     if (w->degen) {        /* esekfom.hpp:1736-1744: mask dx_[0:6] and redo the boxplus serially */
         if (ex.tid == 0) {
-            degenerate_mask(w->HTH, prm.D, w->dxs, w->dnd);
+            lg->degenerate = degenerate_mask(w->HTH, prm.D, w->dxs, w->dnd);   /* the log reports the reference's decision */
             for (int i = 0; i < kStateLen; ++i) w->xn[i] = w->x[i];
             state_boxplus(w->xn, w->dnd);
             make_frame(w->xn, &c->frame);
         }
         ex.sync();
     }
-    if (ex.is_task(1)) lg->degenerate = w->degen;
+    if (ex.is_task(1) && !w->degen) lg->degenerate = 0;
     LV_PAR(i, kStateLen) {
         const double v = w->xn[i];
         w->x[i] = v;

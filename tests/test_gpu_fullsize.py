@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import bench
+import ikfom_mp as M
 
 pytestmark = pytest.mark.gpu
 
@@ -34,7 +35,7 @@ def boundary_ties(om, g):
     return np.array(out, dtype=np.int64)
 
 
-def check_every_evaluation(O, om, oprm, x_prior, P_prior, sweep, logs, loc=None):
+def check_every_evaluation(O, om, oprm, x_prior, P_prior, sweep, logs, loc=None, P_gpu=None):
     """The tight form of "the update matches the oracle": evaluation by evaluation, AT THE ITERATE THE GPU MEASURED.
     For evaluation k the GPU's iterate is x_prior (k = 0) or the previous log's x_after.  At that very iterate the oracle's
     measurement (kNN = the reference ikd-Tree where available, plane fit, rows) must give the same Nm and the same normal
@@ -48,9 +49,15 @@ def check_every_evaluation(O, om, oprm, x_prior, P_prior, sweep, logs, loc=None)
       * with T removed from the sweep, a fresh GPU measurement and the oracle must again agree to 1e-12 (every other query
         is bit-for-bit the same on both sides);
       * the normal equations the update logged may differ from a fresh GPU measurement of the full sweep only by the rows of
-        T: the difference matrix must have rank <= 2 |T| (one row taken out, one put in, per tied query)."""
+        T: the difference matrix must have rank <= 2 |T| (one row taken out, one put in, per tied query).
+    Every evaluation's `converged` flag must be the oracle's decision (its limit test, then the loop rule of
+    esekfom.hpp:1757-1762).  With `P_gpu` (the update's covariance) the exit block is checked too, from the GPU's own last
+    iterate and normal equations: against the 50-digit reference (ikfom_mp) the GPU's P must be at least as close as the
+    oracle's exit block (fp64, the reference's two inverses; ~1e-9 off at these sizes, so a 1e-12 bar against the oracle
+    would measure the oracle), or within 1e-12."""
     x_k = np.array(x_prior, dtype=np.float64)
     ties = 0
+    t = 0
     for k, lg in enumerate(logs):
         st, HTH, HTh, nm = om.measure_reduced(x_k, oprm, sweep)
         assert st == 0
@@ -76,6 +83,22 @@ def check_every_evaluation(O, om, oprm, x_prior, P_prior, sweep, logs, loc=None)
         dx, x_new, P_now, Kx, conv = O.update_step(x_prior, P_prior, x_k, oprm, HTH, HTh)
         assert np.abs(dx - lg["dx"]).max() < 1e-9, (k, np.abs(dx - lg["dx"]).max())
         assert np.abs(x_new - lg["x_after"]).max() < 1e-9, (k, np.abs(x_new - lg["x_after"]).max())
+        t_in = t
+        t += conv
+        if not t and k - 1 == oprm.max_num_iters - 2:               # loop variable i = k - 1
+            conv = 1
+        assert lg["converged"] == conv, (k, lg["converged"], conv)
+        if P_gpu is not None and k == len(logs) - 1:
+            # the exit block from the GPU's own last iterate and normal equations, in 50 digits and in the oracle's fp64
+            r = M.evaluate(x_prior, P_prior, x_k, HTH, HTh, oprm.lidar_noise, oprm.degeneracy_threshold, list(oprm.limits),
+                           k - 1, t_in, oprm.max_num_iters)
+            assert r["finish"]
+            Pm = M.to_np(r["P"])
+            P_o = O.update_finish(x_prior, lg["x_after"], lg["dx"], P_now, Kx)
+            e_gpu = np.abs(P_gpu - Pm).max() / np.abs(Pm).max()
+            e_o = np.abs(P_o - Pm).max() / np.abs(Pm).max()
+            print("check_every_evaluation: final P against 50 digits: GPU %.1e, oracle %.1e (Nm %d)" % (e_gpu, e_o, lg["n_matches"]))
+            assert e_gpu <= max(e_o, 1e-12), (k, e_gpu, e_o)
         x_k = lg["x_after"]
     return ties
 
@@ -99,7 +122,7 @@ def test_full_size_update_matches_oracle(lv, O, full):
         # by ~1e-10 (different but equally valid fp64 evaluation orders); SURVEY 8c states 1e-6 for dx_
         assert np.abs(a["dx"] - b["dx"]).max() < (1e-9 if k == 0 else 1e-8), (k, np.abs(a["dx"] - b["dx"]).max())
     assert np.abs(x - x_o).max() < 1e-8
-    check_every_evaluation(O, om, full["oprm"], x_prop, full["P0"], sweep, logs, loc)
+    check_every_evaluation(O, om, full["oprm"], x_prop, full["P0"], sweep, logs, loc, P_gpu=P)
     err = np.abs(O.boxminus(x, full["truths"][0]))
     assert err[:3].max() < 5e-3 and err[3:6].max() < 5e-4          # centimetre-level localisation
     # per-point parity at full size
@@ -191,7 +214,7 @@ def test_streaming_predict_correct_map_update(lv, O, full):
         st_o, xo, Po, logs_o = om.update_iterated(xo, Po, full["oprm"], sweep)                 # free chain
         assert st == st_s == st_o == 0 and len(logs) == len(logs_s) == len(logs_o)
         # every evaluation, at the GPU's own iterate: same matches, same normal equations, same step (1e-9) — no inference
-        check_every_evaluation(O, om, full["oprm"], x_prior, P_prior, sweep, logs, loc)
+        check_every_evaluation(O, om, full["oprm"], x_prior, P_prior, sweep, logs, loc, P_gpu=P)
         # what the LAST evaluation really fitted its planes to (stored neighbours where lv_reuse_kernel vouched for them, searched
         # ones elsewhere) against a fresh search at the same iterate: the same five map points for every query, except where the
         # 5th and 6th are exactly equidistant
