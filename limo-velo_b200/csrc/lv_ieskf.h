@@ -86,6 +86,7 @@ struct IeskfWork {
     double J[3][9];           /* J blocks: SO3@3, SO3@6 (3x3), S2@21 (2x2 in the first 4) */
     double L[kN * kN];
     double xn[kStateLen];     /* x [+] dx_ while x is still needed                        */
+    Rt32 X, IL;               /* pose and extrinsics of xn, for the frame products        */
     double pivval;
     int64_t n_matches;
     int32_t piv;
@@ -140,57 +141,25 @@ struct ExecBlock {
             if (tid == 0) { *s_piv = r; *s_pivval = M[r * w + k]; }
         }
     }
-    /* Gauss-Jordan with partial pivoting on the 12 x 25 system [A | B] of the gain, inside warp 0, lane j owning column j.
-     * Same pivots and the same operations on the same values as gj_solve(), so the same result; 12 barrier-free steps
-     * instead of 36 block barriers.  On return M[k][12..24] = (A^-1 B)[k].
-     * Two forms.  The default holds each column in 12 registers with every step unrolled: 4 100 straight-line instructions
-     * that warp 0 runs through once per evaluation (clock64, tools/step_timing.py).  -DLV_GJ_SMEM keeps the
-     * matrix in shared memory and rolls the 12 steps (150 instructions of code); it was written against this kernel's
-     * instruction-fetch stalls — and was slower: the shared-memory round trips cost more than the fetches. */
-#if defined(LV_GJ_SMEM)
-    __device__ __noinline__ void solve_12x25(double* M, int32_t*, double*) {
-        if (tid < 32) {
-            const int lane = tid;
-            const bool act = lane < 25;
-            if (lane == 0) LV_TK(48);
-#pragma unroll 1
-            for (int k = 0; k < 12; ++k) {
-                /* every lane finds the pivot of column k itself (broadcast reads): row >= k with the largest |value|, lowest on ties */
-                int p = k;
-                double best = fabs(M[k * 25 + k]);
-#pragma unroll 1
-                for (int i = k + 1; i < 12; ++i) {
-                    const double v = fabs(M[i * 25 + k]);
-                    if (v > best) { best = v; p = i; }
-                }
-                const double ipv = 1.0 / M[p * 25 + k];
-                __syncwarp();                            /* column k is about to change under the readers */
-                double ck = 0.0;                         /* the scaled pivot row, this lane's column */
-                if (act) {
-                    const double a = M[k * 25 + lane], b = M[p * 25 + lane];
-                    if (p != k) M[p * 25 + lane] = a;
-                    ck = b * ipv;
-                    M[k * 25 + lane] = ck;
-                }
-                __syncwarp();
-                double m[12];                            /* the multipliers: column k after the swap */
+    /* c[idx] for a run-time idx in 0..11, by a 4-level multiplexer: the registers stay registers */
+    __device__ __forceinline__ static double pick12(const double (&c)[12], int idx) {
+        double t[6], u[3];
 #pragma unroll
-                for (int i = 0; i < 12; ++i) m[i] = M[i * 25 + k];
-                __syncwarp();
-                if (act) {
+        for (int q = 0; q < 6; ++q) t[q] = (idx & 1) ? c[2 * q + 1] : c[2 * q];
 #pragma unroll
-                    for (int i = 0; i < 12; ++i)
-                        if (i != k) M[i * 25 + lane] -= m[i] * ck;
-                }
-                __syncwarp();
-            }
-            if (lane == 0) { LV_TK(49); LV_TK(52); }
-        }
-        __syncthreads();
+        for (int q = 0; q < 3; ++q) u[q] = (idx & 2) ? t[2 * q + 1] : t[2 * q];
+        return (idx & 8) ? u[2] : ((idx & 4) ? u[1] : u[0]);
     }
-#else
-    /* lane j holds column j in 12 registers, lane k picks the pivot of step k, the multipliers M[i][k] travel by shuffle */
-    __device__ __noinline__ void solve_12x25(double* M, int32_t*, double*) {
+    /* Gauss-Jordan with partial pivoting on the 12 x 25 system [A | B] of the gain, inside warp 0, lane j owning column j
+     * in 12 registers.  Same pivots and the same operations on the same values as gj_solve(), so the same result; 12
+     * barrier-free steps instead of 36 block barriers.  On return M[k][12..24] = (A^-1 B)[k].
+     * The loop over k is rolled, so one step's code stays in the instruction cache (unrolled, the 12 steps were 4 100
+     * straight-line instructions that streamed through it on every evaluation, from HBM after an L2 flush).  At step k,
+     * lane k parks its column in column k of M (dead storage: only columns 12..24 are written back); the pivot search
+     * and the multipliers read it from there.  The arg-max is the pairwise tournament over rows k..11, lowest row on
+     * ties, with lane j holding row k + j: the pairs of the tournament over registers k..11 that lane k ran before;
+     * lanes past row 11 hold -1, which never wins a pair. */
+    __device__ __forceinline__ void solve_12x25(double* M, int32_t*, double*) {
         if (tid < 32) {
             const int lane = tid;
             const unsigned full = 0xffffffffu;
@@ -198,31 +167,38 @@ struct ExecBlock {
 #pragma unroll
             for (int i = 0; i < 12; ++i) col[i] = lane < 25 ? M[i * 25 + lane] : 0.0;
             if (lane == 0) LV_TK(48);
-            /* fully unrolled over k: every register index below is static, only the swap partner p is data */
-#pragma unroll
+#pragma unroll 1
             for (int k = 0; k < 12; ++k) {
-                /* lane k: arg-max of |col[i]|, i >= k, lowest row on ties (pairwise tournament) */
-                double v[12];
-                int r[12];
+                if (lane == k) {
 #pragma unroll
-                for (int i = k; i < 12; ++i) { v[i] = fabs(col[i]); r[i] = i; }
+                    for (int i = 0; i < 12; ++i) M[i * 25 + k] = col[i];
+                }
+                __syncwarp();
+                double v = lane < 12 - k ? fabs(M[(k + lane) * 25 + k]) : -1.0;
+                int r = k + lane;
 #pragma unroll
-                for (int s = 1; s < 12; s *= 2)
+                for (int s = 1; s < 12; s *= 2) {
+                    const double ov = __shfl_down_sync(full, v, s);
+                    const int orow = __shfl_down_sync(full, r, s);
+                    if ((lane & (2 * s - 1)) == 0 && ov > v) { v = ov; r = orow; }
+                }
+                const int p = __shfl_sync(full, r, 0);
+                const double ipv = 1.0 / M[p * 25 + k];
+                /* swap rows k and p: of this lane's column, and of the multipliers (column k) */
+                const double mk = M[k * 25 + k];
+                double m[12];
 #pragma unroll
-                    for (int i = k; i + s < 12; i += 2 * s)
-                        if (v[i + s] > v[i]) { v[i] = v[i + s]; r[i] = r[i + s]; }
-                const int p = __shfl_sync(full, r[k], k);
-                /* swap rows k and p of this lane's column */
-                double ck = col[k];
+                for (int i = 0; i < 12; ++i) m[i] = M[i * 25 + k];
+                const double a = pick12(col, k), b = pick12(col, p);
+                const double ck = b * ipv;               /* the scaled pivot row, this lane's column */
 #pragma unroll
-                for (int i = k + 1; i < 12; ++i)
-                    if (i == p) { const double tmp = col[i]; col[i] = ck; ck = tmp; }
-                const double ipv = 1.0 / __shfl_sync(full, ck, k);
-                ck *= ipv;                               /* the scaled pivot row, this lane's column */
-                col[k] = ck;
+                for (int i = 0; i < 12; ++i) {
+                    if (i == p && i > k) { col[i] = a; m[i] = mk; }
+                    if (i == k) col[i] = ck;
+                }
 #pragma unroll
                 for (int i = 0; i < 12; ++i)
-                    if (i != k) col[i] -= __shfl_sync(full, col[i], k) * ck;
+                    if (i != k) col[i] -= m[i] * ck;
             }
             if (lane == 0) LV_TK(49);
 #pragma unroll
@@ -232,7 +208,6 @@ struct ExecBlock {
         }
         __syncthreads();
     }
-#endif
 };
 #endif
 
@@ -569,27 +544,27 @@ LV_HD_NOINLINE void ieskf_step(Ex& ex, const IeskfParams& prm, UpdateCtrl* c, Ie
     LV_CK(7);
 
     /* x [+]= dx_ (esekfom.hpp:1747), assuming the non-degenerate case (the test of :1736-1744 ran beside the
-     * solve); the rare degenerate case redoes the update below.  Pieces of make_frame() ride along. */
+     * solve); the rare degenerate case redoes the update below.  Pieces of make_frame() ride along: the pose
+     * (task 0) and the extrinsics (task 1) in two warps, their products after the barrier. */
     LV_PAR(i, 144) lg->HTH[i] = w->HTH[i];
     LV_PAR(i, 12) lg->HTh[i] = w->HTh[i];
     LV_PAR(i, n) lg->dx[i] = w->dxs[i];
     LV_TK(24 + (ex.tid >> 5));
-    if (ex.is_task(0)) {   /* pose and extrinsics -> the frame of the next measurement (make_frame, State.cpp:51-62) */
+    if (ex.is_task(0)) {   /* pose -> the frame of the next measurement (make_frame, State.cpp:51-62) */
         for (int i = 0; i < 3; ++i) w->xn[kPos + i] = w->x[kPos + i] + w->dnd[i];
-        for (int i = 0; i < 3; ++i) w->xn[kOffT + i] = w->x[kOffT + i] + w->dnd[9 + i];
         const Quatd q = quat_mul(load_quat(w->x + kRot), so3_exp(load_vec3(w->dnd + 3), 0.5));
-        const Quatd ql = quat_mul(load_quat(w->x + kOffR), so3_exp(load_vec3(w->dnd + 6), 0.5));
         store_quat(w->xn + kRot, q);
-        store_quat(w->xn + kOffR, ql);
         const Mat3d R = quat_to_rot(q), Ri = quat_to_rot(quat_conj(q));
+        for (int i = 0; i < 9; ++i) { w->X.R[i] = (float)R.m[i]; c->frame.R_inv[i] = Ri.m[i]; }
+        for (int i = 0; i < 3; ++i) w->X.t[i] = (float)w->xn[kPos + i];
+    }
+    if (ex.is_task(1)) {   /* extrinsics */
+        for (int i = 0; i < 3; ++i) w->xn[kOffT + i] = w->x[kOffT + i] + w->dnd[9 + i];
+        const Quatd ql = quat_mul(load_quat(w->x + kOffR), so3_exp(load_vec3(w->dnd + 6), 0.5));
+        store_quat(w->xn + kOffR, ql);
         const Mat3d RL = quat_to_rot(ql), RLi = quat_to_rot(quat_conj(ql));
-        Rt32 X, IL;
-        for (int i = 0; i < 9; ++i) { X.R[i] = (float)R.m[i]; IL.R[i] = (float)RL.m[i]; }
-        for (int i = 0; i < 3; ++i) { X.t[i] = (float)w->xn[kPos + i]; IL.t[i] = (float)w->xn[kOffT + i]; }
-        for (int i = 0; i < 9; ++i) { c->frame.R_inv[i] = Ri.m[i]; c->frame.RLI_inv[i] = RLi.m[i]; }
-        c->frame.lidar_to_world = rt_mul(X, IL);
-        c->frame.world_to_lidar = rt_mul(rt_inv(IL), rt_inv(X));
-        c->frame.lidar_to_imu = IL;
+        for (int i = 0; i < 9; ++i) { w->IL.R[i] = (float)RL.m[i]; c->frame.RLI_inv[i] = RLi.m[i]; }
+        for (int i = 0; i < 3; ++i) w->IL.t[i] = (float)w->xn[kOffT + i];
     }
     if (ex.is_task(2)) store_vec3(w->xn + kGrav, s2_boxplus(load_vec3(w->x + kGrav), w->dnd[21], w->dnd[22]));
     if (ex.is_task(3)) {
@@ -616,8 +591,14 @@ LV_HD_NOINLINE void ieskf_step(Ex& ex, const IeskfParams& prm, UpdateCtrl* c, Ie
             make_frame(w->xn, &c->frame);
         }
         ex.sync();
+    } else {
+        if (ex.is_task(0)) c->frame.lidar_to_world = rt_mul(w->X, w->IL);
+        if (ex.is_task(1)) {
+            c->frame.world_to_lidar = rt_mul(rt_inv(w->IL), rt_inv(w->X));
+            c->frame.lidar_to_imu = w->IL;
+            lg->degenerate = 0;
+        }
     }
-    if (ex.is_task(1) && !w->degen) lg->degenerate = 0;
     LV_PAR(i, kStateLen) {
         const double v = w->xn[i];
         w->x[i] = v;

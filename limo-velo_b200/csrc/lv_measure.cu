@@ -793,6 +793,7 @@ __device__ void reduce_partials_block(const double* partials, int n_partials, do
     __syncthreads();
     if (threadIdx.x < 91) {
         double s = 0;
+#pragma unroll 16   /* the loads of a step's 16 warps are issued together, only the additions stay in warp order */
         for (int w = 0; w < nwarps; ++w) s += s_tmp[w * 96 + threadIdx.x];
         const int e = threadIdx.x;
         if (e < 78) {
