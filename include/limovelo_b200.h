@@ -159,6 +159,51 @@ lv_status lv_map_add_device(lv_handle h, const float* d_xyz, int64_t n, int down
 lv_status lv_map_add_sweep_device(lv_handle h, const float* d_xyz_lidar, int64_t n, int downsample);
 lv_status lv_map_add_last_sweep(lv_handle h, int downsample);
 
+/* ---- map capacity.  The ikd-Tree has none: it allocates nodes for as long as the sequence runs (Mapper.cpp:22-30,
+ * ikd_Tree.cpp:478-573).  The device map is sized from lv_params.max_map_points at lv_create and can grow after it:
+ * new, larger tables and arena, the old content re-hashed / copied into them on the handle's stream.  A growth keeps
+ * the content, the point ids, the insertion order and every arena index, so results do not change: only the storage
+ * behind the map gets bigger.  It never shrinks. */
+/* grow now so that the map holds at least `points` points at the ratios of lv_create (4 voxel slots, 96 arena float4
+ * per point).  Asynchronous.  No-op when `points` is not above the current capacity.  LV_ERR_CAPACITY (the map
+ * untouched, lv_last_error names the ceiling) beyond 2^26 voxel slots or 0x7FFFFFF0 arena entries (ids are int32),
+ * i.e. beyond 2^24 points; LV_ERR_CAPACITY with the CUDA error when the device is out of memory (map untouched). */
+lv_status lv_map_reserve(lv_handle h, int64_t points);
+/* automatic growth up to a capacity of `max_points` points (0: off, the default).  With it on, before every add
+ * (lv_map_add*, lv_map_add_last_sweep) the host bounds what the map will hold after it from the newest counter snapshot
+ * the device has finished (no synchronisation) plus the adds queued since: points + n, voxel slots + 27 n, block slots
+ * + n, arena + 96 n; it doubles the capacity while a bound crosses its mark (points above capacity, slots or blocks
+ * above half their table, arena above 3/4).  lv_map_build(_device) of m > capacity and adds of n > the add capacity grow
+ * to fit instead of failing.  What this does NOT guarantee: the arena figure is a planning ratio, not a bound, and the
+ * limit caps every growth, so an add can still overflow (one huge scattered add on a small limit); that is reported as
+ * LV_ERR_CAPACITY by the next synchronising call exactly as without growth.  Growth past the limit is refused with
+ * LV_ERR_CAPACITY where an add cannot even be staged (n above the add capacity at the limit).  Enabling synchronises
+ * once (to read the counters). */
+lv_status lv_map_set_growth(lv_handle h, int64_t max_points);
+/* (a struct tag, not a typedef: the function below has the same name) */
+struct lv_map_info {
+    /* capacity */
+    int64_t capacity_points;   /* points the tables and the arena are sized for                          */
+    int64_t voxel_slots;       /* 32-byte slots of the voxel table                                        */
+    int64_t block_slots;       /* 16-byte slots of the block table                                        */
+    int64_t arena_entries;     /* float4 entries of the arena                                             */
+    int64_t add_capacity;      /* most points one build / add takes                                       */
+    int64_t bytes;             /* device bytes of the map: tables, arena, lists, add scratch               */
+    /* usage (device counters) */
+    int64_t points;
+    int64_t slots_used;
+    int64_t blocks_used;
+    int64_t arena_top;         /* arena entries handed out (abandoned extents included)                   */
+    /* growth */
+    int64_t growths;           /* growths so far: lv_map_reserve and automatic                            */
+    int64_t growth_limit;      /* lv_map_set_growth's max_points; 0 = off                                 */
+    int64_t host_waits;        /* times the growth policy waited for a pending counter snapshot          */
+    uint32_t error_flags;      /* device error flags (0: none; see LV_ERR_CAPACITY)                      */
+    uint32_t pad_;
+};
+/* Mapper::size and more: capacity, usage and growth of the map; synchronises */
+lv_status lv_map_info(lv_handle h, struct lv_map_info* out);
+
 /* ---- operator boundary: the measurement model IKFoM calls (esekfom.hpp:128,1637) --------- */
 /* compat mode: fills h_x (Nm x 12, COLUMN-major like Eigen::MatrixXd) and h (Nm) exactly as
  * IKFoM::h_share_model does (use-ikfom.cpp:16-37); rows in input-point order.                */

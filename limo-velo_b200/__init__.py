@@ -53,6 +53,15 @@ class Profile(C.Structure):
                 ("reuse_ms", C.c_double), ("search_first_ms", C.c_double), ("search_first_launches", C.c_int64)]
 
 
+class MapInfo(C.Structure):
+    """struct lv_map_info: capacity, usage and growth of the device map"""
+    _fields_ = [("capacity_points", C.c_int64), ("voxel_slots", C.c_int64), ("block_slots", C.c_int64),
+                ("arena_entries", C.c_int64), ("add_capacity", C.c_int64), ("bytes", C.c_int64),
+                ("points", C.c_int64), ("slots_used", C.c_int64), ("blocks_used", C.c_int64), ("arena_top", C.c_int64),
+                ("growths", C.c_int64), ("growth_limit", C.c_int64), ("host_waits", C.c_int64),
+                ("error_flags", C.c_uint32), ("pad_", C.c_uint32)]
+
+
 def build(verbose=False):
     """Compile liblimovelo_b200.so in-tree with nvcc for sm_90a (works without a GPU)."""
     cmd = ["make", "-C", _HERE, "-j8"]
@@ -95,6 +104,10 @@ def lib():
     L.lv_map_status.argtypes = [vp]
     L.lv_map_add_sweep_device.argtypes = [vp, vp, i64, C.c_int]
     L.lv_map_add_last_sweep.argtypes = [vp, C.c_int]
+    if hasattr(L, "lv_map_reserve"):   # map growth; absent from older builds that tools/ab_bench.py may load via LV_LIB_PATH
+        L.lv_map_reserve.argtypes = [vp, i64]
+        L.lv_map_set_growth.argtypes = [vp, i64]
+        L.lv_map_info.argtypes = [vp, C.POINTER(MapInfo)]
     L.lv_measure.argtypes = [vp, dp, fp, i64, dp, dp, C.POINTER(i64)]
     L.lv_measure_reduced.argtypes = [vp, dp, fp, i64, dp, dp, C.POINTER(i64)]
     L.lv_match_all.argtypes = [vp, dp, fp, i64, C.POINTER(C.c_uint8), i32p, fp, fp, fp, fp]
@@ -370,6 +383,20 @@ class Localizer:
 
     def map_size(self):
         return int(self.L.lv_map_size(self.h))
+
+    def map_reserve(self, points):
+        """grow the map now to a capacity of at least `points` points (asynchronous; no-op below the capacity)"""
+        return _check(self.L.lv_map_reserve(self.h, int(points)))
+
+    def map_set_growth(self, max_points):
+        """let the map grow by itself before an add that may not fit, up to a capacity of max_points points (0: off)"""
+        return _check(self.L.lv_map_set_growth(self.h, int(max_points)))
+
+    def map_info(self):
+        """capacity, usage (device counters) and growth of the map as a dict; synchronises"""
+        out = MapInfo()
+        _check(self.L.lv_map_info(self.h, C.byref(out)))
+        return {k: getattr(out, k) for k, _ in MapInfo._fields_ if k != "pad_"}
 
     def map_points(self):
         n = self.map_size()

@@ -119,6 +119,21 @@ struct lv_context {
     std::vector<UpdateGraph> graphs;
     MeasureJob* d_job = nullptr;
     bool use_graph = true;
+    /* map growth (lv_map_set_growth): after every add the 64 B of map counters are copied into a pinned ring and an event is
+     * recorded; before the next add the host bounds the map from the newest snapshot the device has finished */
+    enum { kSnapRing = 4 };
+    int64_t grow_limit = 0;            /* 0: off */
+    int64_t growths = 0;
+    int64_t grow_waits = 0;
+    int64_t waited_at_cap = 0;         /* capacity at which the policy last waited for a snapshot */
+    uint32_t* h_snap = nullptr;       /* pinned, kSnapRing x kMapCounters */
+    cudaEvent_t snap_ev[kSnapRing] = {};
+    int64_t snap_seq[kSnapRing] = {-1, -1, -1, -1};   /* add sequence number a slot holds (-1: none) */
+    int64_t snap_cum[kSnapRing] = {};  /* points enqueued up to and including that add */
+    int64_t add_seq = 0;               /* adds enqueued since the last clear */
+    int64_t add_cum = 0;               /* points of those adds */
+    uint32_t known[kMapCounters] = {}; /* newest finished snapshot (or the cleared map) */
+    int64_t known_seq = 0, known_cum = 0;
 };
 
 static lv_status drain_events(lv_context* h) {
@@ -265,7 +280,7 @@ lv_status lv_create(const lv_params* p, lv_handle* out) {
     fill_iprm(h);
     if (p->stream) { h->stream = (cudaStream_t)p->stream; h->own_stream = false; }
     else { LV_CREATE_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    LV_CREATE_CUDA(map_alloc(h->map, p->max_map_points, p->max_points, p->voxel_size, p->map_downsample_size));
+    LV_CREATE_CUDA(map_alloc(h->map, p->max_map_points, p->max_points, p->voxel_size, p->map_downsample_size, h->stream));
     { int l = 0; LV_CREATE_CUDA(map_clear(h->map, h->stream, &l)); }
     LV_CREATE_CUDA(cudaMalloc(&h->d_sweep, sizeof(float) * 3 * p->max_points));
     LV_CREATE_CUDA(cudaMalloc(&h->d_nn_a, sizeof(int4) * p->max_points));
@@ -327,6 +342,8 @@ void lv_destroy(lv_handle h) {
     for (auto& u : h->graphs) { cudaGraphExecDestroy(u.exec); cudaGraphDestroy(u.graph); }
     if (h->imu_copied) cudaEventDestroy(h->imu_copied);
     if (h->ctrl_copied) cudaEventDestroy(h->ctrl_copied);
+    for (cudaEvent_t e : h->snap_ev) if (e) cudaEventDestroy(e);
+    cudaFreeHost(h->h_snap);
     cudaFree(h->d_job); cudaFree(h->d_ref); cudaFree(h->d_redo); cudaFree(h->d_imu); cudaFreeHost(h->h_imu);
     cudaFree(h->d_bin_key); cudaFree(h->d_bin_val); cudaFree(h->d_bin_key_in); cudaFree(h->d_bin_val_in); cudaFree(h->d_redo_flag); cudaFree(h->d_bin_tmp);
     cudaFree(h->d_path); cudaFreeHost(h->h_path); cudaFree(h->d_times); cudaFree(h->d_deskew_in); cudaFree(h->d_bad); cudaFreeHost(h->h_bad);
@@ -354,6 +371,174 @@ static lv_status map_status_from_mirror(lv_context* h) {
 }
 static void count_map_launches(lv_context* h, int launches) { h->prof.total_launches += launches; }
 
+/* ---- map growth (lv_map_reserve, lv_map_set_growth) ------------------------------------------ */
+enum : int64_t { kMaxCapPoints = (int64_t)kMaxSlots / 4 };   /* the largest capacity under both ceilings */
+
+static void drop_update_graphs(lv_context* h) {
+    /* the update graphs bake the map view (table, masks, arena) and the bin sort width into their kernel arguments; a graph
+     * still in flight is freed when it completes */
+    for (auto& u : h->graphs) { cudaGraphExecDestroy(u.exec); cudaGraphDestroy(u.graph); }
+    h->graphs.clear();
+}
+static lv_status map_grow_to(lv_context* h, int64_t cap) {
+    if (cap <= h->map.cap) return LV_OK;
+    char buf[512];
+    if (const char* c = map_ceiling(cap)) {
+        snprintf(buf, sizeof(buf), "map capacity of %lld points is past the %s", (long long)cap, c);
+        set_error(buf);
+        return LV_ERR_CAPACITY;
+    }
+    EventPair ep;
+    const bool pr = prof_begin(h, 2, &ep);
+    const int64_t old_cap = h->map.cap;
+    int launches = 0;
+    const cudaError_t e = map_grow(h->map, cap, h->stream, &launches);
+    if (pr) prof_end(h, &ep);
+    if (e != cudaSuccess) {
+        snprintf(buf, sizeof(buf), "map growth from %lld to %lld points: %s", (long long)old_cap, (long long)cap, cudaGetErrorString(e));
+        set_error(buf);
+        return h->map.cap == old_cap ? LV_ERR_CAPACITY : LV_ERR_CUDA;   /* allocation failed: the old map is intact */
+    }
+    drop_update_graphs(h);
+    h->growths++;
+    count_map_launches(h, launches);
+    return LV_OK;
+}
+/* the smallest capacity, doubling from the current one, at which every bound lies under its mark (DESIGN.md §3) */
+static int64_t grow_target(const lv_context* h, const uint32_t* c, int64_t pend) {
+    const int64_t pts = (int64_t)(int32_t)c[kCtrPoints] + pend;
+    const int64_t slots = (int64_t)c[kCtrSlotsUsed] + 27 * pend;    /* own voxel + 26 dilated neighbours per new point */
+    const int64_t blocks = (int64_t)c[kCtrBlocksUsed] + pend;       /* a new block needs a newly occupied voxel */
+    const int64_t arena = (int64_t)c[kCtrArenaTop] + 96 * pend;     /* map_alloc's planning ratio */
+    int64_t cap = h->map.cap;
+    for (;;) {
+        const MapSizes z = map_sizes(cap, h->map.max_points, false);
+        if (pts <= cap && 2 * slots <= (int64_t)z.slots && 2 * blocks <= (int64_t)z.bslots && 4 * arena <= 3 * (int64_t)z.arena_cap) return cap;
+        if (cap >= kMaxCapPoints) return cap;
+        cap = cap * 2 < kMaxCapPoints ? cap * 2 : kMaxCapPoints;
+    }
+}
+/* newest finished counter snapshot -> h->known; returns the ring slot of the newest one still pending (-1: none).  Never blocks. */
+static int snap_absorb(lv_context* h) {
+    int pending = -1;
+    for (int i = 0; i < lv_context::kSnapRing; ++i) {
+        if (h->snap_seq[i] <= h->known_seq) continue;
+        const cudaError_t q = cudaEventQuery(h->snap_ev[i]);
+        if (q == cudaErrorNotReady) {
+            if (pending < 0 || h->snap_seq[i] > h->snap_seq[pending]) pending = i;
+            continue;
+        }
+        if (q != cudaSuccess) continue;
+        memcpy(h->known, h->h_snap + (size_t)i * kMapCounters, sizeof(h->known));
+        h->known_seq = h->snap_seq[i];
+        h->known_cum = h->snap_cum[i];
+    }
+    if (pending >= 0 && h->snap_seq[pending] <= h->known_seq) pending = -1;
+    if (cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();
+    return pending;
+}
+/* before an add of n points (clears: a build, which empties the map first): grow when the bounds call for it */
+static lv_status grow_before_add(lv_context* h, int64_t n, bool clears) {
+    if (!h->grow_limit) return LV_OK;
+    int64_t want;
+    if (clears) {
+        uint32_t zero[kMapCounters] = {};
+        want = grow_target(h, zero, n);
+    } else {
+        const int pending = snap_absorb(h);
+        want = grow_target(h, h->known, h->add_cum - h->known_cum + n);
+        /* maybe only stale: wait for the newest snapshot, once per capacity (a map that sits near a mark would otherwise
+         * wait on every tick; the next decision at this capacity grows on the stale bound instead) */
+        if (want > h->map.cap && pending >= 0 && h->waited_at_cap != h->map.cap) {
+            LV_CUDA(cudaEventSynchronize(h->snap_ev[pending]));
+            h->waited_at_cap = h->map.cap;
+            h->grow_waits++;
+            snap_absorb(h);
+            want = grow_target(h, h->known, h->add_cum - h->known_cum + n);
+        }
+    }
+    const int64_t lim = h->grow_limit < kMaxCapPoints ? h->grow_limit : kMaxCapPoints;
+    if (want > lim) want = lim;                                    /* at the limit: the add is enqueued as without growth */
+    return map_grow_to(h, want);
+}
+/* after an add: its counters into the pinned ring, behind it on the stream */
+static lv_status snap_after_add(lv_context* h, int64_t n) {
+    h->add_seq++;
+    h->add_cum += n;
+    if (!h->grow_limit) return LV_OK;
+    const int i = (int)(h->add_seq % lv_context::kSnapRing);
+    LV_CUDA(cudaMemcpyAsync(h->h_snap + (size_t)i * kMapCounters, h->map.counters, sizeof(uint32_t) * kMapCounters,
+                            cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaEventRecord(h->snap_ev[i], h->stream));
+    h->snap_seq[i] = h->add_seq;
+    h->snap_cum[i] = h->add_cum;
+    return LV_OK;
+}
+static void snap_reset_cleared(lv_context* h) {                    /* map_clear: the counters are known again */
+    memset(h->known, 0, sizeof(h->known));
+    h->known[kCtrArenaTop] = 16u;
+    h->known_seq = h->known_cum = h->add_seq = h->add_cum = 0;
+    for (int i = 0; i < lv_context::kSnapRing; ++i) h->snap_seq[i] = -1;
+}
+static lv_status capacity_error(lv_context* h, const char* what) {
+    char buf[256];
+    if (h->grow_limit)
+        snprintf(buf, sizeof(buf), "%s: map growth limit reached (%lld points, lv_map_set_growth)", what, (long long)h->grow_limit);
+    else
+        snprintf(buf, sizeof(buf), "%s", what);
+    set_error(buf);
+    return LV_ERR_CAPACITY;
+}
+
+lv_status lv_map_reserve(lv_handle h, int64_t points) {
+    if (!h || points < 0) return LV_ERR_ARG;
+    if (points <= h->map.cap) return LV_OK;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    return map_grow_to(h, points);
+}
+lv_status lv_map_set_growth(lv_handle h, int64_t max_points) {
+    if (!h || max_points < 0) return LV_ERR_ARG;
+    if (max_points == 0) { h->grow_limit = 0; return LV_OK; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    if (!h->h_snap) {
+        LV_CUDA(cudaMallocHost(&h->h_snap, sizeof(uint32_t) * kMapCounters * lv_context::kSnapRing));
+        for (cudaEvent_t& e : h->snap_ev) LV_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    }
+    if (!h->grow_limit) {                                          /* the counters as of now: the base of the bounds */
+        LV_CUDA(map_fetch_counters(h->map, h->stream));
+        LV_CUDA(cudaStreamSynchronize(h->stream));
+        memcpy(h->known, h->map.h_counters, sizeof(h->known));
+        h->known_seq = h->add_seq;
+        h->known_cum = h->add_cum;
+        for (int i = 0; i < lv_context::kSnapRing; ++i) h->snap_seq[i] = -1;
+    }
+    h->grow_limit = max_points;
+    return LV_OK;
+}
+lv_status lv_map_info(lv_handle h, struct lv_map_info* out) {
+    if (!h || !out) return LV_ERR_ARG;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(map_fetch_counters(h->map, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    const MapBuffers& b = h->map;
+    memset(out, 0, sizeof(*out));
+    out->capacity_points = b.cap;
+    out->voxel_slots = b.slots;
+    out->block_slots = b.bslots;
+    out->arena_entries = b.arena_cap;
+    out->add_capacity = b.add_cap;
+    out->bytes = map_bytes(b);
+    out->points = (int64_t)(int32_t)b.h_counters[kCtrPoints];
+    out->slots_used = b.h_counters[kCtrSlotsUsed];
+    out->blocks_used = b.h_counters[kCtrBlocksUsed];
+    out->arena_top = b.h_counters[kCtrArenaTop];
+    out->growths = h->growths;
+    out->growth_limit = h->grow_limit;
+    out->host_waits = h->grow_waits;
+    out->error_flags = b.h_counters[kCtrError];
+    return LV_OK;
+}
+
 static lv_status map_build_device_impl(lv_context* h, const float* d_xyz, int64_t m) {
     EventPair ep;
     const bool pr = prof_begin(h, 2, &ep);
@@ -362,7 +547,8 @@ static lv_status map_build_device_impl(lv_context* h, const float* d_xyz, int64_
     LV_CUDA(map_add(h->map, d_xyz, m, 0, h->stream, &launches));              /* Build: no downsampling (Mapper.cpp:68-71) */
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
-    return LV_OK;
+    snap_reset_cleared(h);
+    return snap_after_add(h, m);
 }
 static lv_status map_add_device_impl(lv_context* h, const float* d_xyz, int64_t n, int downsample) {
     EventPair ep;
@@ -371,22 +557,26 @@ static lv_status map_add_device_impl(lv_context* h, const float* d_xyz, int64_t 
     LV_CUDA(map_add(h->map, d_xyz, n, downsample ? 1 : 0, h->stream, &launches));
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
-    return LV_OK;
+    return snap_after_add(h, n);
 }
 
 lv_status lv_map_build(lv_handle h, const float* xyz, int64_t m) {
     if (!h || (!xyz && m > 0)) return LV_ERR_ARG;
     if (m <= 0) return LV_OK;                                    /* Mapper.cpp:23 */
-    if (m > h->map.cap) { set_error("map capacity exceeded"); return LV_ERR_CAPACITY; }
     LV_CUDA(cudaSetDevice(h->prm.device));
+    lv_status s = grow_before_add(h, m, true);
+    if (s != LV_OK) return s;
+    if (m > h->map.cap) return capacity_error(h, "map capacity exceeded");
     LV_CUDA(cudaMemcpyAsync(h->map.stage_xyz, xyz, sizeof(float) * 3 * m, cudaMemcpyHostToDevice, h->stream));
     return map_build_device_impl(h, h->map.stage_xyz, m);
 }
 lv_status lv_map_build_device(lv_handle h, const float* d_xyz, int64_t m) {
     if (!h || (!d_xyz && m > 0)) return LV_ERR_ARG;
     if (m <= 0) return LV_OK;
-    if (m > h->map.cap) { set_error("map capacity exceeded"); return LV_ERR_CAPACITY; }
     LV_CUDA(cudaSetDevice(h->prm.device));
+    lv_status s = grow_before_add(h, m, true);
+    if (s != LV_OK) return s;
+    if (m > h->map.cap) return capacity_error(h, "map capacity exceeded");
     return map_build_device_impl(h, d_xyz, m);
 }
 int64_t lv_map_size(lv_handle h) {
@@ -416,16 +606,22 @@ lv_status lv_map_add(lv_handle h, const float* xyz, int64_t n, int downsample) {
     if (!h || (!xyz && n > 0)) return LV_ERR_ARG;
     if (n <= 0) return LV_OK;                                    /* Mapper.cpp:23 */
     if (h->map.empty) return lv_map_build(h, xyz, n);            /* Mapper.cpp:26 */
-    if (n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
+    if (!h->grow_limit && n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
     LV_CUDA(cudaSetDevice(h->prm.device));
+    lv_status s = grow_before_add(h, n, false);
+    if (s != LV_OK) return s;
+    if (n > h->map.add_cap) return capacity_error(h, "more points than one lv_map_add can take (max_map_points)");
     LV_CUDA(cudaMemcpyAsync(h->map.stage_xyz, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
     return map_add_device_impl(h, h->map.stage_xyz, n, downsample);
 }
 lv_status lv_map_add_device(lv_handle h, const float* d_xyz, int64_t n, int downsample) {
     if (!h || (!d_xyz && n > 0)) return LV_ERR_ARG;
     if (n <= 0) return LV_OK;
-    if (n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
+    if (!h->grow_limit && n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
     LV_CUDA(cudaSetDevice(h->prm.device));
+    lv_status s = grow_before_add(h, n, h->map.empty);
+    if (s != LV_OK) return s;
+    if (n > h->map.add_cap) return capacity_error(h, "more points than one lv_map_add can take (max_map_points)");
     if (h->map.empty) return map_build_device_impl(h, d_xyz, n);
     return map_add_device_impl(h, d_xyz, n, downsample);
 }
@@ -438,18 +634,21 @@ static lv_status add_sweep_impl(lv_context* h, const float* d_xyz_lidar, int64_t
         if (s != LV_OK) return s;
         h->state_dirty = false;
     }
+    lv_status s = grow_before_add(h, n, false);
+    if (s != LV_OK) return s;
+    if (n > h->map.add_cap) return capacity_error(h, "more points than one lv_map_add can take (max_map_points)");
     EventPair ep;
     const bool pr = prof_begin(h, 2, &ep);
     int launches = 0;
     LV_CUDA(map_add_sweep(h->map, h->d_ctrl, d_xyz_lidar, n, downsample ? 1 : 0, h->stream, &launches));
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
-    return LV_OK;
+    return snap_after_add(h, n);
 }
 lv_status lv_map_add_sweep_device(lv_handle h, const float* d_xyz_lidar, int64_t n, int downsample) {
     if (!h || (!d_xyz_lidar && n > 0)) return LV_ERR_ARG;
     if (n <= 0) return LV_OK;
-    if (n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
+    if (!h->grow_limit && n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
     LV_CUDA(cudaSetDevice(h->prm.device));
     return add_sweep_impl(h, d_xyz_lidar, n, downsample);
 }

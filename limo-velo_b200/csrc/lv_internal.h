@@ -94,14 +94,30 @@ struct MapBuffers {
     void* sort_tmp;
     size_t sort_tmp_bytes;
     int sort_bits;
-    int64_t cap;               /* max_map_points (sizes the tables and the arena)             */
+    int64_t cap;               /* max_map_points, then what the last growth sized for (tables and arena) */
     int64_t add_cap;           /* most points one build / add can take                        */
+    int64_t max_points;        /* lv_params.max_points: add_cap never drops below it          */
     int64_t n_inserted;        /* ids handed out so far                                       */
     bool empty;                /* nothing was ever added (Mapper::exists, Mapper.cpp:32-34)   */
+    cudaStream_t stream;       /* the stream the buffers were allocated on (stream-ordered)   */
 };
 
-cudaError_t map_alloc(MapBuffers& b, int64_t max_map_points, int64_t max_points, float voxel_size, float ds);
+/* what map_alloc / map_grow allocate for a capacity of `cap` points */
+enum : uint32_t { kMaxSlots = 1u << 26, kMaxArena = 0x7FFFFFF0u };   /* hard ceilings: slot << kCellBits and point ids are 32-bit */
+struct MapSizes {
+    uint32_t slots, bslots, arena_cap;
+    int64_t add_cap;
+    size_t sort_tmp_bytes;
+};
+MapSizes map_sizes(int64_t cap, int64_t max_points, bool scratch = true);   /* scratch: size the radix sort's temporary too */
+/* NULL when `cap` points fit under the hard ceilings, else the name of the ceiling it crosses */
+const char* map_ceiling(int64_t cap);
+int64_t map_bytes(const MapBuffers& b);
+
+cudaError_t map_alloc(MapBuffers& b, int64_t max_map_points, int64_t max_points, float voxel_size, float ds, cudaStream_t st);
 void map_free(MapBuffers& b);
+/* grow to a capacity of `cap` points (no-op when cap <= b.cap); keeps content, ids, insertion order and arena indices */
+cudaError_t map_grow(MapBuffers& b, int64_t cap, cudaStream_t st, int* launches);
 /* empty the map (table, block table, counters); asynchronous */
 cudaError_t map_clear(MapBuffers& b, cudaStream_t st, int* launches);
 /* KD_TREE::Build (downsample = 0 on an empty map) / Add_Points: n points in DEVICE memory; asynchronous, no host round trip */

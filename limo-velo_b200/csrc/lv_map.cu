@@ -179,62 +179,35 @@ __global__ void __launch_bounds__(256) lv_sweep_to_world_kernel(const UpdateCtrl
     out[3 * (size_t)i] = g[0]; out[3 * (size_t)i + 1] = g[1]; out[3 * (size_t)i + 2] = g[2];
 }
 
+/* ---- growth (map_grow) ------------------------------------------------------------------------------------ */
+/* the new tables start empty; the re-hash recounts the slots and blocks it re-inserts */
+__global__ void __launch_bounds__(256) lv_map_grow_init_kernel(uint4* table, uint32_t slots, uint4* btable, uint32_t bslots,
+                                                                uint32_t* counters) {
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    for (size_t i = i0; i < 2 * (size_t)slots; i += stride)
+        table[i] = (i & 1u) ? make_uint4(0u, 0u, 0u, 0u) : make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u);
+    for (size_t i = i0; i < (size_t)bslots; i += stride) btable[i] = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0u, 0u);
+    if (i0 == 0) { counters[kCtrSlotsUsed] = 0u; counters[kCtrBlocksUsed] = 0u; }
+}
+/* one thread per old slot: voxel slots first, then block slots (the two tables are independent) */
+__global__ void __launch_bounds__(256) lv_map_rehash_kernel(const VoxelMapRW m, const uint4* __restrict__ old_table, uint32_t old_slots,
+                                                             const uint4* __restrict__ old_btable, uint32_t old_bslots) {
+    const uint32_t stride = gridDim.x * blockDim.x;
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < old_slots + old_bslots; t += stride) {
+        if (t < old_slots) voxel_rehash_item(m, old_table, t);
+        else block_rehash_item(m, old_btable, t - old_slots);
+    }
+}
+/* the used prefix [0, counters[kCtrArenaTop]) of the arena, read on the device: the host never needs the count */
+__global__ void __launch_bounds__(256) lv_map_arena_copy_kernel(const float4* __restrict__ src, float4* __restrict__ dst, uint32_t old_cap,
+                                                                 const uint32_t* __restrict__ counters) {
+    const uint32_t top = min(counters[kCtrArenaTop], old_cap);
+    const uint32_t stride = gridDim.x * blockDim.x;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < top; i += stride) dst[i] = src[i];
+}
+
 /* ---- host side ------------------------------------------------------------------------------------------- */
-static uint32_t pow2_at_least(uint64_t v, uint32_t lo, uint32_t hi) {
-    uint64_t p = lo;
-    while (p < v && p < hi) p <<= 1;
-    return (uint32_t)p;
-}
-
-cudaError_t map_alloc(MapBuffers& b, int64_t max_map_points, int64_t max_points, float voxel_size, float ds) {
-    memset(&b, 0, sizeof(b));
-    b.cap = max_map_points;
-    b.grid.ds = ds;
-    int k = (int)floor((double)voxel_size / (double)ds + 0.5);
-    k = k < 1 ? 1 : (k > kMaxCellsPerVoxel ? kMaxCellsPerVoxel : k);
-    b.grid.k = k;
-    b.grid.cell0 = (float)k * ds;
-    /* occupied + dilated voxels of a surface-like map: ~1 slot per map point; 4x keeps the load below 0.3, scattered
-     * maps (27 slots per isolated point) run out and report LV_ERR_CAPACITY instead of hanging */
-    b.slots = pow2_at_least(4ull * (uint64_t)max_map_points, 1u << 16, 1u << 26);
-    b.bslots = pow2_at_least((uint64_t)b.slots / 4u, 1u << 14, 1u << 27);
-    /* own extents (~1.5x the map) + halo buckets (27 copies of every point, up to 50 % slack) + the extents that
-     * buckets outgrow (geometric growth: at most twice the live ones): 1.5 KB per map point of capacity */
-    uint64_t arena = 96ull * (uint64_t)max_map_points + (4ull << 20);
-    if (arena > 0x7FFFFFF0ull) arena = 0x7FFFFFF0ull;                       /* ids are int32 */
-    b.arena_cap = (uint32_t)arena;
-    b.list_cap = b.slots;
-    b.add_cap = max_map_points > max_points ? max_map_points : max_points;
-    cudaError_t e;
-    if ((e = cudaMalloc(&b.table, sizeof(uint4) * 2 * (size_t)b.slots)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.btable, sizeof(uint4) * (size_t)b.bslots)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.arena, sizeof(float4) * (size_t)b.arena_cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.counters, sizeof(uint32_t) * kMapCounters)) != cudaSuccess) return e;
-    if ((e = cudaMallocHost(&b.h_counters, sizeof(uint32_t) * kMapCounters)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.touched, sizeof(uint32_t) * (size_t)b.list_cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.dirty, sizeof(uint32_t) * (size_t)b.list_cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.stage_xyz, sizeof(float) * 3 * (size_t)b.add_cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.skeys, sizeof(uint32_t) * (size_t)b.add_cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.skeys_alt, sizeof(uint32_t) * (size_t)b.add_cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.svals, sizeof(uint32_t) * (size_t)b.add_cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&b.svals_alt, sizeof(uint32_t) * (size_t)b.add_cap)) != cudaSuccess) return e;
-    b.sort_bits = kCellBits;
-    for (uint32_t s = b.slots; s > 1; s >>= 1) b.sort_bits++;
-    b.sort_tmp_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, b.sort_tmp_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
-                                    (uint32_t*)nullptr, (int)b.add_cap, 0, 32);
-    if ((e = cudaMalloc(&b.sort_tmp, b.sort_tmp_bytes)) != cudaSuccess) return e;
-    b.empty = true;
-    return cudaSuccess;
-}
-
-void map_free(MapBuffers& b) {
-    cudaFree(b.table); cudaFree(b.btable); cudaFree(b.arena); cudaFree(b.counters); cudaFreeHost(b.h_counters);
-    cudaFree(b.touched); cudaFree(b.dirty); cudaFree(b.stage_xyz); cudaFree(b.skeys); cudaFree(b.skeys_alt);
-    cudaFree(b.svals); cudaFree(b.svals_alt); cudaFree(b.sort_tmp);
-    memset(&b, 0, sizeof(b));
-}
-
 static VoxelMapRW map_rw(const MapBuffers& b) {
     VoxelMapRW m;
     m.table = b.table; m.mask = b.slots - 1u; m.btable = b.btable; m.bmask = b.bslots - 1u;
@@ -242,6 +215,140 @@ static VoxelMapRW map_rw(const MapBuffers& b) {
     m.list_cap = b.list_cap; m.grid = b.grid;
     return m;
 }
+
+static uint32_t pow2_at_least(uint64_t v, uint32_t lo, uint32_t hi) {
+    uint64_t p = lo;
+    while (p < v && p < hi) p <<= 1;
+    return (uint32_t)p;
+}
+
+MapSizes map_sizes(int64_t cap, int64_t max_points, bool scratch) {
+    MapSizes z;
+    /* occupied + dilated voxels of a surface-like map: ~1 slot per map point; 4x keeps the load below 0.3, scattered
+     * maps (27 slots per isolated point) run out and report LV_ERR_CAPACITY instead of hanging */
+    z.slots = pow2_at_least(4ull * (uint64_t)cap, 1u << 16, (uint32_t)kMaxSlots);
+    z.bslots = pow2_at_least((uint64_t)z.slots / 4u, 1u << 14, 1u << 27);
+    /* own extents (~1.5x the map) + halo buckets (27 copies of every point, up to 50 % slack) + the extents that
+     * buckets outgrow (geometric growth: at most twice the live ones): 1.5 KB per map point of capacity */
+    uint64_t arena = 96ull * (uint64_t)cap + (4ull << 20);
+    if (arena > kMaxArena) arena = kMaxArena;                                /* ids are int32 */
+    z.arena_cap = (uint32_t)arena;
+    z.add_cap = cap > max_points ? cap : max_points;
+    z.sort_tmp_bytes = 0;
+    if (scratch)
+        cub::DeviceRadixSort::SortPairs(nullptr, z.sort_tmp_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
+                                        (uint32_t*)nullptr, (int)z.add_cap, 0, 32);
+    return z;
+}
+const char* map_ceiling(int64_t cap) {
+    if (4ull * (uint64_t)cap > (uint64_t)kMaxSlots) return "voxel table ceiling (2^26 slots, 4 per point)";
+    if (96ull * (uint64_t)cap + (4ull << 20) > (uint64_t)kMaxArena) return "arena ceiling (0x7FFFFFF0 entries: point ids are int32)";
+    return nullptr;
+}
+int64_t map_bytes(const MapBuffers& b) {
+    return (int64_t)(sizeof(uint4) * (2 * (size_t)b.slots + (size_t)b.bslots) + sizeof(float4) * (size_t)b.arena_cap +
+                     sizeof(uint32_t) * (2 * (size_t)b.list_cap + 4 * (size_t)b.add_cap + kMapCounters) + sizeof(float) * 3 * (size_t)b.add_cap +
+                     b.sort_tmp_bytes);
+}
+
+/* every device buffer of the map comes from the stream-ordered allocator: a growth frees the old ones with cudaFreeAsync
+ * behind the kernels that read them, without synchronising the device */
+struct MapStore {
+    uint4 *table, *btable;
+    float4* arena;
+    uint32_t *touched, *dirty;
+    float* stage_xyz;
+    uint32_t *skeys, *skeys_alt, *svals, *svals_alt;
+    void* sort_tmp;
+};
+static void store_free(MapStore& s, cudaStream_t st) {
+    void* p[] = {s.table, s.btable, s.arena, s.touched, s.dirty, s.stage_xyz, s.skeys, s.skeys_alt, s.svals, s.svals_alt, s.sort_tmp};
+    for (void* q : p) if (q) cudaFreeAsync(q, st);
+    memset(&s, 0, sizeof(s));
+}
+static cudaError_t store_alloc(MapStore& s, const MapSizes& z, cudaStream_t st) {
+    memset(&s, 0, sizeof(s));
+    cudaError_t e;
+    if ((e = cudaMallocAsync((void**)&s.table, sizeof(uint4) * 2 * (size_t)z.slots, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.btable, sizeof(uint4) * (size_t)z.bslots, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.arena, sizeof(float4) * (size_t)z.arena_cap, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.touched, sizeof(uint32_t) * (size_t)z.slots, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.dirty, sizeof(uint32_t) * (size_t)z.slots, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.stage_xyz, sizeof(float) * 3 * (size_t)z.add_cap, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.skeys, sizeof(uint32_t) * (size_t)z.add_cap, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.skeys_alt, sizeof(uint32_t) * (size_t)z.add_cap, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.svals, sizeof(uint32_t) * (size_t)z.add_cap, st)) == cudaSuccess &&
+        (e = cudaMallocAsync((void**)&s.svals_alt, sizeof(uint32_t) * (size_t)z.add_cap, st)) == cudaSuccess &&
+        (e = cudaMallocAsync(&s.sort_tmp, z.sort_tmp_bytes, st)) == cudaSuccess)
+        return cudaSuccess;
+    store_free(s, st);
+    cudaGetLastError();                       /* an allocation failure is not sticky: the old map stays usable */
+    return e;
+}
+static MapStore store_of(const MapBuffers& b) {
+    MapStore s = {b.table, b.btable, b.arena, b.touched, b.dirty, b.stage_xyz, b.skeys, b.skeys_alt, b.svals, b.svals_alt, b.sort_tmp};
+    return s;
+}
+static void store_adopt(MapBuffers& b, const MapStore& s, const MapSizes& z, int64_t cap) {
+    b.table = s.table; b.btable = s.btable; b.arena = s.arena; b.touched = s.touched; b.dirty = s.dirty; b.stage_xyz = s.stage_xyz;
+    b.skeys = s.skeys; b.skeys_alt = s.skeys_alt; b.svals = s.svals; b.svals_alt = s.svals_alt; b.sort_tmp = s.sort_tmp;
+    b.cap = cap;
+    b.slots = z.slots; b.bslots = z.bslots; b.arena_cap = z.arena_cap; b.list_cap = z.slots;
+    b.add_cap = z.add_cap; b.sort_tmp_bytes = z.sort_tmp_bytes;
+    b.sort_bits = kCellBits;
+    for (uint32_t s2 = b.slots; s2 > 1; s2 >>= 1) b.sort_bits++;
+}
+
+cudaError_t map_alloc(MapBuffers& b, int64_t max_map_points, int64_t max_points, float voxel_size, float ds, cudaStream_t st) {
+    memset(&b, 0, sizeof(b));
+    b.grid.ds = ds;
+    int k = (int)floor((double)voxel_size / (double)ds + 0.5);
+    k = k < 1 ? 1 : (k > kMaxCellsPerVoxel ? kMaxCellsPerVoxel : k);
+    b.grid.k = k;
+    b.grid.cell0 = (float)k * ds;
+    b.max_points = max_points;
+    b.stream = st;
+    const MapSizes z = map_sizes(max_map_points, max_points);
+    MapStore s;
+    cudaError_t e;
+    if ((e = store_alloc(s, z, st)) != cudaSuccess) return e;
+    store_adopt(b, s, z, max_map_points);
+    if ((e = cudaMalloc(&b.counters, sizeof(uint32_t) * kMapCounters)) != cudaSuccess) return e;
+    if ((e = cudaMallocHost(&b.h_counters, sizeof(uint32_t) * kMapCounters)) != cudaSuccess) return e;
+    b.empty = true;
+    return cudaSuccess;
+}
+
+void map_free(MapBuffers& b) {
+    MapStore s = store_of(b);
+    store_free(s, b.stream);
+    if (b.stream) cudaStreamSynchronize(b.stream);
+    cudaFree(b.counters); cudaFreeHost(b.h_counters);
+    memset(&b, 0, sizeof(b));
+}
+
+/* re-hash both tables into tables sized for `cap` points, copy the arena's used prefix into a larger arena, grow the
+ * lists and the add scratch; frees the old buffers behind the kernels.  Stream-ordered, no synchronisation.  On an
+ * allocation failure nothing has changed. */
+cudaError_t map_grow(MapBuffers& b, int64_t cap, cudaStream_t st, int* launches) {
+    if (cap <= b.cap) return cudaSuccess;
+    const MapSizes z = map_sizes(cap, b.max_points);
+    MapStore s;
+    cudaError_t e = store_alloc(s, z, st);
+    if (e != cudaSuccess) return e;
+    MapStore old = store_of(b);
+    const uint32_t old_slots = b.slots, old_bslots = b.bslots, old_arena_cap = b.arena_cap;
+    lv_map_grow_init_kernel<<<kNumSMs * 8, 256, 0, st>>>(s.table, z.slots, s.btable, z.bslots, b.counters);
+    store_adopt(b, s, z, cap);
+    const VoxelMapRW m = map_rw(b);
+    lv_map_rehash_kernel<<<kNumSMs * 8, 256, 0, st>>>(m, old.table, old_slots, old.btable, old_bslots);
+    lv_map_arena_copy_kernel<<<kNumSMs * 8, 256, 0, st>>>(old.arena, s.arena, old_arena_cap, b.counters);
+    e = cudaGetLastError();
+    store_free(old, st);
+    if (launches) *launches += 3;
+    return e;
+}
+
 VoxelMapView map_view(const MapBuffers& b) { return map_view_of(map_rw(b)); }
 
 cudaError_t map_clear(MapBuffers& b, cudaStream_t st, int* launches) {

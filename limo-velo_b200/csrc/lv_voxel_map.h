@@ -260,6 +260,49 @@ LV_HD void block_mark(const VoxelMapRW& m, uint32_t bx, uint32_t by, uint32_t bz
     }
     atomic_or_u32(m.counters + kCtrError, (uint32_t)kErrBlockTableFull);
 }
+/* ---- growth: the tables re-hashed into larger ones (lv_map.cu map_grow, lv_map_reserve / lv_map_set_growth) ------------
+ * The arena keeps its indices (its used prefix is copied as it is), so a slot's 32 bytes stay valid word for word: key,
+ * own and halo extents, caps and flags.  Only where a key lives changes.  The new table starts empty and holds at most
+ * half as many keys per slot as the old one; a key that finds no free slot within kMaxProbes (as voxel_insert) sets the
+ * table-full flag, so a lookup never has to probe further than it does today. */
+/* old voxel slot `slot` -> m (same hash and linear probing as voxel_insert); counts kCtrSlotsUsed */
+LV_HD void voxel_rehash_item(const VoxelMapRW& m, const uint4* old_table, uint32_t slot) {
+    const uint4 e0 = old_table[2 * (size_t)slot], e1 = old_table[2 * (size_t)slot + 1];
+    if ((e0.x & e0.y) == 0xFFFFFFFFu) return;
+    const uint64_t key = (uint64_t)e0.x | ((uint64_t)e0.y << 32);
+    unsigned long long* tab64 = reinterpret_cast<unsigned long long*>(m.table);
+    uint32_t s = voxel_hash(key) & m.mask;
+    for (int probes = 0; probes < kMaxProbes; ++probes) {
+        if (atomic_cas_u64(tab64 + 4 * (size_t)s, LV_EMPTY_KEY, (unsigned long long)key) == LV_EMPTY_KEY) {
+            uint32_t* d32 = reinterpret_cast<uint32_t*>(m.table + 2 * (size_t)s);
+            d32[2] = e0.z; d32[3] = e0.w;
+            m.table[2 * (size_t)s + 1] = e1;
+            atomic_add_u32(m.counters + kCtrSlotsUsed, 1u);
+            return;
+        }
+        s = (s + 1) & m.mask;
+    }
+    atomic_or_u32(m.counters + kCtrError, (uint32_t)kErrTableFull);
+}
+/* old block slot `slot` -> m (block_mark's hash and probing, occupancy mask OR-ed in); counts kCtrBlocksUsed */
+LV_HD void block_rehash_item(const VoxelMapRW& m, const uint4* old_btable, uint32_t slot) {
+    const uint4 e = old_btable[slot];
+    if ((e.x & e.y) == 0xFFFFFFFFu) return;
+    const uint64_t key = (uint64_t)e.x | ((uint64_t)e.y << 32);
+    unsigned long long* tab64 = reinterpret_cast<unsigned long long*>(m.btable);
+    uint32_t s = (voxel_hash(key) * 0x9E3779B1u) & m.bmask;
+    for (int probes = 0; probes < kMaxProbes; ++probes) {
+        const unsigned long long prev = atomic_cas_u64(tab64 + 2 * (size_t)s, LV_EMPTY_KEY, (unsigned long long)key);
+        if (prev == LV_EMPTY_KEY || prev == (unsigned long long)key) {
+            if (prev == LV_EMPTY_KEY) atomic_add_u32(m.counters + kCtrBlocksUsed, 1u);
+            atomic_or_u64(tab64 + 2 * (size_t)s + 1, (unsigned long long)e.z | ((unsigned long long)e.w << 32));
+            return;
+        }
+        s = (s + 1) & m.bmask;
+    }
+    atomic_or_u32(m.counters + kCtrError, (uint32_t)kErrBlockTableFull);
+}
+
 /* bump allocation of `cap` float4 from the arena; 0xFFFFFFFF when exhausted (sets kErrArenaFull) */
 LV_HD uint32_t arena_alloc(const VoxelMapRW& m, uint32_t cap) {
     const uint32_t at = atomic_add_u32(m.counters + kCtrArenaTop, cap);

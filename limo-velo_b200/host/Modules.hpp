@@ -84,6 +84,10 @@ class Mapper {
         check(lv_map_add_last_sweep(ctx.h, downsample ? 1 : 0), "Mapper::add_corrected_sweep");
         last_map_time = time;
     }
+    /* the ikd-Tree has no capacity (ikd_Tree.cpp:478-573): grow the device map now to hold `points`, or let it grow by itself
+     * before the adds that may not fit, up to `max_points` (0: off) — lv_map_reserve / lv_map_set_growth */
+    void reserve(int64_t points) { check(lv_map_reserve(ctx.h, points), "Mapper::reserve"); }
+    void set_growth(int64_t max_points) { check(lv_map_set_growth(ctx.h, max_points), "Mapper::set_growth"); }
 
    private:
     Context& ctx;
