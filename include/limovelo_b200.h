@@ -311,7 +311,8 @@ lv_status lv_temporal_downsample(lv_handle h, const float* xyz, int64_t n, int32
  * this (n_out = n, LV_OK, the warning in lv_last_error()).                                                          */
 lv_status lv_voxelgrid_downsample(lv_handle h, const float* xyz, int64_t n, float downsample_prec, float* xyz_out,
                                   int64_t* n_out);
-/* the same on device-resident buffers (d_xyz_out must not alias d_xyz)                                    */
+/* the same on device-resident buffers; LV_ERR_ARG (and a message in lv_last_error()) when the n-point ranges at
+ * d_xyz and d_xyz_out overlap                                                                              */
 lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_t n, float downsample_prec,
                                          float* d_xyz_out, int64_t* n_out);
 

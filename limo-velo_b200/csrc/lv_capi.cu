@@ -1130,6 +1130,13 @@ static lv_status ds_stage(lv_context* h, int64_t n) {
     return LV_OK;
 }
 lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_t n, float leaf, float* d_xyz_out, int64_t* n_out) {
+    /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids: an output
+     * range that overlaps the input would be read after it is overwritten */
+    if (d_xyz && d_xyz_out && n > 0 && n <= 0x7fffffff && (uintptr_t)d_xyz_out < (uintptr_t)(d_xyz + 3 * n) &&
+        (uintptr_t)d_xyz < (uintptr_t)(d_xyz_out + 3 * n)) {
+        set_error("voxel grid: the output range overlaps the input range");
+        return LV_ERR_ARG;
+    }
     if (!h || !d_xyz || !d_xyz_out || !n_out || n < 0 || !(leaf > 0.f) || n > 0x7fffffff) return LV_ERR_ARG;
     *n_out = 0;
     if (n == 0) return LV_OK;
@@ -1143,7 +1150,7 @@ lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_
         /* pcl::VoxelGrid::applyFilter warns "Leaf size is too small for the input dataset. Integer indices would overflow."
          * and hands the input on unchanged; Compensator::voxelgrid_downsample carries on with it.  Same here. */
         set_error("voxel grid: leaf size too small for the extent of the cloud (cell index overflows): input passed through");
-        if (d_xyz_out != d_xyz) LV_CUDA(cudaMemcpyAsync(d_xyz_out, d_xyz, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToDevice, h->stream));
+        LV_CUDA(cudaMemcpyAsync(d_xyz_out, d_xyz, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToDevice, h->stream));
         LV_CUDA(cudaStreamSynchronize(h->stream));
         *n_out = n;
         return LV_OK;

@@ -7,7 +7,7 @@
  *
  * fp32 arithmetic is unfused (lv_hd.h) and 3-term products are summed like the rest of the fp32 geometry
  * (lv_point_math.h); sinf / cosf are the platform's (CUDA's differ from glibc's in the last ulp, which is why
- * this stage is held to a tolerance, not to bit-exactness: tests/test_gpu_deskew.py).
+ * this stage is held to a tolerance, not to bit-exactness: tests/test_gpu_frontend.py).
  */
 #ifndef LV_DESKEW_H_
 #define LV_DESKEW_H_

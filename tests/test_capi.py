@@ -71,6 +71,10 @@ def test_argument_errors(lv):
     assert L.lv_compensate_device(None, None, 0, None, None, None, C.c_int64(0), None) == lv.ERR_ARG
     assert L.lv_voxelgrid_downsample(None, None, C.c_int64(0), C.c_float(0.5), None, C.byref(n_out)) == lv.ERR_ARG
     assert L.lv_temporal_downsample(None, None, C.c_int64(0), 4, C.c_double(4.0), None, None, C.byref(n_out)) == lv.ERR_ARG
+    # the device voxel grid refuses an output range that overlaps its input (checked before anything touches the device)
+    base = 1 << 40
+    assert L.lv_voxelgrid_downsample_device(None, C.c_void_p(base), C.c_int64(10), C.c_float(0.5), C.c_void_p(base + 12 * 9),
+                                            C.byref(n_out)) == lv.ERR_ARG and b"overlaps" in L.lv_last_error()
     assert L.lv_pointcloud2_to_points(0, None, None, C.c_int64(0), C.c_uint64(0), 0, 1, C.c_double(0.1), None, None, None, None) == lv.ERR_ARG
     lay = lv.CloudLayout(16, 0, 4, 8, 12, 12, 0)
     buf = (C.c_uint8 * 16)()
