@@ -79,8 +79,7 @@ typedef struct lv_params {
     float voxel_size;                 /* edge of the hashed search voxels [m], default 0.4; rounded to a whole number
                                        * (1..3) of map_downsample_size cells: a voxel is k x k x k downsample cells */
     int32_t device;                   /* CUDA device ordinal                               */
-    int32_t sort_queries;             /* 1: bin the sweep by home voxel once per update and search from shared memory
-                                       * (lv_search_staged_kernel); 0: per-query search from global memory       */
+    int32_t pad1_;                    /* reserved (keeps the layout of earlier releases), ignored */
     int64_t max_map_points;           /* capacity of the device map                        */
     int64_t max_points;               /* capacity of one sweep                             */
     void* stream;                     /* cudaStream_t to run on; NULL = own stream         */

@@ -34,7 +34,7 @@ class Params(C.Structure):
         ("covariance_bias_gyroscope", C.c_double), ("covariance_bias_acceleration", C.c_double),
         ("initial_gravity", C.c_float * 3), ("I_Translation_L", C.c_float * 3), ("I_Rotation_L", C.c_float * 9),
         ("map_downsample_size", C.c_float), ("voxel_size", C.c_float), ("device", C.c_int32),
-        ("sort_queries", C.c_int32), ("max_map_points", C.c_int64), ("max_points", C.c_int64),
+        ("pad1_", C.c_int32), ("max_map_points", C.c_int64), ("max_points", C.c_int64),
         ("stream", C.c_void_p),
     ]
 

@@ -60,10 +60,6 @@ struct lv_context {
     uint32_t* d_hard_list = nullptr;   /* kHardBuckets segments of hard_segment(max_points) entries, then kCounters counters */
     float4* d_ref = nullptr;           /* max_points: reuse reference (lv_reuse_kernel) */
     uint32_t* d_redo = nullptr;        /* max_points */
-    uint32_t *d_bin_key = nullptr, *d_bin_val = nullptr, *d_bin_key_in = nullptr, *d_bin_val_in = nullptr;   /* sort_queries */
-    uint8_t* d_redo_flag = nullptr;
-    void* d_bin_tmp = nullptr;
-    size_t bin_tmp_bytes = 0;
     double* d_imu = nullptr;           /* kImuBatch x 7: lv_propagate_device */
     double* h_imu = nullptr;           /* pinned */
     /* recorded after the last H2D copy out of h_imu / h_ctrl: the calls return before those copies run (they queue behind
@@ -212,13 +208,6 @@ static MeasureArgs make_measure_args(lv_context* h, const float* d_xyz, int64_t 
     a.hard_list = h->d_hard_list;
     a.hard_seg = hard_segment(h->prm.max_points);
     a.hard_count = h->d_hard_list + (size_t)kHardBuckets * a.hard_seg;
-    if (h->prm.sort_queries) {
-        a.bin_key = h->d_bin_key; a.bin_val = h->d_bin_val; a.bin_key_in = h->d_bin_key_in; a.bin_val_in = h->d_bin_val_in;
-        a.redo_flag = h->d_redo_flag;
-        a.sort_tmp = h->d_bin_tmp; a.sort_tmp_bytes = h->bin_tmp_bytes;
-        a.sort_bits = 0;
-        for (uint32_t sl = h->map.slots; sl > 1; sl >>= 1) a.sort_bits++;
-    }
     return a;
 }
 
@@ -295,16 +284,6 @@ lv_status lv_create(const lv_params* p, lv_handle* out) {
     LV_CREATE_CUDA(cudaMemset(h->d_nn_b, 0xFF, sizeof(int2) * p->max_points));
     LV_CREATE_CUDA(cudaMemset(h->d_ref, 0, sizeof(float4) * p->max_points));
     LV_CREATE_CUDA(cudaMemset(h->d_hard_list, 0, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
-    if (p->sort_queries) {
-        LV_CREATE_CUDA(cudaMalloc(&h->d_bin_key, sizeof(uint32_t) * p->max_points));
-        LV_CREATE_CUDA(cudaMalloc(&h->d_bin_val, sizeof(uint32_t) * p->max_points));
-        LV_CREATE_CUDA(cudaMalloc(&h->d_bin_key_in, sizeof(uint32_t) * p->max_points));
-        LV_CREATE_CUDA(cudaMalloc(&h->d_bin_val_in, sizeof(uint32_t) * p->max_points));
-        LV_CREATE_CUDA(cudaMalloc(&h->d_redo_flag, p->max_points));
-        LV_CREATE_CUDA(cudaMemset(h->d_redo_flag, 1, p->max_points));
-        h->bin_tmp_bytes = bin_sort_tmp_bytes(p->max_points);
-        LV_CREATE_CUDA(cudaMalloc(&h->d_bin_tmp, h->bin_tmp_bytes));
-    }
     h->use_reuse = getenv("LV_NO_REUSE") == nullptr;
     h->use_pdl = getenv("LV_NO_PDL") == nullptr;
     LV_CREATE_CUDA(cudaMalloc(&h->d_job, sizeof(MeasureJob)));
@@ -345,7 +324,6 @@ void lv_destroy(lv_handle h) {
     for (cudaEvent_t e : h->snap_ev) if (e) cudaEventDestroy(e);
     cudaFreeHost(h->h_snap);
     cudaFree(h->d_job); cudaFree(h->d_ref); cudaFree(h->d_redo); cudaFree(h->d_imu); cudaFreeHost(h->h_imu);
-    cudaFree(h->d_bin_key); cudaFree(h->d_bin_val); cudaFree(h->d_bin_key_in); cudaFree(h->d_bin_val_in); cudaFree(h->d_redo_flag); cudaFree(h->d_bin_tmp);
     cudaFree(h->d_path); cudaFreeHost(h->h_path); cudaFree(h->d_times); cudaFree(h->d_deskew_in); cudaFree(h->d_bad); cudaFreeHost(h->h_bad);
     ds_free(h->ds); cudaFree(h->d_ds_in); cudaFree(h->d_ds_out);
     map_free(h->map);
@@ -375,7 +353,7 @@ static void count_map_launches(lv_context* h, int launches) { h->prof.total_laun
 enum : int64_t { kMaxCapPoints = (int64_t)kMaxSlots / 4 };   /* the largest capacity under both ceilings */
 
 static void drop_update_graphs(lv_context* h) {
-    /* the update graphs bake the map view (table, masks, arena) and the bin sort width into their kernel arguments; a graph
+    /* the update graphs bake the map view (table, masks, arena) into their kernel arguments; a graph
      * still in flight is freed when it completes */
     for (auto& u : h->graphs) { cudaGraphExecDestroy(u.exec); cudaGraphDestroy(u.graph); }
     h->graphs.clear();
@@ -840,7 +818,7 @@ static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n) {
     kp.kernelParams = args;
     LV_CUDA(cudaGraphExecKernelNodeSetParams(g->exec, g->begin_node, &kp));
     LV_CUDA(cudaGraphLaunch(g->exec, h->stream));
-    h->prof.total_launches += 1 + 4 * (h->prm.MAX_NUM_ITERS + 1) + (h->use_reuse ? h->prm.MAX_NUM_ITERS : 0) + (h->prm.sort_queries ? 5 : 0);
+    h->prof.total_launches += 1 + 4 * (h->prm.MAX_NUM_ITERS + 1) + (h->use_reuse ? h->prm.MAX_NUM_ITERS : 0);
     return LV_OK;
 }
 
@@ -851,11 +829,6 @@ static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64
     if (!as_job) h->prof.total_launches += 1;
     MeasureArgs a = update_measure_args(h, d_xyz, n, as_job);
     const int grid = measure_grid((int)n);
-    if (a.bin_key) {                                              /* once per update: the sweep binned by home voxel */
-        int l = 0;
-        LV_CUDA(launch_bin(a, h->stream, pdl, &l));
-        if (!as_job) h->prof.total_launches += l;
-    }
     for (int e = 0; e <= h->prm.MAX_NUM_ITERS; ++e) {            /* i = -1 .. max_iter-1, esekfom.hpp:1634 */
         EventPair ep;
         bool pr;
@@ -951,7 +924,6 @@ static lv_status run_measure_once(lv_context* h, const double* x, const float* x
         a.g_world = h->d_gworld;
     }
     const int grid = measure_grid((int)n);
-    if (a.bin_key) { int l = 0; LV_CUDA(launch_bin(a, h->stream, 0, &l)); h->prof.total_launches += l; }
     LV_CUDA(launch_measure_timed(h, a, grid, 1, 0, -1, 0));
     LV_CUDA(launch_reduce_partials(h->d_group_rows, partial_groups(grid), h->d_reduced, h->stream));
     LV_CUDA(cudaMemcpyAsync(h->h_reduced, h->d_reduced, sizeof(double) * 157, cudaMemcpyDeviceToHost, h->stream));

@@ -64,15 +64,6 @@ struct MeasureArgs {
     /* reuse of neighbours across the evaluations of one update (NULL: off) */
     float4* ref;               /* n: world position the stored neighbours were searched from + outsider bound */
     uint32_t* redo_list;       /* n: queries whose neighbours could not be reused (Kv -> K1)  */
-    /* binned order of the sweep (lv_params.sort_queries; NULL: per-query search from global memory) */
-    const uint32_t* bin_key;   /* n: home-voxel slot at the propagated state, ascending (0xFFFFFFFF: none) */
-    const uint32_t* bin_val;   /* n: the query at that position                                            */
-    uint32_t* bin_key_in;      /* n: unsorted, written by lv_bin_kernel                                    */
-    uint32_t* bin_val_in;
-    uint8_t* redo_flag;        /* n: 1 = search again (written by lv_reuse_kernel)                         */
-    void* sort_tmp;            /* cub::DeviceRadixSort scratch for n pairs                                 */
-    size_t sort_tmp_bytes;
-    int32_t sort_bits;         /* significant bits of a slot index                                         */
 };
 
 /* device map storage (layout: lv_voxel_map.h) + scratch of one add */
@@ -138,9 +129,6 @@ struct MeasureProbe { void (*at)(void* ctx, int stage); void* ctx; };
  * the shape of the level-0 search kernel (search_group() in lv_measure.cu). */
 cudaError_t launch_measure(const MeasureArgs& a, int grid, cudaStream_t st, const MeasureProbe* probe = nullptr,
                            int reuse = 0, int pdl = 0);
-/* once per update when a.bin_key is set: lv_bin_kernel + radix sort of the (slot, query) pairs */
-cudaError_t launch_bin(const MeasureArgs& a, cudaStream_t st, int pdl, int* launches);
-size_t bin_sort_tmp_bytes(int64_t max_points);
 cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n, uint32_t* counters, cudaStream_t st);
 const void* ieskf_begin_kernel_ptr();
 void measure_init();                          /* constant tables; call once before any capture           */

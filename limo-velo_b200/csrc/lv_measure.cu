@@ -12,7 +12,7 @@
  * and the 23x23 algebra between two evaluations (esekfom.hpp:1647-1817, csrc/lv_ieskf.h).
  *
  * Kernels of one evaluation (DESIGN.md 4): lv_reuse_kernel (evaluations after the first: keep the neighbours the
- * exact search provably returns again), lv_search_kernel (exact 5-NN at level 0, thin, 8 lanes per query),
+ * exact search provably returns again), lv_search_kernel (exact 5-NN at level 0, thin, 4 or 8 lanes per query),
  * lv_search_rings_kernel (the queries level 0 cannot certify, one warp each), lv_fit_kernel (plane fit, Jacobian
  * row, the 78 + 12 unique normal-equation sums per block in a fixed order; one spare block runs ieskf_prepare),
  * lv_ieskf_step_kernel (one block: reduction of the partials, gain, dx, next frame, loop control).  H (Nm x 12
@@ -43,8 +43,6 @@ __device__ long long g_step_clk[64];
 #ifndef LV_FK
 #define LV_FK(k)
 #endif
-
-#include <cub/device/device_radix_sort.cuh>
 
 #include "lv_internal.h"
 #include "lv_predict.h"
@@ -108,7 +106,6 @@ __device__ __forceinline__ JobView job_view(const MeasureArgs& a) {
 
 #define LV_ROW_STRIDE (kMeasureThreads + 4)   /* 132 doubles = 4 (mod 16): the 8 x 4 fragment loads of the fold below are conflict-free */
 #define LV_SEARCH_THREADS 128
-#define LV_GROUP 8                              /* lanes per query in K1 (LV_SEARCH_GROUP=1|8 overrides) */
 
 __device__ __forceinline__ void store_neighbours(const MeasureArgs& a, int qi, const Top5& t) {
     a.nn_a[qi] = make_int4(t.i0, t.i1, t.i2, t.i3);                  /* positions in the arena, -1 = none */
@@ -179,275 +176,6 @@ __global__ void __launch_bounds__(LV_SEARCH_THREADS) lv_search_kernel(const Meas
 }
 
 /*
- * K1c — search, level 0, query-per-lane prologue + 8-lane scans (LV_SEARCH_GROUP=32).  In K1 every instruction of a query's
- * prologue (world transform, three IEEE divisions for the voxel coordinate, hash, probe, face distances) is issued for a warp
- * that holds only FOUR queries, a large share of K1's instructions.  Here a warp holds 32 queries: each lane does the
- * prologue of its own query (32 probes in flight per warp), then the warp walks its queries four at a time — the owner
- * lanes hand (point, bucket, certified radius) to the 8-lane groups by shuffle, which scan and merge exactly as K1 does.
- * Same candidates, same merge, same answers; an eighth of the prologue instructions.
- */
-#define LV_COOP_THREADS 64
-template <bool LIST>
-__global__ void __launch_bounds__(LV_COOP_THREADS) lv_search_coop_kernel(const MeasureArgs a) {
-    typedef GroupLanes<8> Grp;
-    LV_TL_SCHED();
-    pdl_wait();
-    pdl_trigger();
-    LV_TL_WORK(a.ctrl, 2);
-    const int done = a.ctrl->done;
-    const Rt32 T = a.ctrl->frame.lidar_to_world;
-    const JobView jb = job_view(a);
-    const int n_redo = LIST ? (int)a.hard_count[2] : 0;
-    const int slot = (int)(blockIdx.x * LV_COOP_THREADS + threadIdx.x);
-    const int listed = LIST ? (int)a.redo_list[slot < (int)a.n ? slot : 0] : 0;
-    if (done) return;
-    if (LIST && (int)(blockIdx.x * LV_COOP_THREADS) >= n_redo) return;
-    const bool have = LIST ? slot < n_redo : slot < jb.n;
-    const int qi = have ? (LIST ? listed : slot) : 0;
-    /* 1. one query per lane */
-    float g[3] = {0.f, 0.f, 0.f}, cert = 0.f;
-    uint32_t bs = 0, bc = 0, vox[3] = {0u, 0u, 0u};
-    int st = 0;                       /* 0 no query / not finite, 1 bucket, 2 no level-0 slot */
-    if (have) {
-        rt_apply(T, jb.xyz[3 * qi], jb.xyz[3 * qi + 1], jb.xyz[3 * qi + 2], g);   /* Mapper.cpp:51 */
-        const bool finite = (fabsf(g[0]) < 1e9f) && (fabsf(g[1]) < 1e9f) && (fabsf(g[2]) < 1e9f);
-        if (finite) st = level0_probe(a.map, g[0], g[1], g[2], &bs, &bc, vox) >= 0 ? 1 : 2;
-        if (st == 1) cert = certified_d2(home_geom(a.map.grid, vox[0], vox[1], vox[2], g[0], g[1], g[2]));
-    }
-    /* 2. four queries at a time, 8 lanes each */
-    const int lane = (int)(threadIdx.x & 31u);
-#pragma unroll 1
-    for (int r = 0; r < 8; ++r) {
-        const int src = 4 * r + (lane >> 3);
-        const int st_r = __shfl_sync(0xffffffffu, st, src);
-        const bool have_r = __shfl_sync(0xffffffffu, have ? 1 : 0, src) != 0;
-        if (!__ballot_sync(0xffffffffu, have_r)) break;           /* slots ascend with the lane: nothing further either */
-        const float gx = __shfl_sync(0xffffffffu, g[0], src), gy = __shfl_sync(0xffffffffu, g[1], src), gz = __shfl_sync(0xffffffffu, g[2], src);
-        const uint32_t bs_r = __shfl_sync(0xffffffffu, bs, src), bc_r = __shfl_sync(0xffffffffu, bc, src);
-        const float cert_r = __shfl_sync(0xffffffffu, cert, src);
-        const int qi_r = __shfl_sync(0xffffffffu, qi, src);
-        Top5 t;
-        float region = 0.f;
-        const bool settled = level0_scan<Grp>(a.map, gx, gy, gz, a.max_d2, bs_r, bc_r, st_r == 1, t, &region, nullptr, &cert_r);
-        if (have_r && (lane & 7) == 0) {
-            store_neighbours(a, qi_r, t);
-            const bool hard = st_r == 2 || (st_r == 1 && !settled);
-            const float gq[3] = {gx, gy, gz};
-            store_ref(a, qi_r, gq, (st_r == 1 && settled) ? outsider_bound(t.d5, region) : 0.f);
-            if (hard) {
-                const uint32_t b = blockIdx.x % kHardBuckets;
-                a.hard_list[(size_t)b * a.hard_seg + atomicAdd(a.hard_count + 4 + b, 1u)] = (uint32_t)qi_r;
-            }
-        }
-    }
-    LV_TL_END(2);
-}
-
-/* ---- bulk copies into shared memory (TMA engine, 1-D form) and the mbarrier they complete on ---------------- */
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                 : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
-}
-/* global -> shared, `bytes` a multiple of 16, both addresses 16-byte aligned; completes `bytes` of transaction on `bar` */
-__device__ __forceinline__ void bulk_copy_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-/*
- * Kb — bin.  Once per update (the sweep does not change across its evaluations): the home voxel's slot of every
- * query at the propagated state.  A radix sort of the (slot, query) pairs follows (launch_bin), after which the
- * queries of one voxel sit next to each other and lv_search_staged_kernel fetches each halo bucket once per block.
- */
-__global__ void __launch_bounds__(128) lv_bin_kernel(const MeasureArgs a) {
-    pdl_wait();
-    pdl_trigger();
-    if (a.ctrl->done) return;
-    const JobView jb = job_view(a);
-    const int i = (int)(blockIdx.x * blockDim.x + threadIdx.x);
-    if (i >= a.n) return;
-    if (i >= jb.n) {            /* graph replay: the sort covers the capacity a.n; the padding sorts behind every query */
-        a.bin_key_in[i] = 0xFFFFFFFFu;
-        a.bin_val_in[i] = 0xFFFFFFFFu;
-        return;
-    }
-    const Rt32& T = a.ctrl->frame.lidar_to_world;
-    float g[3];
-    rt_apply(T, jb.xyz[3 * i], jb.xyz[3 * i + 1], jb.xyz[3 * i + 2], g);
-    uint32_t key = 0xFFFFFFFFu, bs, bc;
-    const bool finite = (fabsf(g[0]) < 1e9f) && (fabsf(g[1]) < 1e9f) && (fabsf(g[2]) < 1e9f);
-    if (finite) {
-        const int slot = level0_probe(a.map, g[0], g[1], g[2], &bs, &bc);
-        if (slot >= 0) key = (uint32_t)slot;
-    }
-    a.bin_key_in[i] = key;
-    a.bin_val_in[i] = (uint32_t)i;
-}
-
-/*
- * K1s — search, level 0, from shared memory.  One block = LV_STAGE_QUERIES consecutive queries of the binned order,
- * i.e. a handful of voxel runs.  Per block: the run heads read their voxel's slot (one 32-byte sector: key, bucket
- * start and count), a block scan places the buckets in shared memory, each head issues ONE bulk copy
- * (cp.async.bulk, completing on an mbarrier) for its bucket, and after the wait every thread scans its query's
- * bucket out of shared memory: no per-lane merge, no shuffles, one global fetch per bucket instead of one per query
- * (a 65 536-point Velodyne sweep has ~6 queries per home voxel).  Buckets beyond the staging budget are scanned from
- * global memory by the same loop.
- *   Certification is relative to the voxel the query was BINNED in (at the propagated state): the bucket holds every
- * map point of that voxel's 3x3x3 neighbourhood, so whatever lies closer to the query than the neighbourhood's
- * boundary is exact — also when a later iterate has moved the query into a neighbouring voxel.  What cannot be
- * certified goes to lv_search_rings_kernel, as in the per-query kernel.  Results are identical to lv_search_kernel's.
- *   With REDO (evaluations after the first, reuse on) the queries lv_reuse_kernel vouched for are skipped.
- */
-#define LV_STAGE_QUERIES 128
-#define LV_STAGE_PTS 2560                      /* float4 of staged buckets per block: 40 KB */
-/* one thread scans a whole bucket: p[0 .. n) are the points, ids are bstart + j */
-__device__ __forceinline__ void scan_bucket(const float4* p, uint32_t n, uint32_t bstart, const float* g, Top5& t) {
-    uint32_t j = 0;
-    for (; j + 4 <= n; j += 4) {
-        const float4 q0 = p[j], q1 = p[j + 1], q2 = p[j + 2], q3 = p[j + 3];
-        top5_insert(t, sq_dist(g[0], g[1], g[2], q0.x, q0.y, q0.z), (int)(bstart + j));
-        top5_insert(t, sq_dist(g[0], g[1], g[2], q1.x, q1.y, q1.z), (int)(bstart + j + 1));
-        top5_insert(t, sq_dist(g[0], g[1], g[2], q2.x, q2.y, q2.z), (int)(bstart + j + 2));
-        top5_insert(t, sq_dist(g[0], g[1], g[2], q3.x, q3.y, q3.z), (int)(bstart + j + 3));
-    }
-    for (; j < n; ++j) {
-        const float4 q = p[j];
-        top5_insert(t, sq_dist(g[0], g[1], g[2], q.x, q.y, q.z), (int)(bstart + j));
-    }
-}
-__device__ __noinline__ void scan_bucket_global(const float4* p, uint32_t n, uint32_t bstart, const float* g, Top5& t) {
-    for (uint32_t j = 0; j < n; ++j) {
-        const float4 q = load_point(p + j);
-        top5_insert(t, sq_dist(g[0], g[1], g[2], q.x, q.y, q.z), (int)(bstart + j));
-    }
-}
-template <bool REDO>
-__global__ void __launch_bounds__(LV_STAGE_QUERIES) lv_search_staged_kernel(const MeasureArgs a) {
-    __shared__ __align__(16) float4 s_pts[LV_STAGE_PTS];
-    __shared__ __align__(8) uint64_t s_bar;
-    __shared__ uint32_t s_key[LV_STAGE_QUERIES];
-    __shared__ uint32_t s_run_start[LV_STAGE_QUERIES];    /* bucket position in the arena                         */
-    __shared__ uint32_t s_run_count[LV_STAGE_QUERIES];
-    __shared__ uint32_t s_run_off[LV_STAGE_QUERIES];      /* position in s_pts, 0xFFFFFFFF: read from the arena   */
-    __shared__ uint32_t s_run_vox[LV_STAGE_QUERIES][3];   /* biased voxel coordinates of the run's voxel          */
-    __shared__ uint32_t s_run_need[LV_STAGE_QUERIES];
-    __shared__ uint32_t s_warp_heads[LV_STAGE_QUERIES / 32], s_warp_pts[LV_STAGE_QUERIES / 32];
-    LV_TL_SCHED();
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) mbar_init(&s_bar, 1);
-    s_run_need[tid] = 0u;
-    pdl_wait();                 /* frame (step kernel), binned order (sort), redo flags (reuse kernel) */
-    pdl_trigger();
-    LV_TL_WORK(a.ctrl, 2);
-    const int done = a.ctrl->done;
-    const Rt32 T = a.ctrl->frame.lidar_to_world;
-    const JobView jb = job_view(a);
-    if (done || (int)blockIdx.x * LV_STAGE_QUERIES >= jb.n) return;
-    const int pos = (int)blockIdx.x * LV_STAGE_QUERIES + tid;
-    const bool have = pos < jb.n;
-    const uint32_t key = have ? a.bin_key[pos] : 0xFFFFFFFFu;
-    const int qi = have ? (int)a.bin_val[pos] : 0;
-    bool active = have;
-    if (REDO && have) active = a.redo_flag[qi] != 0;
-    s_key[tid] = key;
-    __syncthreads();
-    /* runs of equal keys inside the block */
-    const bool binned = key != 0xFFFFFFFFu;
-    const bool head = binned && (tid == 0 || s_key[tid - 1] != key);
-    const unsigned hb = __ballot_sync(0xffffffffu, head);
-    if (lane == 0) s_warp_heads[warp] = (uint32_t)__popc(hb);
-    __syncthreads();
-    uint32_t run = (uint32_t)__popc(hb & (0xffffffffu >> (31 - lane)));      /* heads at or before this lane */
-    for (int w = 0; w < warp; ++w) run += s_warp_heads[w];
-    run = binned ? run - 1u : 0u;                                             /* a binned query's run index */
-    uint32_t n_runs = 0;
-    for (int w = 0; w < LV_STAGE_QUERIES / 32; ++w) n_runs += s_warp_heads[w];
-    if (binned && active) s_run_need[run] = 1u;                               /* benign race: everybody writes 1 */
-    __syncthreads();
-    /* the head of a run fetches its voxel's slot */
-    uint32_t my_count = 0;
-    if (head) {
-        const uint4 e0 = load_slot(a.map.table + 2 * (size_t)key), e1 = load_slot(a.map.table + 2 * (size_t)key + 1);
-        const uint64_t vk = (uint64_t)e0.x | ((uint64_t)e0.y << 32);
-        s_run_vox[run][0] = (uint32_t)vk & 0x1FFFFFu;
-        s_run_vox[run][1] = (uint32_t)(vk >> 21) & 0x1FFFFFu;
-        s_run_vox[run][2] = (uint32_t)(vk >> 42) & 0x1FFFFFu;
-        s_run_start[run] = e1.x;
-        s_run_count[run] = e1.y;
-        my_count = s_run_need[run] ? e1.y : 0u;
-    }
-    /* block-wide exclusive scan of the heads' counts -> staging offsets */
-    uint32_t incl = my_count;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
-        if (lane >= d) incl += v;
-    }
-    if (lane == 31) s_warp_pts[warp] = incl;
-    __syncthreads();
-    uint32_t off = incl - my_count;
-    for (int w = 0; w < warp; ++w) off += s_warp_pts[w];
-    const bool staged = head && my_count > 0u && off + my_count <= (uint32_t)LV_STAGE_PTS;
-    if (head) s_run_off[run] = staged ? off : 0xFFFFFFFFu;
-    /* bytes in flight: the sum over the staged runs */
-    uint32_t my_bytes = staged ? my_count * 16u : 0u;
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) my_bytes += __shfl_xor_sync(0xffffffffu, my_bytes, d);
-    __syncthreads();                              /* s_warp_pts is reused below: everybody has read it */
-    if (lane == 0) s_warp_pts[warp] = my_bytes;
-    __syncthreads();
-    if (tid == 0) {
-        uint32_t total = 0;
-        for (int w = 0; w < LV_STAGE_QUERIES / 32; ++w) total += s_warp_pts[w];
-        mbar_arrive_expect_tx(&s_bar, total);     /* the one arrival the barrier waits for + the bytes the copies bring */
-    }
-    if (staged) bulk_copy_g2s(s_pts + off, a.map.arena + s_run_start[run], my_count * 16u, &s_bar);
-    /* meanwhile: this thread's query */
-    float g[3] = {0.f, 0.f, 0.f};
-    bool finite = false;
-    if (active) {
-        rt_apply(T, jb.xyz[3 * qi], jb.xyz[3 * qi + 1], jb.xyz[3 * qi + 2], g);   /* Mapper.cpp:51 */
-        finite = (fabsf(g[0]) < 1e9f) && (fabsf(g[1]) < 1e9f) && (fabsf(g[2]) < 1e9f);
-    }
-    {   /* wait for the buckets (bounded: a lost transaction must not hang the GPU) */
-        uint32_t spins = 0;
-        while (!mbar_try_wait(&s_bar, 0u)) {
-            if (++spins > (1u << 24)) { __trap(); }
-        }
-    }
-    if (!active) return;
-    Top5 t;
-    top5_init(t, a.max_d2);
-    float cert = 0.f;
-    int st = 0;                                    /* 0 not finite, 1 bucket, 2 no bin */
-    if (finite) st = binned ? 1 : 2;
-    if (st == 1) {
-        const uint32_t bstart = s_run_start[run], n = s_run_count[run], so = s_run_off[run];
-        if (so != 0xFFFFFFFFu) scan_bucket(s_pts + so, n, bstart, g, t);          /* shared memory: LDS.128 */
-        else scan_bucket_global(a.map.arena + bstart, n, bstart, g, t);             /* did not fit the staging budget */
-        cert = neighbourhood_certified_d2(a.map.grid, s_run_vox[run][0], s_run_vox[run][1], s_run_vox[run][2], g[0], g[1], g[2]);
-    }
-    const bool settled = st == 1 && t.d4 <= cert;
-    store_neighbours(a, qi, t);
-    store_ref(a, qi, g, settled ? outsider_bound(t.d5, cert) : 0.f);
-    if (st == 2 || (st == 1 && !settled)) {
-        const uint32_t b = blockIdx.x % kHardBuckets;
-        a.hard_list[(size_t)b * a.hard_seg + atomicAdd(a.hard_count + 4 + b, 1u)] = (uint32_t)qi;
-    }
-    LV_TL_END(2);
-}
-
-/*
  * Kv — reuse.  Evaluations after the first of an update: the iterate moved by millimetres, the map not at all.
  * One thread per query re-measures its five stored neighbours from the new world position and keeps them when
  * query_reusable() proves the exact search would return the same five (lv_voxel_search.h); the others go to
@@ -497,7 +225,6 @@ __global__ void __launch_bounds__(128) lv_reuse_kernel(const MeasureArgs a) {
             redo = false;
         }
     }
-    if (have && a.redo_flag) a.redo_flag[qi] = redo ? 1 : 0;       /* the staged search walks the binned order and skips the rest */
     /* one atomic per warp */
     const unsigned m = __ballot_sync(0xffffffffu, redo);
     if (m) {
@@ -909,27 +636,25 @@ int measure_grid(int n) {
 
 void measure_init() { init_pairs(); }
 
-/* K1 variant of one launch: lanes per query (1, 4, 8) or 32 = lv_search_coop_kernel.
+/* K1 variant of one launch: lanes per query (4 or 8).
  * 4 lanes per query issue a quarter fewer instructions per query than 8 (the prologue is shared by eight queries of a warp
  * instead of four), which pays when a launch has tens of thousands of queries; 8 lanes have the shorter chain per query (a
  * bucket of 36 points is one batch of loads instead of two), which pays on the short work lists of late evaluations and on
  * small sweeps (tools/timeline.py and bench.py's kernel_ms locate the crossover).  So the choice follows the number of queries the launch can expect:
  * all of them in the first evaluation, ~90 % / 45 % / 12 % in evaluations 2 / 3 / 4 of an update with neighbour reuse (cfg1).
- * LV_SEARCH_GROUP overrides for tuning runs and tests (read at every direct launch and when a handle's graph is built). */
+ * LV_SEARCH_GROUP=4|8 overrides for tuning runs and tests (read at every direct launch and when a handle's graph is built). */
 static int search_group(const MeasureArgs& a, int eval) {
     const char* e = getenv("LV_SEARCH_GROUP");
     if (e) {
         const int group = atoi(e);
-        if (group == 1 || group == 4 || group == 8 || group == 32) return group;
+        if (group == 4 || group == 8) return group;
     }
     static const double kRedoShare[4] = {1.0, 0.9, 0.45, 0.12};
     const double share = (eval > 0 && a.ref) ? kRedoShare[eval < 3 ? eval : 3] : 1.0;
     return (double)a.n * share >= 40000.0 ? 4 : 8;
 }
-static int search_block(int group) { return group == 32 ? LV_COOP_THREADS : LV_SEARCH_THREADS; }
 static int search_grid(const MeasureArgs& a, int group) {
-    const int sgrid = group == 32 ? (int)(((int64_t)a.n + LV_COOP_THREADS - 1) / LV_COOP_THREADS)
-                                  : (int)(((int64_t)a.n * group + LV_SEARCH_THREADS - 1) / LV_SEARCH_THREADS);
+    const int sgrid = (int)(((int64_t)a.n * group + LV_SEARCH_THREADS - 1) / LV_SEARCH_THREADS);
     return sgrid < 1 ? 1 : sgrid;
 }
 /* <<<>>> with the programmatic-dependent-launch attribute when `pdl` (see pdl_wait above) */
@@ -950,8 +675,6 @@ static cudaError_t launch_k(void (*kernel)(Params...), unsigned grid, unsigned b
 template <bool LIST>
 static void launch_search(const MeasureArgs& a, int group, int sgrid, cudaStream_t st, bool pdl) {
     switch (group) {
-        case 1: launch_k(lv_search_kernel<1, LIST>, sgrid, LV_SEARCH_THREADS, st, pdl, a); break;
-        case 32: launch_k(lv_search_coop_kernel<LIST>, sgrid, LV_COOP_THREADS, st, pdl, a); break;
         case 4: launch_k(lv_search_kernel<4, LIST>, sgrid, LV_SEARCH_THREADS, st, pdl, a); break;
         default: launch_k(lv_search_kernel<8, LIST>, sgrid, LV_SEARCH_THREADS, st, pdl, a); break;
     }
@@ -964,17 +687,14 @@ cudaError_t launch_measure(const MeasureArgs& a, int grid, cudaStream_t st, cons
     /* work-list length, a spare word, redo-list length; inside an update with pdl the kernels
      * reset them themselves (begin kernel, fit kernel) so that every node of the update is a kernel */
     if (!pdl) cudaMemsetAsync(a.hard_count, 0, kCounters * sizeof(uint32_t), st);
-    const unsigned qgrid = (unsigned)((a.n + LV_STAGE_QUERIES - 1) / LV_STAGE_QUERIES > 0 ? (a.n + LV_STAGE_QUERIES - 1) / LV_STAGE_QUERIES : 1);
     if (reuse && a.ref) {
         if (probe) probe->at(probe->ctx, 4);
         launch_k(lv_reuse_kernel, (a.n + 127) / 128 > 0 ? (a.n + 127) / 128 : 1, 128, st, pdl != 0, a);
         if (probe) probe->at(probe->ctx, 0);
-        if (a.bin_key) launch_k(lv_search_staged_kernel<true>, qgrid, LV_STAGE_QUERIES, st, pdl != 0, a);
-        else launch_search<true>(a, group, sgrid, st, pdl != 0);
+        launch_search<true>(a, group, sgrid, st, pdl != 0);
     } else {
         if (probe) probe->at(probe->ctx, 0);
-        if (a.bin_key) launch_k(lv_search_staged_kernel<false>, qgrid, LV_STAGE_QUERIES, st, pdl != 0, a);
-        else launch_search<false>(a, group, sgrid, st, pdl != 0);
+        launch_search<false>(a, group, sgrid, st, pdl != 0);
     }
     static const bool dbg_sync = getenv("LV_DEBUG_SYNC") != nullptr;   /* diagnosis: name the kernel that does not finish */
     if (dbg_sync) { cudaStreamSynchronize(st); fprintf(stderr, "[lv] search done\n"); fflush(stderr); }
@@ -986,22 +706,6 @@ cudaError_t launch_measure(const MeasureArgs& a, int grid, cudaStream_t st, cons
     if (dbg_sync) { cudaStreamSynchronize(st); fprintf(stderr, "[lv] fit done\n"); fflush(stderr); }
     if (probe) probe->at(probe->ctx, 3);
     return cudaGetLastError();
-}
-size_t bin_sort_tmp_bytes(int64_t max_points) {
-    size_t bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
-                                    (uint32_t*)nullptr, (int)max_points, 0, 32);
-    return bytes;
-}
-cudaError_t launch_bin(const MeasureArgs& a, cudaStream_t st, int pdl, int* launches) {
-    launch_k(lv_bin_kernel, (unsigned)((a.n + 127) / 128 > 0 ? (a.n + 127) / 128 : 1), 128, st, pdl != 0, a);
-    size_t tmp = a.sort_tmp_bytes;
-    /* with a device-side job (graph replay) the sort covers the capacity a.n: positions past the sweep's n hold the
-     * previous sweep's pairs, which lv_search_staged_kernel never reads (keys are sorted per launch over [0, a.n)) */
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(a.sort_tmp, tmp, a.bin_key_in, const_cast<uint32_t*>(a.bin_key), a.bin_val_in,
-                                                    const_cast<uint32_t*>(a.bin_val), a.n, 0, a.sort_bits, st);
-    if (launches) *launches += 1 + 4;
-    return e != cudaSuccess ? e : cudaGetLastError();
 }
 cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n, uint32_t* counters, cudaStream_t st) {
     lv_ieskf_begin_kernel<<<1, 256, 0, st>>>(c, job, xyz, n, counters);

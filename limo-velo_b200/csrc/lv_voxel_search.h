@@ -14,8 +14,7 @@
  *   level 0     ONE probe finds the query's home voxel and ONE contiguous scan of its halo bucket sees every map
  *               point within Chebyshev ring 1, i.e. within the certified radius (edge + distance to the nearest
  *               face) of the query.  If the 5th best lies inside that radius the answer is exact and final (the
- *               bulk of a sweep).  lv_measure.cu runs this tier from shared memory: the queries of a block are
- *               binned by home voxel and each bucket is fetched once (bulk copy).
+ *               bulk of a sweep).  lv_measure.cu runs this tier with 4 or 8 lanes per query.
  *   knn5_rings  the rest — sparse spot, or a query more than a voxel away from the map — one warp per query:
  *               every voxel whose box lies closer than the bound level 0 established (or the search radius) is
  *               visited through the 4x4x4 block occupancy masks; exact by construction.
@@ -102,7 +101,7 @@ struct GroupSerial {   /* host / single lane */
 };
 #if defined(__CUDACC__)
 template <int G>
-struct GroupLanes {    /* G consecutive lanes of a warp (G = 8 or 32); every lane of the WARP must call merge() */
+struct GroupLanes {    /* G consecutive lanes of a warp (G = 4 or 8 per level-0 query, 32 = GroupWarp for the ring search); every lane of the WARP must call merge() */
     enum { size = G };
     __device__ __forceinline__ static int lane() { return (int)(threadIdx.x & (G - 1)); }
     __device__ __forceinline__ static uint32_t bcast(uint32_t v, int src) {
@@ -172,27 +171,6 @@ LV_HD float certified_d2(const HomeGeom& h) {
     cert = cert > 0.f ? cert : 0.f;
     return cert * cert;
 }
-/* The bucket of voxel (bx, by, bz) holds every map point of the voxel's 3x3x3 neighbourhood.  For a query ANYWHERE
- * (it may have left the voxel it was binned in), every other map point is at least as far as the neighbourhood's
- * boundary: the squared certified radius is the squared distance to the nearest face of that 3-voxel cube, 0 outside.
- * For a query inside the centre voxel this equals certified_d2(home_geom()). */
-LV_HD float neighbourhood_certified_d2(const MapGrid& grid, uint32_t bx, uint32_t by, uint32_t bz, float gx, float gy, float gz) {
-    const uint32_t b[3] = {bx, by, bz};
-    const float g[3] = {gx, gy, gz};
-    const float c = grid.cell0;
-    float gap = INFINITY;
-    for (int a = 0; a < 3; ++a) {
-        const float o = voxel_low(grid, b[a]);
-        const float lo = (g[a] - o) + c, hi = (c - (g[a] - o)) + c;      /* to the low / high face of the 3-voxel cube */
-        gap = gap < lo ? gap : lo;
-        gap = gap < hi ? gap : hi;
-    }
-    float amax = fabsf(gx) > fabsf(gy) ? fabsf(gx) : fabsf(gy);
-    amax = amax > fabsf(gz) ? amax : fabsf(gz);
-    float cert = gap - 2e-6f * (amax + 4.0f);
-    cert = cert > 0.f ? cert : 0.f;
-    return cert * cert;
-}
 /* squared distance from the query to the voxel at offset (dx, dy, dz) from its home voxel, rounded down */
 LV_HD float voxel_box_d2(const HomeGeom& h, int dx, int dy, int dz) {
     const int d[3] = {dx, dy, dz};
@@ -236,7 +214,7 @@ LV_HD float level0_certified(const VoxelMapView& m, float gx, float gy, float gz
 
 template <class Grp>
 LV_HD bool level0_scan(const VoxelMapView& m, float gx, float gy, float gz, float max_d2, uint32_t bstart, uint32_t bcount,
-                       bool active, Top5& out, float* region_d2 = nullptr, const uint32_t* vox = nullptr, const float* cert_d2 = nullptr) {
+                       bool active, Top5& out, float* region_d2 = nullptr, const uint32_t* vox = nullptr) {
     Top5 loc;
     top5_init(loc, max_d2);
     if (active) {
@@ -267,9 +245,7 @@ LV_HD bool level0_scan(const VoxelMapView& m, float gx, float gy, float gz, floa
     }
     Grp::merge(loc, max_d2, out);
     if (!active) return false;
-    /* cert_d2: the caller computed certified_d2() already (lv_search_coop_kernel does it once per query, not once per lane group) */
-    const float cert = cert_d2 ? *cert_d2
-                               : (vox ? certified_d2(home_geom(m.grid, vox[0], vox[1], vox[2], gx, gy, gz)) : level0_certified(m, gx, gy, gz));
+    const float cert = vox ? certified_d2(home_geom(m.grid, vox[0], vox[1], vox[2], gx, gy, gz)) : level0_certified(m, gx, gy, gz);
     if (region_d2) *region_d2 = cert;     /* every map point outside the bucket is at least this far (squared) */
     return out.d4 <= cert;                /* out.d4 <= max_d2 always */
 }

@@ -37,7 +37,6 @@ extern "C" void lv_default_params(lv_params* p) {
     p->map_downsample_size = 0.2f;            /* Mapper.cpp:65 */
     p->voxel_size = 0.4f;
     p->device = 0;
-    p->sort_queries = 0;
     p->max_map_points = 4 * 1024 * 1024;
     p->max_points = 512 * 1024;
     p->stream = NULL;
@@ -158,6 +157,5 @@ extern "C" lv_status lv_params_from_yaml(const char* path, lv_params* p) {
     }
     /* device tuning keys are optional extensions */
     numf("voxel_size", &p->voxel_size);
-    numi("sort_queries", &p->sort_queries);
     return LV_OK;
 }

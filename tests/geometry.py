@@ -11,8 +11,8 @@ update (lv_voxel_map.h):
   blind         surfaces, queries 0.9-1.9 m off them: no level-0 slot but five points inside the gate (the blind path)
   cavity        every 0.4 m voxel of a volume occupied except an empty sphere of radius 1.3 m, queries near its centre: blind,
                 with more than kRingCands (1024) occupied voxels in the r = 5 cube
-  cluster       one 0.4 m voxel holding 3200 points, repeated map points, then a downsampled add into both: a halo bucket
-                larger than LV_STAGE_PTS (2560, global scan in the staged kernel), cells with several old points
+  cluster       one 0.4 m voxel holding 3200 points, repeated map points, then a downsampled add into both: a 3200-point
+                halo bucket through the per-query scan, cells with several old points
   tiny          maps of 1, 4, 5 and 6 points: fewer than five neighbours
   far           sweep_built and sparse moved to (2e5, -3e5, 50) and (4.3e5, 0, 0): fp32 ulps of 0.016-0.03 m, and voxel
                 coordinates past the 21-bit key range, where voxel_of_cell clamps
@@ -65,11 +65,10 @@ class GeoScene:
         loc.map_status()
         return loc
 
-    def params(self, lv, voxel, sort_queries=0):
+    def params(self, lv, voxel):
         prm = lv.params_from_yaml(lv.CONFIG_DIR + "/xaloc.yaml", max_map_points=max(1 << 16, self.capacity),
                                   max_points=max(4096, len(self.queries), max((len(a) for a in self.adds), default=0)))
         prm.voxel_size = voxel
-        prm.sort_queries = sort_queries
         return prm
 
 
@@ -163,7 +162,7 @@ def cluster(lv):
                         base[rng.integers(0, 2500, 2500)] + rng.normal(0, 0.05, (2500, 3)),
                         base[rng.integers(0, len(base), 2000)] + rng.normal(0, 0.1, (2000, 3))])
     x, _ = identity_state(lv)
-    return GeoScene("cluster", build, q, x, (0.4,), [add.astype(np.float32)], "bucket > LV_STAGE_PTS, n_old > 1")
+    return GeoScene("cluster", build, q, x, (0.4,), [add.astype(np.float32)], "3200-point bucket, n_old > 1")
 
 
 def tiny(lv, n):

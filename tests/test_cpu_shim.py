@@ -257,7 +257,7 @@ import geometry as geo  # noqa: E402
 
 # Floors on the share of queries that take each scene's path, at each voxel size it runs at: about half the share measured on
 # these seeded scenes.  "uncert" = level 0 does not settle the query (ring search), "blind" = no level-0 slot while five map
-# points lie inside the gate, "big" = the home halo bucket holds more than LV_STAGE_PTS (2560) points.
+# points lie inside the gate, "big" = the home halo bucket holds more than 2560 points (many scan rounds per lane group).
 SCENE_FLOORS = {
     "sweep_built": ("uncert", {0.2: 0.18, 0.4: 0.06, 0.6: 0.035}),
     "sparse": ("uncert", {0.2: 0.5, 0.4: 0.38, 0.6: 0.025}),

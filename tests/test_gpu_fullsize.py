@@ -172,11 +172,9 @@ def test_neighbour_reuse_and_graph_replay_change_nothing(lv, full, monkeypatch):
         loc.close()
         return out
     base = run(["LV_NO_REUSE", "LV_NO_GRAPH", "LV_NO_PDL"])
-    # ... nor may the shape of the level-0 search kernel: 4 or 8 lanes per query (the default picks by launch size), one lane
-    # per query, or the query-per-lane prologue with 8-lane scans (lv_search_coop_kernel)
+    # ... nor may the shape of the level-0 search kernel: 4 or 8 lanes per query (the default picks by launch size)
     for env in ([], ["LV_NO_GRAPH"], ["LV_NO_REUSE"], ["LV_NO_PDL"], ["LV_NO_GRAPH", "LV_NO_PDL"],
-                ["LV_SEARCH_GROUP=1"], ["LV_SEARCH_GROUP=4"], ["LV_SEARCH_GROUP=8"], ["LV_SEARCH_GROUP=32"],
-                ["LV_SEARCH_GROUP=32", "LV_NO_GRAPH", "LV_NO_REUSE"]):
+                ["LV_SEARCH_GROUP=4"], ["LV_SEARCH_GROUP=8"], ["LV_SEARCH_GROUP=8", "LV_NO_GRAPH", "LV_NO_REUSE"]):
         got = run(env)
         for (st0, x0, P0, l0), (st1, x1, P1, l1) in zip(base, got):
             assert st0 == st1 == 0 and len(l0) == len(l1)

@@ -2,9 +2,9 @@
 device tick started from an empty map.
 
 Each scene is built for a path the dense surface map never takes (a map grown from raw sweeps, sparse and blind queries,
-a cavity with more occupied voxels around it than the ring search lists, a bucket too big to stage, tiny maps, coordinates
-far from the origin); test_cpu_shim proves the share of queries on that path.  Here every K1 shape — LV_SEARCH_GROUP 1, 4,
-8 and 32 (read at every direct launch) and the staged kernel (sort_queries: 1) — must give the oracle's answers: no
+a cavity with more occupied voxels around it than the ring search lists, a 3 200-point halo bucket, tiny maps, coordinates
+far from the origin); test_cpu_shim proves the share of queries on that path.  Here every K1 shape — LV_SEARCH_GROUP 4 and
+8 (read at every direct launch) and the unpinned per-launch policy — must give the oracle's answers: no
 query with five neighbours inside the gate missed, squared distances bit-exact, accept bit / plane / distance bit-exact
 except for queries whose 5th and 6th neighbours are exactly equidistant at different coordinates, normal equations to
 1e-12.  On the scenes with enough matches a whole update must not depend on reuse, graph replay or PDL, and must pass
@@ -19,7 +19,7 @@ from test_gpu_fullsize import check_every_evaluation
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1200, method="thread")]
 
-SHAPES = [("group", 1), ("group", 4), ("group", 8), ("group", 32), ("sorted", None)]
+SHAPES = (4, 8, None)                                        # LV_SEARCH_GROUP; None: search_group()'s policy
 UPDATE_SCENES = ("sweep_built", "blind", "cluster")          # enough matches for a whole update
 
 
@@ -50,30 +50,27 @@ def test_every_search_shape_matches_the_oracle(lv, O, scenes, monkeypatch, name,
     oprm = O.make_params()
     ref_set = set(map(tuple, om.points().tolist())) if sc.adds else None
     st_o, HTH_o, HTh_o, nm_o = om.measure_reduced(sc.x, oprm, sc.queries)
-    for sort_queries in (0, 1):
-        loc = sc.localizer(lv, sc.params(lv, voxel, sort_queries))
-        if sc.adds:                                                 # the map the rule grew: the oracle's, up to voxel-face ulps
-            got_set = set(map(tuple, loc.map_points().tolist()))
-            assert len(got_set ^ ref_set) <= 1e-4 * len(ref_set), (len(got_set ^ ref_set), len(ref_set))
+    loc = sc.localizer(lv, sc.params(lv, voxel))
+    if sc.adds:                                                     # the map the rule grew: the oracle's, up to voxel-face ulps
+        got_set = set(map(tuple, loc.map_points().tolist()))
+        assert len(got_set ^ ref_set) <= 1e-4 * len(ref_set), (len(got_set ^ ref_set), len(ref_set))
+    else:
+        assert loc.map_size() == len(sc.build)
+    for group in SHAPES:
+        if group is None:
+            monkeypatch.delenv("LV_SEARCH_GROUP", raising=False)
         else:
-            assert loc.map_size() == len(sc.build)
-        for kind, group in SHAPES:
-            if (kind == "sorted") != (sort_queries == 1):
-                continue
-            if group is None:
-                monkeypatch.delenv("LV_SEARCH_GROUP", raising=False)
-            else:
-                monkeypatch.setenv("LV_SEARCH_GROUP", str(group))
-            got = _check_points(loc, om, oprm, sc.x, sc.queries, max_ties=None if name == "cluster" else 4)
-            st, HTH, HTh, nm = loc.measure_reduced(sc.x, sc.queries)
-            assert st == st_o
-            if got["ties"] == 0:
-                assert nm == nm_o, (kind, group, nm, nm_o)
-                assert np.abs(HTH - HTH_o).max() <= 1e-12 * max(np.abs(HTH_o).max(), 1e-300)
-                assert np.abs(HTh - HTh_o).max() <= 1e-12 * max(np.abs(HTh_o).max(), 1e-300) + 1e-15
-            else:
-                assert abs(nm - nm_o) <= got["ties"]
-        loc.close()
+            monkeypatch.setenv("LV_SEARCH_GROUP", str(group))
+        got = _check_points(loc, om, oprm, sc.x, sc.queries, max_ties=None if name == "cluster" else 4)
+        st, HTH, HTh, nm = loc.measure_reduced(sc.x, sc.queries)
+        assert st == st_o
+        if got["ties"] == 0:
+            assert nm == nm_o, (group, nm, nm_o)
+            assert np.abs(HTH - HTH_o).max() <= 1e-12 * max(np.abs(HTH_o).max(), 1e-300)
+            assert np.abs(HTh - HTh_o).max() <= 1e-12 * max(np.abs(HTh_o).max(), 1e-300) + 1e-15
+        else:
+            assert abs(nm - nm_o) <= got["ties"]
+    loc.close()
 
 
 @pytest.mark.parametrize("name", UPDATE_SCENES)
@@ -85,12 +82,12 @@ def test_update_on_the_scene_needs_no_switch_and_matches_the_oracle(lv, O, scene
     prm = sc.params(lv, 0.4)
     x0, P0 = lv.init_state_host(prm)
 
-    def run(env, sort_queries=0):
+    def run(env):
         for k in ("LV_NO_REUSE", "LV_NO_GRAPH", "LV_NO_PDL", "LV_SEARCH_GROUP"):
             monkeypatch.delenv(k, raising=False)
         for k in env:
             monkeypatch.setenv(*(k.split("=") if "=" in k else (k, "1")))
-        loc = sc.localizer(lv, sc.params(lv, 0.4, sort_queries))     # the switches are read by lv_create
+        loc = sc.localizer(lv, sc.params(lv, 0.4))                   # the switches are read by lv_create
         loc.set_state(sc.x, P0)
         out = loc.correct(sc.queries)
         return loc, out
@@ -100,8 +97,8 @@ def test_update_on_the_scene_needs_no_switch_and_matches_the_oracle(lv, O, scene
     assert st == 0 and logs[0]["n_matches"] > 1000
     check_every_evaluation(O, om, oprm, sc.x, P0, sc.queries, logs, loc)
     loc.close()
-    for env, sq in (([], 0), ([], 1), (["LV_SEARCH_GROUP=1"], 0), (["LV_SEARCH_GROUP=4"], 0), (["LV_SEARCH_GROUP=32"], 0)):
-        loc, (st1, x1, P1, l1) = run(env, sq)
+    for env in ([], ["LV_SEARCH_GROUP=4"], ["LV_SEARCH_GROUP=8"]):
+        loc, (st1, x1, P1, l1) = run(env)
         loc.close()
         assert st1 == 0 and len(l1) == len(logs), env
         assert (x1 == x).all() and (P1 == P).all(), env

@@ -3,7 +3,7 @@
 A growth re-hashes the voxel and block tables into larger ones and copies the arena's used prefix, on the handle's stream;
 content, ids, insertion order and arena indices are kept.  So a handle that starts small and grows must give, tick by tick,
 exactly what a handle born at the final capacity gives: the same status, bit-identical logs, x and P, the same neighbours
-and the same map.  That holds with the update graph, neighbour reuse and binned queries on or off (a growth drops the
+and the same map.  That holds with the update graph and neighbour reuse on or off (a growth drops the
 cached update graphs: they embed the old table and arena pointers).
 
 Peak device memory: the scattered-cloud test needs a 4 M-point capacity (27 table slots per isolated point), about 6.5 GB
@@ -39,10 +39,8 @@ def road(lv, O):
     return dict(world=world, sweeps=sweeps, x_props=x_props, truths=truths)
 
 
-def _params(lv, cap, sort_queries=0):
-    prm = bench.config_params(lv, "cfg1", max_points=RINGS * AZIMUTHS, max_map_points=cap)
-    prm.sort_queries = sort_queries
-    return prm
+def _params(lv, cap):
+    return bench.config_params(lv, "cfg1", max_points=RINGS * AZIMUTHS, max_map_points=cap)
 
 
 def _stream(lv, road, prm, grow_limit=0, checkpoints=(9, 19, 29)):
@@ -93,20 +91,20 @@ def _same_run(a, b):
 
 def test_growth_during_the_device_tick(lv, road, monkeypatch):
     """a handle born at 8192 points with growth on grows at least three times while it streams; a handle born at the final
-    capacity must agree tick by tick, with and without graph replay, reuse and binned queries"""
+    capacity must agree tick by tick, with and without graph replay and reuse"""
     base = None
-    for env, sq in (([], 0), (["LV_NO_GRAPH"], 0), (["LV_NO_REUSE"], 0), ([], 1)):
+    for env in ([], ["LV_NO_GRAPH"], ["LV_NO_REUSE"]):
         for k in ("LV_NO_GRAPH", "LV_NO_REUSE"):
             monkeypatch.delenv(k, raising=False)
         for k in env:
             monkeypatch.setenv(k, "1")
-        grown, info, final, caps = _stream(lv, road, _params(lv, 8192, sq), grow_limit=1 << 22)
+        grown, info, final, caps = _stream(lv, road, _params(lv, 8192), grow_limit=1 << 22)
         assert info["growths"] >= 3, info
         assert info["error_flags"] == 0
         # growths between two ticks that replay the same update graph (one sweep size: one capacity bucket)
         assert sum(1 for t in range(2, N_TICKS) if caps[t] != caps[t - 1]) >= 1, caps
         assert sum(1 for r in grown if r["st"] == lv.OK) >= N_TICKS // 2
-        big, binfo, bfinal, _ = _stream(lv, road, _params(lv, info["capacity_points"], sq))
+        big, binfo, bfinal, _ = _stream(lv, road, _params(lv, info["capacity_points"]))
         assert binfo["growths"] == 0 and binfo["capacity_points"] == info["capacity_points"]
         _same_run(grown, big)
         assert np.array_equal(final, bfinal) and len(final) == info["points"] == binfo["points"]

@@ -2,9 +2,10 @@
 
 Round 1 left a hang open: lv_search_kernel<4> (4 lanes per query) never finished on bench sweeps 5 and 7 at
 voxel_size 0.35 (deterministic in isolation; the 1- and 8-lane instantiations of the same source were fine).  The per-query
-kernel exists with 1, 4 and 8 lanes (lv_search_kernel<4> is the default for launches of 40 000 queries or more; every
-shape runs on the maps of test_gpu_geometry.py), and this test pins the whole family: every voxel size the grid can take (k = 1, 2, 3 downsample cells per edge; 0.3,
-0.35 and 0.5 round to a neighbour), every bench sweep, both query orders, bit-exact against the oracle.
+kernel exists with 4 and 8 lanes (lv_search_kernel<4> is the default for launches of 40 000 queries or more; both run on
+the maps of test_gpu_geometry.py), and this test pins both, LV_SEARCH_GROUP=4 and =8: every voxel size the grid can take
+(k = 1, 2, 3 downsample cells per edge; 0.3, 0.35 and 0.5 round to a neighbour), every bench sweep, bit-exact against the
+oracle.
 A kernel that does not terminate fails the test through pytest-timeout (thread method: the process is ended)."""
 import numpy as np
 import pytest
@@ -31,12 +32,12 @@ def scene(lv, O):
     return dict(prm=prm, map=mp, sweeps=sweeps, x_props=x_props, ref=ref)
 
 
-@pytest.mark.parametrize("sorted_queries", [0, 1])
+@pytest.mark.parametrize("group", [4, 8])
 @pytest.mark.parametrize("voxel", VOXELS)
-def test_every_voxel_size_every_sweep(lv, scene, voxel, sorted_queries):
+def test_every_voxel_size_every_sweep(lv, scene, monkeypatch, voxel, group):
+    monkeypatch.setenv("LV_SEARCH_GROUP", str(group))              # read at every direct launch and when a graph is built
     prm = bench.config_params(lv, "cfg1")
     prm.voxel_size = voxel
-    prm.sort_queries = sorted_queries
     loc = lv.Localizer(prm)
     loc.map_build(scene["map"])
     loc.map_status()

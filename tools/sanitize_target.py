@@ -6,14 +6,14 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import __graft_entry__ as G
 lv = G.load_package(); O = G.load_oracle()
-VARIANTS = ((0, None), (0, "4"), (0, "32"), (0, "1"), (1, None))                    # every shape of the level-0 search
+VARIANTS = (None, "4", "8")                    # every shape of the level-0 search (None: the per-launch policy)
 if os.environ.get("LV_SANITIZE_QUICK"):
-    VARIANTS = ((0, "4"), (1, None))
-for sort_queries, group in VARIANTS:
+    VARIANTS = ("4",)
+for group in VARIANTS:
     os.environ.pop("LV_SEARCH_GROUP", None)
     if group:
         os.environ["LV_SEARCH_GROUP"] = group
-    prm = lv.params_from_yaml(os.path.join(lv.CONFIG_DIR, "xaloc.yaml"), max_map_points=1 << 17, max_points=1 << 13, sort_queries=sort_queries)
+    prm = lv.params_from_yaml(os.path.join(lv.CONFIG_DIR, "xaloc.yaml"), max_map_points=1 << 17, max_points=1 << 13)
     world = lv.SynthWorld(20260924, 40000)
     truth = world.pose(10.0, prm)
     sweep = world.sweep(truth, rings=16, azimuths=256, seed=1)
@@ -43,4 +43,4 @@ for sort_queries, group in VARIANTS:
         assert abs(loc.map_size() - len(om.points())) <= 2
         loc.propagate_device(np.tile([0.0, 0.0, 9.8], (4, 1)), np.zeros((4, 3)), np.full(4, 1e-3))
     loc.close()
-    print("sanitize target: sort_queries=%d search group %s ok" % (sort_queries, group or "default"), flush=True)
+    print("sanitize target: search group %s ok" % (group or "default"), flush=True)

@@ -3,7 +3,7 @@
 
     python tools/sass_table.py [lib.so] > profiles/r2_sass_opcodes.txt
 Shows, kernel by kernel, which memory / shuffle / tensor / bulk-copy instructions the compiler emitted
-(e.g. UBLKCP + SYNCS = cp.async.bulk + mbarrier in the staged search; LDG.E.128.CONSTANT = the read-only point loads).
+(e.g. LDG.E.128.CONSTANT = the read-only point loads, DMMA = the fp64 tensor-core fold of the fit kernel).
 """
 import collections, re, subprocess, sys
 lib = sys.argv[1] if len(sys.argv) > 1 else "limo-velo_b200/liblimovelo_b200.so"

@@ -8,7 +8,6 @@ lv = G.load_package()
 CFG = os.environ.get("LV_TIMELINE_CFG", "cfg1")             # any of bench.CONFIGS but cfg4
 prm = bench.config_params(lv, CFG)
 world, mp, sweeps, x_props, truths = bench.make_scene(lv, 0, n_sweeps=2, prm=prm, cfg=CFG)
-prm.sort_queries = int(os.environ.get("LV_TIMELINE_SORT", "0"))
 x0, P0 = lv.init_state_host(prm)
 loc = lv.Localizer(prm); loc.map_build(mp)
 d = [loc.upload(s) for s in sweeps]
