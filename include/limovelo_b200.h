@@ -261,6 +261,7 @@ void lv_host_free(void* p);
 void* lv_device_alloc(lv_handle h, int64_t bytes);
 void lv_device_free(lv_handle h, void* p);
 lv_status lv_memcpy_h2d(lv_handle h, void* dst, const void* src, int64_t bytes);
+lv_status lv_memcpy_d2h(lv_handle h, void* dst, const void* src, int64_t bytes);   /* both synchronise */
 lv_status lv_synchronize(lv_handle h);
 lv_status lv_profile_enable(lv_handle h, int on);             /* CUDA-event timing per kernel  */
 lv_status lv_profile_get(lv_handle h, lv_profile* out, int reset);
@@ -342,6 +343,25 @@ lv_status lv_time_sort_indices(const double* time, int64_t n, int32_t* idx_out);
 lv_status lv_pointcloud2_to_points_checked(lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* data, int64_t data_bytes,
                                            int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning,
                                            double full_rotation_time, float* xyz, double* time, float* intensity, float* range);
+
+/* Accumulator::process (Accumulator.cpp:142-151) on the device: msg2points (PointCloudProcessor.cpp:24-99) ->
+ * temporal_downsample (:101-112) -> sort_points (:114-123).  d_data: DEVICE copy of the message's point bytes
+ * (data_bytes long, any alignment); layout / type / time flags as for lv_pointcloud2_to_points_checked.  Outputs are
+ * DEVICE buffers with room for n points (d_intensity, d_range, d_idx may be NULL); *n_out = points kept.
+ * Output ascending in time, ties in message order: d_xyz / d_time feed lv_compensate_device as they are.
+ * d_idx = index of each output point in the message (for the caller's other fields, e.g. ring).  Synchronises (n_out).
+ * Bit for bit lv_pointcloud2_to_points_checked, then the decimation rule of lv_temporal_downsample on the message index,
+ * then lv_time_sort_indices on the kept times, then the gathers.  The begin time comes from the first and last point of
+ * the whole message, as on the host.  LV_ERR_ARG, before any device work, for a null handle / layout / data / xyz / time /
+ * n_out, n outside [0, 2^31 - 1], a layout _checked refuses, or an output range that overlaps [d_data, d_data +
+ * data_bytes); LV_ERR_ARG after the device work when a kept point's time is NaN (the sort has no order for it).  A NaN
+ * coordinate is no error: min_dist < |p| drops the point.  n == 0, or nothing kept: LV_OK with *n_out = 0. */
+lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout,
+                                  const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t header_stamp_us,
+                                  int stamp_beginning, int offset_beginning, double full_rotation_time,
+                                  int32_t downsample_rate, double min_dist,
+                                  float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
+                                  int64_t* n_out);
 
 /* ---- rosbag reader (format 2.0; replaces roscpp / `rosbag play` in front of Accumulator::receive_lidar / receive_imu,
  * src/main.cpp:27-39, src/Modules/Accumulator.cpp:39-60).  Sequential read of uncompressed bags (bz2 / lz4 chunks are

@@ -133,6 +133,9 @@ def lib():
     L.lv_device_free.argtypes = [vp, vp]
     L.lv_device_free.restype = None
     L.lv_memcpy_h2d.argtypes = [vp, vp, vp, i64]
+    L.lv_memcpy_d2h.argtypes = [vp, vp, vp, i64]
+    L.lv_process_cloud_device.argtypes = [vp, C.c_int, C.POINTER(CloudLayout), vp, i64, i64, C.c_uint64, C.c_int, C.c_int,
+                                          C.c_double, C.c_int32, C.c_double, vp, vp, vp, vp, vp, C.POINTER(i64)]
     L.lv_synchronize.argtypes = [vp]
     L.lv_profile_enable.argtypes = [vp, C.c_int]
     L.lv_profile_get.argtypes = [vp, C.POINTER(Profile), C.c_int]
@@ -287,14 +290,19 @@ class CloudLayout(C.Structure):
 LIDAR_TYPES = {"velodyne": 0, "hesai": 1, "ouster": 2, "custom": 3}
 
 
+def cloud_layout(lidar, dtype):
+    """lv_cloud_layout of a numpy structured dtype with the fields of `lidar`'s point struct"""
+    f = dtype.fields
+    tname = {"velodyne": "time", "ouster": "t"}.get(lidar, "timestamp")
+    iname = "reflectivity" if lidar == "ouster" else "intensity"
+    return CloudLayout(dtype.itemsize, f["x"][1], f["y"][1], f["z"][1], f[iname][1], f[tname][1],
+                       f["range"][1] if "range" in f else 0)
+
+
 def pointcloud2_to_points(lidar, pts, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time):
     """PointCloudProcessor::msg2points on a numpy structured array (its buffer is the message's `data`)"""
     pts = np.ascontiguousarray(pts)
-    f = pts.dtype.fields
-    tname = {"velodyne": "time", "ouster": "t"}.get(lidar, "timestamp")
-    iname = "reflectivity" if lidar == "ouster" else "intensity"
-    lay = CloudLayout(pts.dtype.itemsize, f["x"][1], f["y"][1], f["z"][1], f[iname][1], f[tname][1],
-                      f["range"][1] if "range" in f else 0)
+    lay = cloud_layout(lidar, pts.dtype)
     n = len(pts)
     xyz, t = np.zeros((n, 3), np.float32), np.zeros(n, np.float64)
     inten, rng = np.zeros(n, np.float32), np.zeros(n, np.float32)
@@ -508,6 +516,42 @@ class Localizer:
         _check(self.L.lv_voxelgrid_downsample_device(self.h, C.c_void_p(d_xyz), C.c_int64(n), C.c_float(leaf), C.c_void_p(d_out),
                                                      C.byref(m)))
         return m.value
+
+    def process_cloud_device(self, lidar, layout, d_data, data_bytes, n, header_stamp_us, stamp_beginning, offset_beginning,
+                             full_rotation_time, downsample_rate, min_dist, d_xyz, d_time, d_intensity=None, d_range=None,
+                             d_idx=None):
+        """Accumulator::process on message bytes already in device memory (raw pointers); returns the points kept"""
+        m = C.c_int64(0)
+        _check(self.L.lv_process_cloud_device(self.h, LIDAR_TYPES[lidar], C.byref(layout), C.c_void_p(d_data), int(data_bytes), int(n),
+                                              int(header_stamp_us), int(stamp_beginning), int(offset_beginning),
+                                              float(full_rotation_time), int(downsample_rate), float(min_dist), C.c_void_p(d_xyz),
+                                              C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
+                                              C.byref(m)))
+        return m.value
+
+    def process_cloud(self, lidar, pts, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time, downsample_rate,
+                      min_dist):
+        """Accumulator::process on a numpy structured array (its buffer is the message's `data`): uploads it, returns
+        (xyz, time, intensity, range, index in the message) of the kept points in time order"""
+        pts = np.ascontiguousarray(pts)
+        n = len(pts)
+        out = (np.empty((n, 3), np.float32), np.empty(n, np.float64), np.empty(n, np.float32), np.empty(n, np.float32),
+               np.empty(n, np.int32))
+        bufs = [self.device_alloc(max(pts.nbytes, 1))] + [self.device_alloc(max(a.nbytes, 1)) for a in out]
+        try:
+            _check(self.L.lv_memcpy_h2d(self.h, bufs[0], pts.ctypes.data_as(C.c_void_p), pts.nbytes))
+            m = self.process_cloud_device(lidar, cloud_layout(lidar, pts.dtype), bufs[0], pts.nbytes, n, header_stamp_us,
+                                          stamp_beginning, offset_beginning, full_rotation_time, downsample_rate, min_dist, *bufs[1:])
+            return tuple(self.download(d, a[:m]) for a, d in zip(out, bufs[1:]))
+        finally:
+            for d in bufs:
+                self.device_free(d)
+
+    def download(self, d_ptr, out):
+        """copy device memory into the contiguous numpy array `out` (its whole size); returns out"""
+        if out.nbytes:
+            _check(self.L.lv_memcpy_d2h(self.h, out.ctypes.data_as(C.c_void_p), C.c_void_p(d_ptr), out.nbytes))
+        return out
 
     def correct_buffers(self):
         """preallocated outputs for correct_raw (benchmarks: keeps numpy / ctypes construction out of the timed call)"""

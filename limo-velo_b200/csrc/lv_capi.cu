@@ -19,6 +19,7 @@
 #include "lv_host.h"
 #include "lv_internal.h"
 #include "lv_predict.h"
+#include "lv_wire.h"
 
 using namespace lv;
 
@@ -1034,6 +1035,13 @@ lv_status lv_memcpy_h2d(lv_handle h, void* dst, const void* src, int64_t bytes) 
     LV_CUDA(cudaStreamSynchronize(h->stream));
     return LV_OK;
 }
+lv_status lv_memcpy_d2h(lv_handle h, void* dst, const void* src, int64_t bytes) {
+    if (!h || !dst || !src || bytes < 0) return LV_ERR_ARG;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(cudaMemcpyAsync(dst, src, (size_t)bytes, cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    return LV_OK;
+}
 /* ---- Compensator::compensate ------------------------------------------------------------------ */
 static lv_status deskew_common(lv_context* h, const lv_state32* path, int32_t ns, const lv_state32* Xt2,
                                const float* d_xyz, const double* d_t, int64_t n, float* d_out) {
@@ -1163,6 +1171,42 @@ lv_status lv_temporal_downsample(lv_handle h, const float* xyz, int64_t n, int32
     if (idx_out) LV_CUDA(cudaMemcpyAsync(idx_out, h->ds.sel, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(cudaStreamSynchronize(h->stream));
     *n_out = m;
+    return LV_OK;
+}
+
+/* ---- Accumulator::process ------------------------------------------------------------------------ */
+lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
+                                  int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
+                                  int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                  int32_t* d_idx, int64_t* n_out) {
+    /* every check before the first device call */
+    if (n_out) *n_out = 0;
+    if (!layout || !d_data || !d_xyz || !d_time || !n_out) { set_error("process cloud: null layout, data, xyz, time or n_out"); return LV_ERR_ARG; }
+    if (n < 0 || n > 0x7fffffff) { set_error("process cloud: n outside [0, 2^31 - 1] (point indices are int32)"); return LV_ERR_ARG; }
+    if (const char* why = cloud_layout_error(type, *layout, n, data_bytes)) { set_error(std::string("process cloud: ") + why); return LV_ERR_ARG; }
+    /* the gather decodes the message while it writes the outputs: an output that overlaps the bytes would be read after it is
+     * overwritten */
+    const struct { const void* p; int64_t bytes; } outs[5] = {{d_xyz, 12 * n}, {d_time, 8 * n}, {d_intensity, 4 * n}, {d_range, 4 * n},
+                                                            {d_idx, 4 * n}};
+    for (const auto& o : outs)
+        if (o.p && n > 0 && (uintptr_t)o.p < (uintptr_t)d_data + (uintptr_t)data_bytes && (uintptr_t)d_data < (uintptr_t)o.p + (uintptr_t)o.bytes) {
+            set_error("process cloud: an output range overlaps the message bytes");
+            return LV_ERR_ARG;
+        }
+    if (!h) { set_error("process cloud: null handle"); return LV_ERR_ARG; }
+    if (cloud_bound(n, downsample_rate) == 0) return LV_OK;      /* nothing can be kept */
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(ds_reserve(h->ds, n));
+    const CloudArgs a = {d_data, n, *layout, type, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time, downsample_rate, min_dist};
+    int launches = 0;
+    LV_CUDA(launch_process_cloud(h->ds, a, CloudOut{d_xyz, d_time, d_intensity, d_range, d_idx}, h->stream, &launches));
+    h->prof.total_launches += launches;
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    if (h->ds.h_count[1]) {
+        set_error("process cloud: a kept point's timestamp is NaN (the time sort has no order for it)");
+        return LV_ERR_ARG;
+    }
+    *n_out = h->ds.h_count[0];
     return LV_OK;
 }
 

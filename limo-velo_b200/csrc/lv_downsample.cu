@@ -18,6 +18,7 @@
 #include <cub/iterator/counting_input_iterator.cuh>
 
 #include "lv_internal.h"
+#include "lv_wire.h"
 
 namespace lv {
 
@@ -99,15 +100,12 @@ __global__ void __launch_bounds__(256) lv_ds_centroid_kernel(const float* __rest
     out[3 * (size_t)r] = fdiv(sx, cnt); out[3 * (size_t)r + 1] = fdiv(sy, cnt); out[3 * (size_t)r + 2] = fdiv(sz, cnt);
 }
 
-/* temporal_downsample: keep = (rate <= 1 or (i + 1) % rate == 0) and min_dist < |p| */
+/* temporal_downsample: keep = (rate <= 1 or (i + 1) % rate == 0) and min_dist < |p| (lv_wire.h) */
 __global__ void __launch_bounds__(256) lv_ds_temporal_flag_kernel(const float* __restrict__ xyz, int64_t n, int rate, double min_dist,
                                                                   uint8_t* __restrict__ keep) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-    const float nrm = fsqrt(fadd(fadd(fmul(x, x), fmul(y, y)), fmul(z, z)));
-    const bool k = (rate <= 1 || (i + 1) % rate == 0) && min_dist < (double)nrm;
-    keep[i] = k ? 1 : 0;
+    keep[i] = temporal_keep(i, rate, min_dist, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2]) ? 1 : 0;
 }
 __global__ void __launch_bounds__(256) lv_ds_gather_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ idx,
                                                            const int* __restrict__ n_sel, float* __restrict__ out) {
@@ -121,11 +119,12 @@ __global__ void __launch_bounds__(256) lv_ds_gather_kernel(const float* __restri
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n) {
     if (n <= s.cap) return cudaSuccess;
     cudaFree(s.keys); cudaFree(s.keys_sorted); cudaFree(s.vals); cudaFree(s.vals_sorted); cudaFree(s.flags); cudaFree(s.sel);
+    cudaFree(s.keys64); cudaFree(s.keys64_sorted);
     cudaFree(s.tmp);
     if (!s.box) {
         cudaError_t e = cudaMalloc(&s.box, sizeof(GridBox));
         if (e != cudaSuccess) return e;
-        if ((e = cudaMalloc(&s.count, sizeof(int))) != cudaSuccess) return e;
+        if ((e = cudaMalloc(&s.count, 2 * sizeof(int))) != cudaSuccess) return e;
         if ((e = cudaMallocHost(&s.h_count, 2 * sizeof(int))) != cudaSuccess) return e;
     }
     const int64_t cap = n + n / 4 + 1024;
@@ -134,7 +133,11 @@ cudaError_t ds_reserve(DownsampleScratch& s, int64_t n) {
                                     (uint32_t*)nullptr, (int)cap);
     cub::DeviceSelect::Flagged(nullptr, b, cub::CountingInputIterator<int32_t>(0), (const uint8_t*)nullptr, (int32_t*)nullptr,
                                (int*)nullptr, (int)cap);
-    s.tmp_bytes = (a > b ? a : b) + 256;
+    size_t c = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, c, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const uint32_t*)nullptr,
+                                    (uint32_t*)nullptr, (int)cap);
+    s.tmp_bytes = (a > b ? a : b);
+    s.tmp_bytes = (s.tmp_bytes > c ? s.tmp_bytes : c) + 256;
     cudaError_t e;
     if ((e = cudaMalloc(&s.keys, sizeof(uint32_t) * cap)) != cudaSuccess) return e;
     if ((e = cudaMalloc(&s.keys_sorted, sizeof(uint32_t) * cap)) != cudaSuccess) return e;
@@ -142,12 +145,15 @@ cudaError_t ds_reserve(DownsampleScratch& s, int64_t n) {
     if ((e = cudaMalloc(&s.vals_sorted, sizeof(uint32_t) * cap)) != cudaSuccess) return e;
     if ((e = cudaMalloc(&s.flags, sizeof(uint8_t) * cap)) != cudaSuccess) return e;
     if ((e = cudaMalloc(&s.sel, sizeof(int32_t) * cap)) != cudaSuccess) return e;
+    if ((e = cudaMalloc(&s.keys64, sizeof(uint64_t) * cap)) != cudaSuccess) return e;
+    if ((e = cudaMalloc(&s.keys64_sorted, sizeof(uint64_t) * cap)) != cudaSuccess) return e;
     if ((e = cudaMalloc(&s.tmp, s.tmp_bytes)) != cudaSuccess) return e;
     s.cap = cap;
     return cudaSuccess;
 }
 void ds_free(DownsampleScratch& s) {
     cudaFree(s.keys); cudaFree(s.keys_sorted); cudaFree(s.vals); cudaFree(s.vals_sorted); cudaFree(s.flags); cudaFree(s.sel);
+    cudaFree(s.keys64); cudaFree(s.keys64_sorted);
     cudaFree(s.tmp); cudaFree(s.box); cudaFree(s.count); cudaFreeHost(s.h_count);
     s = DownsampleScratch();
 }

@@ -145,13 +145,14 @@ cudaError_t launch_l2_flush(void* buf, size_t bytes, cudaStream_t st);
 struct DownsampleScratch {
     int64_t cap = 0;
     uint32_t *keys = nullptr, *keys_sorted = nullptr, *vals = nullptr, *vals_sorted = nullptr;
+    uint64_t *keys64 = nullptr, *keys64_sorted = nullptr;   /* time keys of lv_cloud.cu */
     uint8_t* flags = nullptr;
     int32_t* sel = nullptr;
     void* tmp = nullptr;
     size_t tmp_bytes = 0;
     void* box = nullptr;           /* GridBox */
-    int* count = nullptr;
-    int* h_count = nullptr;        /* pinned: [0] output count, [1] overflow flag */
+    int* count = nullptr;          /* [0] output count, [1] NaN-time flag (lv_cloud.cu) */
+    int* h_count = nullptr;        /* pinned: [0] output count, [1] overflow flag (voxel grid) / NaN-time flag (cloud) */
 };
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n);
 void ds_free(DownsampleScratch& s);
@@ -159,6 +160,25 @@ cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, int64_t n
                              int* launches);
 cudaError_t launch_temporal(DownsampleScratch& s, const float* d_xyz, int64_t n, int rate, double min_dist, float* d_out,
                             int32_t* d_idx_out, cudaStream_t st, int* launches);
+
+/* lv_cloud.cu: Accumulator::process (msg2points -> temporal_downsample -> sort_points) on the message bytes in HBM */
+struct CloudArgs {
+    const uint8_t* data;       /* the message's point bytes (device, any alignment) */
+    int64_t n;
+    lv_cloud_layout layout;
+    lv_lidar_type type;
+    uint64_t stamp_us;
+    int32_t stamp_beginning, offset_beginning;
+    double full_rotation_time;
+    int32_t rate;
+    double min_dist;
+};
+struct CloudOut { float* xyz; double* time; float* intensity; float* range; int32_t* idx; };   /* intensity / range / idx may be NULL */
+/* most points the decimator can keep: the slots the sort runs over */
+int64_t cloud_bound(int64_t n, int rate);
+/* enqueues everything (needs ds_reserve(s, n) and cloud_bound > 0); afterwards s.h_count[0] = points kept, s.h_count[1] = 1 if a
+ * kept point's time is NaN (after a stream sync) */
+cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const CloudOut& o, cudaStream_t st, int* launches);
 
 /* lv_deskew.cu: Compensator::compensate.  d_bad (one int) is set when a timestamp is out of range / out of order */
 int deskew_max_states();

@@ -1,0 +1,124 @@
+/*
+ * lv_wire.h — the per-point arithmetic of the LiDAR message, compiled by the host (lv_pointcloud2_to_points) and the device
+ * (lv_process_cloud_device, the temporal decimator) alike, so that both give the same bits:
+ *   PointCloudProcessor::msg2points / get_begin_time   src/Utils/PointCloudProcessor.cpp:24-99
+ *   Point(const <driver>::Point&, double time_offset)   src/Objects/Point.cpp:37-111,153-175
+ *   Conversions::microsec2Sec / nanosec2Sec             src/Utils/Utils.cpp:18-30
+ *   PointCloudProcessor::temporal_downsample            src/Utils/PointCloudProcessor.cpp:101-112
+ * Fields sit at whatever byte offsets the message declares and the message itself may start at any address, so every
+ * value is assembled from single bytes (little endian): no 2-, 4- or 8-byte load is ever misaligned.  The doubles go
+ * through lv::dadd / lv::dmul so that nvcc cannot contract them into FMAs the host build does not form.
+ */
+#ifndef LV_WIRE_H_
+#define LV_WIRE_H_
+
+#include <stdint.h>
+#include <string.h>
+
+#include "../../include/limovelo_b200.h"
+#include "lv_hd.h"
+
+namespace lv {
+
+LV_HD uint32_t wire_u8(const uint8_t* p) { return p[0]; }
+LV_HD uint32_t wire_u16(const uint8_t* p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8; }
+LV_HD uint32_t wire_u32(const uint8_t* p) {
+    return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24;
+}
+LV_HD float wire_f32(const uint8_t* p) {
+    const uint32_t u = wire_u32(p);
+#if defined(__CUDA_ARCH__)
+    return __uint_as_float(u);
+#else
+    float f;
+    memcpy(&f, &u, 4);
+    return f;
+#endif
+}
+LV_HD double wire_f64(const uint8_t* p) {
+    const uint64_t u = (uint64_t)wire_u32(p) | (uint64_t)wire_u32(p + 4) << 32;
+#if defined(__CUDA_ARCH__)
+    return __longlong_as_double((long long)u);
+#else
+    double d;
+    memcpy(&d, &u, 8);
+    return d;
+#endif
+}
+
+/* Utils.cpp:18-23: int arithmetic on the quotient and the remainder, as written (the int cast keeps the low 32 bits) */
+LV_HD double microsec2sec(uint64_t t) {
+    const int order = 1000000;
+    const int secs = (int)(t / (uint64_t)order);
+    const int musecs = (int)(t % (uint64_t)order);
+    return dadd((double)secs, dmul((double)musecs, 1e-6));
+}
+LV_HD double nanosec2sec(uint32_t t) {   /* Utils.cpp:25-30 */
+    const int order = 1000000000;
+    const int secs = (int)(t / (uint32_t)order);
+    const int nsecs = (int)(t % (uint32_t)order);
+    return dadd((double)secs, dmul((double)nsecs, 1e-9));
+}
+
+/* the point's own time field in seconds, before any offset */
+LV_HD double wire_raw_time(lv_lidar_type type, const lv_cloud_layout& L, const uint8_t* p) {
+    switch (type) {
+        case LV_LIDAR_VELODYNE: return (double)wire_f32(p + L.off_time);
+        case LV_LIDAR_OUSTER: return nanosec2sec(wire_u32(p + L.off_time));
+        default: return wire_f64(p + L.off_time);                          /* hesai, custom: absolute */
+    }
+}
+LV_HD bool wire_relative(lv_lidar_type type) { return type == LV_LIDAR_VELODYNE || type == LV_LIDAR_OUSTER; }
+
+/* get_begin_time (PointCloudProcessor.cpp:42-88), from the first and the last point of the whole message: relative stamps
+ * hang off the header stamp, absolute ones get 0 */
+LV_HD double wire_begin_time(lv_lidar_type type, const lv_cloud_layout& L, const uint8_t* data, int64_t n, uint64_t header_stamp_us,
+                             int stamp_beginning) {
+    if (!wire_relative(type) || n <= 0) return 0.0;
+    const double front = wire_raw_time(type, L, data), back = wire_raw_time(type, L, data + (uint64_t)(n - 1) * (uint64_t)L.point_step);
+    const double s = dadd(microsec2sec(header_stamp_us), front);
+    return stamp_beginning ? s : dsub(s, back);
+}
+/* absolute time of one point: Point.cpp:58-60,77-79 (full_rotation_time + t unless offset_beginning), then + begin */
+LV_HD double wire_time(lv_lidar_type type, const lv_cloud_layout& L, const uint8_t* p, int offset_beginning, double full_rotation_time,
+                       double begin) {
+    double t = wire_raw_time(type, L, p);
+    if (wire_relative(type) && !offset_beginning) t = dadd(full_rotation_time, t);
+    return dadd(t, begin);
+}
+
+LV_HD float wire_norm(float x, float y, float z) { return fsqrt(fadd(fadd(fmul(x, x), fmul(y, y)), fmul(z, z))); }
+LV_HD float wire_intensity(lv_lidar_type type, const lv_cloud_layout& L, const uint8_t* p) {
+    return type == LV_LIDAR_HESAI ? (float)wire_u8(p + L.off_intensity)
+         : type == LV_LIDAR_OUSTER ? (float)wire_u16(p + L.off_intensity)
+                                   : wire_f32(p + L.off_intensity);
+}
+/* Point.cpp:166-169: the driver's range for the ouster, |p| otherwise */
+LV_HD float wire_range(lv_lidar_type type, const lv_cloud_layout& L, const uint8_t* p, float x, float y, float z) {
+    return type == LV_LIDAR_OUSTER ? (float)wire_u32(p + L.off_range) : wire_norm(x, y, z);
+}
+
+/* temporal_downsample: keep point i (its index in the raw message) iff rate <= 1 or (i + 1) % rate == 0, and
+ * min_dist < |p| (a strict <, the double against the fp32 norm; a NaN coordinate drops the point) */
+LV_HD bool temporal_keep(int64_t i, int rate, double min_dist, float x, float y, float z) {
+    return (rate <= 1 || (i + 1) % rate == 0) && min_dist < (double)wire_norm(x, y, z);
+}
+
+/* the bounds pcl::fromROSMsg takes from the message itself: a LiDAR type this reader knows, every field that type reads
+ * inside point_step, and n points inside data_bytes.  NULL when the layout is usable, else what is wrong with it. */
+inline const char* cloud_layout_error(lv_lidar_type type, const lv_cloud_layout& L, int64_t n, int64_t data_bytes) {
+    if (type != LV_LIDAR_VELODYNE && type != LV_LIDAR_HESAI && type != LV_LIDAR_OUSTER && type != LV_LIDAR_CUSTOM) return "unknown LiDAR type";
+    if (n < 0 || data_bytes < 0) return "negative point count or data length";
+    if (L.point_step <= 0) return "point_step must be positive";
+    const int tsz = type == LV_LIDAR_VELODYNE ? 4 : (type == LV_LIDAR_OUSTER ? 4 : 8);
+    const int isz = type == LV_LIDAR_HESAI ? 1 : (type == LV_LIDAR_OUSTER ? 2 : 4);
+    const int32_t offs[6] = {L.off_x, L.off_y, L.off_z, L.off_intensity, L.off_time, type == LV_LIDAR_OUSTER ? L.off_range : 0};
+    const int32_t szs[6] = {4, 4, 4, isz, tsz, type == LV_LIDAR_OUSTER ? 4 : 0};
+    for (int k = 0; k < 6; ++k)
+        if (offs[k] < 0 || (int64_t)offs[k] + szs[k] > L.point_step) return "a field of the layout lies outside point_step";
+    if (n > data_bytes / L.point_step) return "data_bytes is too short for n points of point_step bytes";
+    return nullptr;
+}
+
+}  // namespace lv
+#endif

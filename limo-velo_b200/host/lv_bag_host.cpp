@@ -30,6 +30,7 @@
 #include <vector>
 
 #include "../../include/limovelo_b200.h"
+#include "../csrc/lv_wire.h"
 
 namespace {
 
@@ -283,19 +284,12 @@ lv_status lv_bag_parse_imu(const uint8_t* data, int64_t size, lv_imu_sample* out
     return r.ok ? LV_OK : LV_ERR_IO;
 }
 
-/* lv_pointcloud2_to_points with the bounds pcl::fromROSMsg gets from the message itself: every field used must lie inside
- * point_step and n points must fit data_bytes */
+/* lv_pointcloud2_to_points with the bounds pcl::fromROSMsg gets from the message itself (lv::cloud_layout_error, which
+ * lv_process_cloud_device applies as well) */
 lv_status lv_pointcloud2_to_points_checked(lv_lidar_type type, const lv_cloud_layout* L, const uint8_t* data, int64_t data_bytes, int64_t n,
                                            uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
                                            float* xyz, double* time, float* intensity, float* range) {
-    if (!L || !data || n < 0 || data_bytes < 0 || L->point_step <= 0) return LV_ERR_ARG;
-    const int tsz = type == LV_LIDAR_VELODYNE ? 4 : (type == LV_LIDAR_OUSTER ? 4 : 8);
-    const int isz = type == LV_LIDAR_HESAI ? 1 : (type == LV_LIDAR_OUSTER ? 2 : 4);
-    const int32_t offs[6] = {L->off_x, L->off_y, L->off_z, L->off_intensity, L->off_time, type == LV_LIDAR_OUSTER ? L->off_range : 0};
-    const int32_t szs[6] = {4, 4, 4, isz, tsz, type == LV_LIDAR_OUSTER ? 4 : 0};
-    for (int k = 0; k < 6; ++k)
-        if (offs[k] < 0 || offs[k] + szs[k] > L->point_step) return LV_ERR_ARG;
-    if ((uint64_t)n * (uint64_t)L->point_step > (uint64_t)data_bytes) return LV_ERR_ARG;
+    if (!L || !data || lv::cloud_layout_error(type, *L, n, data_bytes)) return LV_ERR_ARG;
     return lv_pointcloud2_to_points(type, L, data, n, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time, xyz, time,
                                     intensity, range);
 }

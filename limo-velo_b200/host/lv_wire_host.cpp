@@ -4,50 +4,14 @@
  *   Point(const <driver>::Point&, double time_offset)               src/Objects/Point.cpp:37-111,153-175
  *   Conversions::microsec2Sec / nanosec2Sec                         src/Utils/Utils.cpp:18-30
  *   PointCloudProcessor::sort_points                                src/Utils/PointCloudProcessor.cpp:114-123
- * One pass over the message bytes per sweep (a few MB); the decimator and everything after it run on the GPU
- * (lv_temporal_downsample, lv_compensate, lv_voxelgrid_downsample, lv_correct).
+ * One pass over the message bytes per sweep (a few MB); the per-point arithmetic is csrc/lv_wire.h, which
+ * lv_process_cloud_device (csrc/lv_cloud.cu) runs on the device.
  */
-#include <math.h>
-#include <string.h>
-
 #include <algorithm>
 #include <numeric>
-#include <vector>
 
 #include "../../include/limovelo_b200.h"
-#include "../csrc/lv_hd.h"
-
-namespace {
-
-template <class T>
-T rd(const uint8_t* p) {
-    T v;
-    memcpy(&v, p, sizeof(T));
-    return v;
-}
-/* Utils.cpp:18-23: int arithmetic on the quotient and the remainder, as written */
-double microsec2sec(uint64_t t) {
-    const int order = 1000000;
-    const int secs = (int)(t / (uint64_t)order);
-    const int musecs = (int)(t % (uint64_t)order);
-    return secs + musecs * 1e-6;
-}
-double nanosec2sec(uint32_t t) {   /* Utils.cpp:25-30 */
-    const int order = 1000000000;
-    const int secs = (int)(t / (uint32_t)order);
-    const int nsecs = (int)(t % (uint32_t)order);
-    return secs + nsecs * 1e-9;
-}
-/* the point's own time field in seconds, before any offset */
-double raw_time(lv_lidar_type type, const lv_cloud_layout& L, const uint8_t* p) {
-    switch (type) {
-        case LV_LIDAR_VELODYNE: return (double)rd<float>(p + L.off_time);
-        case LV_LIDAR_OUSTER: return nanosec2sec(rd<uint32_t>(p + L.off_time));
-        default: return rd<double>(p + L.off_time);                         /* hesai, custom: absolute */
-    }
-}
-
-}  // namespace
+#include "../csrc/lv_wire.h"
 
 extern "C" {
 
@@ -58,29 +22,14 @@ lv_status lv_pointcloud2_to_points(lv_lidar_type type, const lv_cloud_layout* la
     if (type != LV_LIDAR_VELODYNE && type != LV_LIDAR_HESAI && type != LV_LIDAR_OUSTER && type != LV_LIDAR_CUSTOM) return LV_ERR_ARG;
     if (n == 0) return LV_OK;
     const lv_cloud_layout& L = *layout;
-    const bool relative = type == LV_LIDAR_VELODYNE || type == LV_LIDAR_OUSTER;
-    /* get_begin_time (PointCloudProcessor.cpp:42-88): relative stamps hang off the header stamp */
-    double begin = 0.0;
-    if (relative) {
-        const double front = raw_time(type, L, data), back = raw_time(type, L, data + (size_t)(n - 1) * L.point_step);
-        begin = stamp_beginning ? microsec2sec(header_stamp_us) + front : microsec2sec(header_stamp_us) + front - back;
-    }
+    const double begin = lv::wire_begin_time(type, L, data, n, header_stamp_us, stamp_beginning);
     for (int64_t i = 0; i < n; ++i) {
         const uint8_t* p = data + (size_t)i * L.point_step;
-        const float x = rd<float>(p + L.off_x), y = rd<float>(p + L.off_y), z = rd<float>(p + L.off_z);
+        const float x = lv::wire_f32(p + L.off_x), y = lv::wire_f32(p + L.off_y), z = lv::wire_f32(p + L.off_z);
         xyz[3 * i] = x; xyz[3 * i + 1] = y; xyz[3 * i + 2] = z;
-        double t = raw_time(type, L, p);
-        if (relative && !offset_beginning) t = full_rotation_time + t;            /* Point.cpp:58-60,77-79 */
-        time[i] = t + begin;                                                     /* Point(p, time_offset) */
-        if (intensity) {
-            intensity[i] = type == LV_LIDAR_HESAI ? (float)rd<uint8_t>(p + L.off_intensity)
-                         : type == LV_LIDAR_OUSTER ? (float)rd<uint16_t>(p + L.off_intensity)
-                                                   : rd<float>(p + L.off_intensity);
-        }
-        if (range) {
-            range[i] = type == LV_LIDAR_OUSTER ? (float)rd<uint32_t>(p + L.off_range)
-                                               : lv::fsqrt(lv::fadd(lv::fadd(lv::fmul(x, x), lv::fmul(y, y)), lv::fmul(z, z)));
-        }
+        time[i] = lv::wire_time(type, L, p, offset_beginning, full_rotation_time, begin);
+        if (intensity) intensity[i] = lv::wire_intensity(type, L, p);
+        if (range) range[i] = lv::wire_range(type, L, p, x, y, z);
     }
     return LV_OK;
 }

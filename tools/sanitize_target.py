@@ -1,5 +1,6 @@
 """What compute-sanitizer runs (tools/gpu_sanitize.sh): every kernel of the path once or twice on a small scene, checked against
-the oracle so that a sanitizer-induced slowdown cannot hide a wrong result.  Both search paths, the map update, the device tick."""
+the oracle so that a sanitizer-induced slowdown cannot hide a wrong result.  Both search paths, the map update, the device tick,
+the message front end."""
 import os
 import sys
 import numpy as np
@@ -44,3 +45,16 @@ for group in VARIANTS:
         loc.propagate_device(np.tile([0.0, 0.0, 9.8], (4, 1)), np.zeros((4, 3)), np.full(4, 1e-3))
     loc.close()
     print("sanitize target: search group %s ok" % (group or "default"), flush=True)
+
+# the message front end (lv_process_cloud_device): velodyne / ouster bytes at an odd device address, against the host composition
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+import test_gpu_cloud_frontend as T
+from test_wire_format import make_cloud
+loc = lv.Localizer(lv.default_params(max_points=1 << 13, max_map_points=1 << 13))
+rng = np.random.default_rng(3)
+for lidar in ("velodyne", "ouster"):
+    pts = make_cloud(lidar, 3000, rng)[rng.permutation(3000)]
+    T.assert_same(T.device_process(lv, loc, lidar, pts, T.STAMP_US, False, True, 0.1, 4, 3.0, shift=1),
+                  T.host_process(lv, lidar, pts, T.STAMP_US, False, True, 0.1, 4, 3.0), lidar)
+loc.close()
+print("sanitize target: process cloud ok", flush=True)
