@@ -41,7 +41,8 @@ typedef enum lv_status {
     LV_ERR_ARG = 3,
     LV_ERR_CUDA = 4,           /* no device / CUDA failure (see lv_last_error)                */
     LV_ERR_CAPACITY = 5,       /* more points than the handle was created for                 */
-    LV_ERR_IO = 6              /* YAML file unreadable                                        */
+    LV_ERR_IO = 6,             /* YAML file unreadable                                        */
+    LV_TOO_FEW_POINTS = 7      /* main.cpp:81: fewer points than MAX_POINTS2MATCH, no update (lv_correct_device_async) */
 } lv_status;
 
 /*
@@ -253,7 +254,8 @@ lv_status lv_correct(lv_handle h, const float* xyz_lidar, int64_t n, double time
  * and records the sweep for lv_map_add_last_sweep, like lv_correct.                          */
 lv_status lv_correct_device(lv_handle h, const float* d_xyz_lidar, int64_t n, double time);
 lv_status lv_last_logs(lv_handle h, lv_iter_log* logs, int32_t* n_evals);
-double lv_last_time_updated(lv_handle h);                     /* Localizator::last_time_updated */
+/* Localizator::last_time_updated; synchronises when an lv_correct_device_async is still to be resolved */
+double lv_last_time_updated(lv_handle h);
 
 /* ---- utilities --------------------------------------------------------------------------- */
 void* lv_host_alloc(int64_t bytes);                           /* pinned host memory            */
@@ -362,6 +364,47 @@ lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_clou
                                   int32_t downsample_rate, double min_dist,
                                   float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
                                   int64_t* n_out);
+
+/* ---- the tick without a host wait (main.cpp:76-105) ------------------------------------------------------------------------
+ * Stream-ordered forms of the tick's device calls.  Each takes its input count from DEVICE memory (d_n, an int64_t) and writes
+ * its output count to device memory (d_n_out), so that one stage hands its count to the next without the host: none of them
+ * synchronises.  n_max is a host-known upper bound of the count (the message's n, or max_points) in [1, min(max_points,
+ * 2^31 - 1)]: it sizes the grids and the sorts, which run over n_max slots with padding keys that sort last.  A device count
+ * outside [0, n_max] is clamped to it and flagged.  Errors found on the device are not returned: they are recorded and
+ * reported (and cleared) by lv_async_status, which names the stage.  Argument errors are LV_ERR_ARG before any device work.
+ * Each call's results equal those of its synchronous form bit for bit (counts, values, order). */
+/* Accumulator::process (Accumulator.cpp:142-151) as lv_process_cloud_device; *d_n_out = points kept.  A kept point whose time
+ * is NaN is a deferred error.  The output buffers have room for n points. */
+lv_status lv_process_cloud_device_async(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout,
+                                        const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t header_stamp_us,
+                                        int stamp_beginning, int offset_beginning, double full_rotation_time,
+                                        int32_t downsample_rate, double min_dist,
+                                        float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
+                                        int64_t* d_n_out);
+/* Compensator::compensate (Compensator.cpp:123-146) as lv_compensate_device over *d_n points.  The path and Xt2 stay host-built
+ * (Compensator::upsample / get_t2); they are staged through pinned memory, so the host buffers may be reused on return.  A
+ * timestamp outside the path (or out of order) is a deferred error.  d_xyz_out may equal d_xyz; other overlaps of the
+ * n_max-point ranges of d_xyz, d_t and d_xyz_out are refused. */
+lv_status lv_compensate_device_async(lv_handle h, const lv_state32* path, int32_t ns, const lv_state32* Xt2, const float* d_xyz,
+                                     const double* d_t, const int64_t* d_n, int64_t n_max, float* d_xyz_out);
+/* Compensator::downsample -> voxelgrid_downsample (Compensator.cpp:115-118,148-163) as lv_voxelgrid_downsample_device over *d_n
+ * points; *d_n_out = leaves.  PCL's cell-index overflow pass-through (d_xyz_out = the input, *d_n_out = *d_n) is decided on the
+ * device.  The n_max-point ranges of d_xyz and d_xyz_out must not overlap. */
+lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max,
+                                               float downsample_prec, float* d_xyz_out, int64_t* d_n_out);
+/* main.cpp:81-88: `if (ds_compensated.size() < MAX_POINTS2MATCH) break; localizator.correct(ds_compensated, t2)` on *d_n points of
+ * d_xyz (device, LiDAR frame).  Below max(min_points, 1) points the update does not run: state, P and last_time_updated are left
+ * as they are and the status lv_last_logs fetches is LV_TOO_FEW_POINTS.  On a map the host knows to be empty it returns
+ * LV_EMPTY_MAP at once, like lv_correct_device; after an asynchronous first build (which the gate may have left empty) the device
+ * checks the map's point count and records LV_EMPTY_MAP the same way (Localizator.cpp:24).  last_time_updated becomes `time` when
+ * the update runs, resolved by the next call that fetches the results (lv_last_logs, lv_get_state, ...).  The sweep and its
+ * device count are recorded for lv_map_add_last_sweep, which then adds *d_n points, or none when the gate stopped the tick
+ * (main.cpp:81 breaks before map.add), the first tick's build included; its growth bound (lv_map_set_growth) uses n_max. */
+lv_status lv_correct_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int64_t min_points,
+                                  double time);
+/* the deferred errors of the _async calls since the last lv_async_status, and the map's capacity flags (as lv_map_status):
+ * LV_ERR_ARG (lv_last_error names the stage), LV_ERR_CAPACITY or LV_OK.  Clears them; the handle stays usable.  Synchronises. */
+lv_status lv_async_status(lv_handle h);
 
 /* ---- rosbag reader (format 2.0; replaces roscpp / `rosbag play` in front of Accumulator::receive_lidar / receive_imu,
  * src/main.cpp:27-39, src/Modules/Accumulator.cpp:39-60).  Sequential read of uncompressed bags (bz2 / lz4 chunks are

@@ -19,9 +19,9 @@ LIB_PATH = os.environ.get("LV_LIB_PATH") or os.path.join(_HERE, "liblimovelo_b20
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "limovelo_b200.h")
 
 STATE_LEN, DOF, MAX_EVALS = 26, 23, 8
-OK, EMPTY_MAP, TOO_FEW_MATCHES, ERR_ARG, ERR_CUDA, ERR_CAPACITY, ERR_IO = range(7)
+OK, EMPTY_MAP, TOO_FEW_MATCHES, ERR_ARG, ERR_CUDA, ERR_CAPACITY, ERR_IO, TOO_FEW_POINTS = range(8)
 STATUS_NAMES = ["LV_OK", "LV_EMPTY_MAP", "LV_TOO_FEW_MATCHES", "LV_ERR_ARG", "LV_ERR_CUDA", "LV_ERR_CAPACITY",
-                "LV_ERR_IO"]
+                "LV_ERR_IO", "LV_TOO_FEW_POINTS"]
 
 
 class Params(C.Structure):
@@ -136,6 +136,13 @@ def lib():
     L.lv_memcpy_d2h.argtypes = [vp, vp, vp, i64]
     L.lv_process_cloud_device.argtypes = [vp, C.c_int, C.POINTER(CloudLayout), vp, i64, i64, C.c_uint64, C.c_int, C.c_int,
                                           C.c_double, C.c_int32, C.c_double, vp, vp, vp, vp, vp, C.POINTER(i64)]
+    if hasattr(L, "lv_async_status"):   # the stream-ordered tick; absent from older builds that tools/ab_bench.py may load
+        L.lv_process_cloud_device_async.argtypes = [vp, C.c_int, C.POINTER(CloudLayout), vp, i64, i64, C.c_uint64, C.c_int, C.c_int,
+                                                    C.c_double, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
+        L.lv_compensate_device_async.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, i64, vp]
+        L.lv_voxelgrid_downsample_device_async.argtypes = [vp, vp, vp, i64, C.c_float, vp, vp]
+        L.lv_correct_device_async.argtypes = [vp, vp, vp, i64, i64, C.c_double]
+        L.lv_async_status.argtypes = [vp]
     L.lv_synchronize.argtypes = [vp]
     L.lv_profile_enable.argtypes = [vp, C.c_int]
     L.lv_profile_get.argtypes = [vp, C.POINTER(Profile), C.c_int]
@@ -569,13 +576,49 @@ class Localizer:
     def correct_device(self, d_ptr, n, time=0.0):
         return _check(self.L.lv_correct_device(self.h, d_ptr, n, float(time)), allow=(EMPTY_MAP,))
 
+    # the tick without a host wait: counts live in device memory (int64 at d_n / d_n_out), nothing synchronises
+    def process_cloud_device_async(self, lidar, layout, d_data, data_bytes, n, header_stamp_us, stamp_beginning, offset_beginning,
+                                   full_rotation_time, downsample_rate, min_dist, d_xyz, d_time, d_n_out, d_intensity=None,
+                                   d_range=None, d_idx=None):
+        """lv_process_cloud_device with the count of kept points written to d_n_out"""
+        return _check(self.L.lv_process_cloud_device_async(
+            self.h, LIDAR_TYPES[lidar], C.byref(layout), C.c_void_p(d_data), int(data_bytes), int(n), int(header_stamp_us),
+            int(stamp_beginning), int(offset_beginning), float(full_rotation_time), int(downsample_rate), float(min_dist),
+            C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
+            C.c_void_p(d_n_out)))
+
+    def compensate_device_async(self, path, Xt2, d_xyz, d_t, d_n, n_max, d_out):
+        """lv_compensate_device over the *d_n points"""
+        arr = (State32 * len(path))(*path)
+        return _check(self.L.lv_compensate_device_async(self.h, arr, len(path), C.byref(Xt2), C.c_void_p(d_xyz), C.c_void_p(d_t),
+                                                        C.c_void_p(d_n), int(n_max), C.c_void_p(d_out)))
+
+    def voxelgrid_downsample_device_async(self, d_xyz, d_n, n_max, leaf, d_out, d_n_out):
+        """lv_voxelgrid_downsample_device over the *d_n points; the leaf count goes to d_n_out"""
+        return _check(self.L.lv_voxelgrid_downsample_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_n), int(n_max), C.c_float(leaf),
+                                                                  C.c_void_p(d_out), C.c_void_p(d_n_out)))
+
+    def correct_device_async(self, d_ptr, d_n, n_max, min_points, time=0.0):
+        """Localizator::correct on the *d_n points behind main.cpp:81's MAX_POINTS2MATCH gate; LV_EMPTY_MAP while the host knows the
+        map is empty, else LV_OK (the update's own status is fetched later, e.g. by last_logs)"""
+        return _check(self.L.lv_correct_device_async(self.h, C.c_void_p(d_ptr), C.c_void_p(d_n), int(n_max), int(min_points),
+                                                     float(time)), allow=(EMPTY_MAP,))
+
+    def async_status(self):
+        """the deferred errors of the async calls (cleared by the call): returns (status, lv_last_error text); synchronises"""
+        st = self.L.lv_async_status(self.h)
+        return st, (self.L.lv_last_error().decode() if st != OK else "")
+
+    def last_time_updated(self):
+        return float(self.L.lv_last_time_updated(self.h))
+
     def result_bytes(self):
         return int(self.L.lv_result_bytes())
 
     def last_logs(self):
         logs = (IterLog * MAX_EVALS)()
         ne = C.c_int32(0)
-        st = _check(self.L.lv_last_logs(self.h, logs, C.byref(ne)), allow=(TOO_FEW_MATCHES,))
+        st = _check(self.L.lv_last_logs(self.h, logs, C.byref(ne)), allow=(TOO_FEW_MATCHES, TOO_FEW_POINTS, EMPTY_MAP))
         return st, _logs_to_py(logs, ne.value)
 
     # utilities

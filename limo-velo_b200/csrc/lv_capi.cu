@@ -69,6 +69,14 @@ struct lv_context {
     cudaEvent_t ctrl_copied = nullptr;
     int64_t last_sweep_n = 0;          /* points of the sweep d_sweep holds (lv_correct / lv_measure*), for lv_map_add_last_sweep */
     const float* last_sweep = nullptr; /* device pointer of the sweep of the last update */
+    const int64_t* last_sweep_dn = nullptr;   /* lv_correct_device_async: its device count (last_sweep_n is then the bound) ... */
+    int64_t last_sweep_min = 0;               /* ... and its min_points */
+    /* the async tick: deferred errors and the time of the last update that ran (lv_correct_device_async) */
+    AsyncWords* d_async = nullptr;
+    AsyncWords* h_async = nullptr;     /* pinned */
+    bool time_pending = false;         /* last_time_updated waits for the device's decision (next fetch) */
+    bool map_unknown = false;          /* an async add may have left the map without points: the device checks it */
+    cudaEvent_t path_copied = nullptr; /* the last H2D copy out of h_path (lv_compensate_device_async returns before it runs) */
     bool use_reuse = true;
     bool use_pdl = true;               /* programmatic dependent launch between the kernels of an update */
     /* Compensator (deskew) staging: lazily allocated */
@@ -295,6 +303,10 @@ lv_status lv_create(const lv_params* p, lv_handle* out) {
     LV_CREATE_CUDA(cudaMallocHost(&h->h_ctrl, sizeof(UpdateCtrl)));
     LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->imu_copied, cudaEventDisableTiming));
     LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->ctrl_copied, cudaEventDisableTiming));
+    LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->path_copied, cudaEventDisableTiming));
+    LV_CREATE_CUDA(cudaMalloc(&h->d_async, sizeof(AsyncWords)));
+    LV_CREATE_CUDA(cudaMemset(h->d_async, 0, sizeof(AsyncWords)));
+    LV_CREATE_CUDA(cudaMallocHost(&h->h_async, sizeof(AsyncWords)));
     LV_CREATE_CUDA(cudaMalloc(&h->d_partials, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
     LV_CREATE_CUDA(cudaMemset(h->d_partials, 0, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
     LV_CREATE_CUDA(cudaMalloc(&h->d_group_rows, sizeof(double) * kPartialStride * 32));
@@ -322,6 +334,8 @@ void lv_destroy(lv_handle h) {
     for (auto& u : h->graphs) { cudaGraphExecDestroy(u.exec); cudaGraphDestroy(u.graph); }
     if (h->imu_copied) cudaEventDestroy(h->imu_copied);
     if (h->ctrl_copied) cudaEventDestroy(h->ctrl_copied);
+    if (h->path_copied) cudaEventDestroy(h->path_copied);
+    cudaFree(h->d_async); cudaFreeHost(h->h_async);
     for (cudaEvent_t e : h->snap_ev) if (e) cudaEventDestroy(e);
     cudaFreeHost(h->h_snap);
     cudaFree(h->d_job); cudaFree(h->d_ref); cudaFree(h->d_redo); cudaFree(h->d_imu); cudaFreeHost(h->h_imu);
@@ -607,7 +621,8 @@ lv_status lv_map_add_device(lv_handle h, const float* d_xyz, int64_t n, int down
 
 /* ---- the tick on the device: main.cpp:99-105 ------------------------------------------------- */
 static lv_status upload_state(lv_context* h, const double* x, const double* P);
-static lv_status add_sweep_impl(lv_context* h, const float* d_xyz_lidar, int64_t n, int downsample) {
+/* n: the sweep's points, or with cnt.n the host bound of its device count */
+static lv_status add_sweep_impl(lv_context* h, const float* d_xyz_lidar, int64_t n, int downsample, const MapAddCount& cnt = MapAddCount()) {
     if (h->state_dirty) {                                         /* the transform uses the device copy of the state */
         lv_status s = upload_state(h, h->x, h->P);
         if (s != LV_OK) return s;
@@ -619,7 +634,8 @@ static lv_status add_sweep_impl(lv_context* h, const float* d_xyz_lidar, int64_t
     EventPair ep;
     const bool pr = prof_begin(h, 2, &ep);
     int launches = 0;
-    LV_CUDA(map_add_sweep(h->map, h->d_ctrl, d_xyz_lidar, n, downsample ? 1 : 0, h->stream, &launches));
+    if (cnt.n && h->map.empty) h->map_unknown = true;             /* the gate may leave the build without a point */
+    LV_CUDA(map_add_sweep(h->map, h->d_ctrl, d_xyz_lidar, n, downsample ? 1 : 0, h->stream, &launches, cnt));
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
     return snap_after_add(h, n);
@@ -635,7 +651,15 @@ lv_status lv_map_add_last_sweep(lv_handle h, int downsample) {
     if (!h) return LV_ERR_ARG;
     if (!h->last_sweep || h->last_sweep_n <= 0) { set_error("no sweep has been corrected yet"); return LV_ERR_ARG; }
     LV_CUDA(cudaSetDevice(h->prm.device));
-    return add_sweep_impl(h, h->last_sweep, h->last_sweep_n, downsample);
+    if (!h->last_sweep_dn) return add_sweep_impl(h, h->last_sweep, h->last_sweep_n, downsample);
+    /* after lv_correct_device_async: *d_n points, none when its gate stopped the tick; a map that an earlier gated build left
+     * without points is built (the reference's map does not exist yet, Mapper.cpp:26) */
+    MapAddCount cnt;
+    cnt.n = h->last_sweep_dn;
+    cnt.min_points = h->last_sweep_min;
+    cnt.build_if_empty = 1;
+    cnt.err = &h->d_async->err;
+    return add_sweep_impl(h, h->last_sweep, h->last_sweep_n, downsample, cnt);
 }
 
 /* ---- state ----------------------------------------------------------------------------------- */
@@ -709,7 +733,11 @@ lv_status lv_propagate_device(lv_handle h, const double* acc, const double* gyro
     h->pending_fetch = true;                                      /* the device now holds the newest (x, P) */
     return LV_OK;
 }
-double lv_last_time_updated(lv_handle h) { return h ? h->last_time_updated : -1; }
+double lv_last_time_updated(lv_handle h) {
+    if (!h) return -1;
+    if (h->time_pending) sync_mirror(h);                          /* an async update's time is known once its results are */
+    return h->last_time_updated;
+}
 
 static lv_status upload_state(lv_context* h, const double* x, const double* P) {
     /* x, P are staged through the pinned mirror so the copy is truly asynchronous; an earlier upload may still be queued
@@ -753,13 +781,14 @@ static MeasureArgs update_measure_args(lv_context* h, const float* d_xyz, int64_
     return a;
 }
 
-/* enqueue begin + all evaluations on h->stream; with `job` the sweep comes from device memory (graph capture) */
-static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64_t n, bool as_job);
+/* enqueue begin + all evaluations on h->stream; with `as_job` the sweep comes from device memory (graph capture, or a count
+ * in device memory), `capture`: inside a stream capture */
+static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64_t n, bool as_job, bool capture, const UpdateGate& gate);
 
 static lv_status build_update_graph(lv_context* h, int64_t cap, lv_context::UpdateGraph* out) {
     cudaGraph_t graph = nullptr;
     LV_CUDA(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-    lv_status s = enqueue_update_kernels(h, nullptr, cap, true);
+    lv_status s = enqueue_update_kernels(h, nullptr, cap, true, true, UpdateGate());
     cudaError_t e = cudaStreamEndCapture(h->stream, &graph);
     if (s != LV_OK || e != cudaSuccess) {
         if (graph) cudaGraphDestroy(graph);
@@ -788,13 +817,15 @@ static lv_status build_update_graph(lv_context* h, int64_t cap, lv_context::Upda
     return LV_OK;
 }
 
-static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n) {
+/* n: the sweep's points, or with gate.n the host bound of its device count (the graph bucket is chosen by it) */
+static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n, UpdateGate gate = UpdateGate()) {
     if (h->state_dirty) {
         lv_status s = upload_state(h, h->x, h->P);
         if (s != LV_OK) return s;
         h->state_dirty = false;
     }
-    if (h->profile || !h->use_graph) return enqueue_update_kernels(h, d_xyz, n, false);
+    if (h->map_unknown) gate.map_counters = h->map.counters;     /* an async build may have added nothing */
+    if (h->profile || !h->use_graph) return enqueue_update_kernels(h, d_xyz, n, gate.n != nullptr, false, gate);
     int64_t cap = 4096;
     while (cap < n) cap <<= 1;
     if (cap > h->prm.max_points) cap = h->prm.max_points;
@@ -811,7 +842,7 @@ static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n) {
     MeasureJob* job = h->d_job;
     int n32 = (int)n;
     uint32_t* counters = h->d_hard_list + (size_t)kHardBuckets * hard_segment(h->prm.max_points);
-    void* args[5] = {&c, &job, &d_xyz, &n32, &counters};
+    void* args[6] = {&c, &job, &d_xyz, &n32, &counters, &gate};
     cudaKernelNodeParams kp = {};
     kp.func = const_cast<void*>(ieskf_begin_kernel_ptr());
     kp.gridDim = dim3(1, 1, 1);
@@ -823,22 +854,22 @@ static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n) {
     return LV_OK;
 }
 
-static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64_t n, bool as_job) {
+static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64_t n, bool as_job, bool capture, const UpdateGate& gate) {
     const int pdl = (h->use_pdl && !h->profile) ? 1 : 0;
     uint32_t* counters = h->d_hard_list + (size_t)kHardBuckets * hard_segment(h->prm.max_points);
-    LV_CUDA(launch_ieskf_begin(h->d_ctrl, as_job ? h->d_job : nullptr, d_xyz, (int)n, counters, h->stream));
-    if (!as_job) h->prof.total_launches += 1;
+    LV_CUDA(launch_ieskf_begin(h->d_ctrl, as_job ? h->d_job : nullptr, d_xyz, (int)n, counters, gate, h->stream));
+    if (!capture) h->prof.total_launches += 1;
     MeasureArgs a = update_measure_args(h, d_xyz, n, as_job);
     const int grid = measure_grid((int)n);
     for (int e = 0; e <= h->prm.MAX_NUM_ITERS; ++e) {            /* i = -1 .. max_iter-1, esekfom.hpp:1634 */
         EventPair ep;
         bool pr;
-        LV_CUDA(launch_measure_timed(h, a, grid, as_job ? 0 : 1, e /* evaluation index: > 0 = reuse + work list */, (int)(h->update_seq % kNevalsRing), e, pdl));
+        LV_CUDA(launch_measure_timed(h, a, grid, capture ? 0 : 1, e /* evaluation index: > 0 = reuse + work list */, (int)(h->update_seq % kNevalsRing), e, pdl));
         pr = prof_begin(h, 1, &ep);
         ep.upd = (int)(h->update_seq % kNevalsRing); ep.slot = e;
         LV_CUDA(launch_ieskf_step(h->d_ctrl, h->iprm, h->d_group_rows, partial_groups(grid), h->stream, pdl));
         if (pr) prof_end(h, &ep);
-        if (!as_job) h->prof.total_launches += 4 + ((e > 0 && h->use_reuse) ? 1 : 0);
+        if (!capture) h->prof.total_launches += 4 + ((e > 0 && h->use_reuse) ? 1 : 0);
     }
     if (h->profile) {
         LV_CUDA(cudaMemcpyAsync(&h->h_nevals[h->update_seq % kNevalsRing], &h->d_ctrl->n_evals, sizeof(int32_t),
@@ -851,10 +882,24 @@ static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64
 static lv_status fetch_results(lv_context* h) {
     LV_CUDA(cudaMemcpyAsync(h->h_ctrl, h->d_ctrl, sizeof(UpdateCtrl), cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(map_fetch_counters(h->map, h->stream));       /* 64 bytes: the map's error flags ride along */
+    if (h->time_pending) {                                /* what the async updates decided about last_time_updated */
+        LV_CUDA(cudaMemcpyAsync(h->h_async, h->d_async, sizeof(AsyncWords), cudaMemcpyDeviceToHost, h->stream));
+        LV_CUDA(cudaMemsetAsync(&h->d_async->time_set, 0, sizeof(int32_t), h->stream));
+    }
     LV_CUDA(cudaStreamSynchronize(h->stream));
+    if (h->time_pending) {
+        if (h->h_async->time_set) h->last_time_updated = h->h_async->time_updated;
+        h->time_pending = false;
+    }
+    if (h->map_unknown) {                                 /* the gate left the async build without a point: no map yet */
+        if ((int32_t)h->map.h_counters[kCtrPoints] == 0) h->map.empty = true;
+        h->map_unknown = false;
+    }
     const UpdateCtrl* c = h->h_ctrl;
     memcpy(h->x, c->x, sizeof(h->x));
-    if (c->status == LV_OK) memcpy(h->P, c->P, sizeof(h->P));
+    /* a gated update (LV_TOO_FEW_POINTS, or LV_EMPTY_MAP found on the device) leaves P as it was on the device, which may be
+     * newer than the mirror (lv_propagate_device) */
+    if (c->status == LV_OK || c->status == LV_TOO_FEW_POINTS || c->status == LV_EMPTY_MAP) memcpy(h->P, c->P, sizeof(h->P));
     h->n_evals = c->n_evals;
     memcpy(h->logs, c->logs, sizeof(h->logs));
     h->last_status = c->status;
@@ -872,12 +917,12 @@ lv_status lv_correct(lv_handle h, const float* xyz, int64_t n, double time, lv_i
     LV_CUDA(cudaSetDevice(h->prm.device));
     /* the sweep is uploaded and recorded even on an empty map: the first tick's lv_map_add_last_sweep builds the map from it */
     LV_CUDA(cudaMemcpyAsync(h->d_sweep, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
-    h->last_sweep = h->d_sweep; h->last_sweep_n = n;
+    h->last_sweep = h->d_sweep; h->last_sweep_n = n; h->last_sweep_dn = nullptr;
     if (h->map.empty) return LV_EMPTY_MAP;                       /* Localizator.cpp:24: the state is left as it is */
     lv_status s = enqueue_update(h, h->d_sweep, n);
     if (s != LV_OK) return s;
     s = fetch_results(h);
-    h->last_time_updated = time;                                  /* Localizator.cpp:26 */
+    if (s != LV_EMPTY_MAP) h->last_time_updated = time;          /* Localizator.cpp:26 (LV_EMPTY_MAP: an async build added nothing) */
     if (logs) memcpy(logs, h->logs, sizeof(lv_iter_log) * (size_t)h->n_evals);
     if (n_evals) *n_evals = h->n_evals;
     if (x_out) memcpy(x_out, h->x, sizeof(h->x));
@@ -887,11 +932,40 @@ lv_status lv_correct(lv_handle h, const float* xyz, int64_t n, double time, lv_i
 
 lv_status lv_correct_device(lv_handle h, const float* d_xyz, int64_t n, double time) {
     if (!h || !d_xyz || n <= 0) return LV_ERR_ARG;
-    h->last_sweep = d_xyz; h->last_sweep_n = n;                   /* recorded on an empty map too (see lv_correct) */
+    h->last_sweep = d_xyz; h->last_sweep_n = n; h->last_sweep_dn = nullptr;   /* recorded on an empty map too (see lv_correct) */
     if (h->map.empty) return LV_EMPTY_MAP;
     LV_CUDA(cudaSetDevice(h->prm.device));
-    lv_status s = enqueue_update(h, d_xyz, n);
-    h->last_time_updated = time;
+    UpdateGate gate;
+    if (h->map_unknown) {                                         /* whether the update runs is the device's decision */
+        gate.words = h->d_async;
+        gate.time = time;
+    } else if (h->time_pending) {                                 /* this time supersedes what an earlier async update recorded */
+        LV_CUDA(cudaMemsetAsync(&h->d_async->time_set, 0, sizeof(int32_t), h->stream));
+    }
+    lv_status s = enqueue_update(h, d_xyz, n, gate);
+    h->time_pending = h->map_unknown;
+    if (!h->map_unknown) h->last_time_updated = time;
+    h->pending_fetch = true;
+    return s;
+}
+
+lv_status lv_correct_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int64_t min_points, double time) {
+    if (!d_xyz || !d_n) { set_error("correct async: null sweep or count"); return LV_ERR_ARG; }
+    if (n_max < 1 || n_max > 0x7fffffff) { set_error("correct async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (min_points < 0) { set_error("correct async: negative min_points"); return LV_ERR_ARG; }
+    if (!h) { set_error("correct async: null handle"); return LV_ERR_ARG; }
+    if (n_max > h->prm.max_points) { set_error("correct async: n_max above max_points"); return LV_ERR_ARG; }
+    /* recorded on an empty map too: lv_map_add_last_sweep builds the map from *d_n points unless the gate stops the tick */
+    h->last_sweep = d_xyz; h->last_sweep_n = n_max; h->last_sweep_dn = d_n; h->last_sweep_min = min_points;
+    if (h->map.empty) return LV_EMPTY_MAP;                        /* Localizator.cpp:24 */
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    UpdateGate gate;
+    gate.n = d_n;
+    gate.min_points = min_points;
+    gate.words = h->d_async;
+    gate.time = time;
+    lv_status s = enqueue_update(h, d_xyz, n_max, gate);
+    h->time_pending = true;
     h->pending_fetch = true;
     return s;
 }
@@ -1043,18 +1117,23 @@ lv_status lv_memcpy_d2h(lv_handle h, void* dst, const void* src, int64_t bytes) 
     return LV_OK;
 }
 /* ---- Compensator::compensate ------------------------------------------------------------------ */
+/* d_n: NULL (n points, the flag is read back into h_bad) or the device count of the async form (n is its bound) */
 static lv_status deskew_common(lv_context* h, const lv_state32* path, int32_t ns, const lv_state32* Xt2,
-                               const float* d_xyz, const double* d_t, int64_t n, float* d_out) {
+                               const float* d_xyz, const double* d_t, const int64_t* d_n, int64_t n, float* d_out) {
     if (!h->d_path) {
         LV_CUDA(cudaMalloc(&h->d_path, sizeof(lv_state32) * deskew_max_states()));
         LV_CUDA(cudaMallocHost(&h->h_path, sizeof(lv_state32) * deskew_max_states()));
         LV_CUDA(cudaMalloc(&h->d_bad, sizeof(int)));
         LV_CUDA(cudaMallocHost(&h->h_bad, sizeof(int)));
     }
+    /* the pinned staging buffer is reused: the copy out of it queued by an earlier async call must have run */
+    LV_CUDA(cudaEventSynchronize(h->path_copied));
     memcpy(h->h_path, path, sizeof(lv_state32) * (size_t)ns);
     LV_CUDA(cudaMemcpyAsync(h->d_path, h->h_path, sizeof(lv_state32) * (size_t)ns, cudaMemcpyHostToDevice, h->stream));
-    LV_CUDA(launch_deskew(h->d_path, ns, *Xt2, path[0].time, path[ns - 1].time, d_xyz, d_t, n, d_out, h->d_bad, h->stream));
-    LV_CUDA(cudaMemcpyAsync(h->h_bad, h->d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaEventRecord(h->path_copied, h->stream));
+    LV_CUDA(launch_deskew(h->d_path, ns, *Xt2, path[0].time, path[ns - 1].time, d_xyz, d_t, d_n, n, d_out, h->d_bad,
+                          d_n ? &h->d_async->err : nullptr, h->stream));
+    if (!d_n) LV_CUDA(cudaMemcpyAsync(h->h_bad, h->d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     h->prof.total_launches += 2;
     return LV_OK;
 }
@@ -1072,11 +1151,31 @@ lv_status lv_compensate_device(lv_handle h, const lv_state32* path, int32_t ns, 
     lv_status s = deskew_args_ok(h, path, ns, Xt2, d_xyz, d_t, n, d_xyz_out);
     if (s != LV_OK) return s;
     LV_CUDA(cudaSetDevice(h->prm.device));
-    s = deskew_common(h, path, ns, Xt2, d_xyz, d_t, n, d_xyz_out);
+    s = deskew_common(h, path, ns, Xt2, d_xyz, d_t, nullptr, n, d_xyz_out);
     if (s != LV_OK) return s;
     LV_CUDA(cudaStreamSynchronize(h->stream));
     if (*h->h_bad) { set_error("deskew: a timestamp lies outside the path or the points are not time-sorted"); return LV_ERR_ARG; }
     return LV_OK;
+}
+static bool ranges_overlap(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes) {
+    return (uintptr_t)a < (uintptr_t)b + (uintptr_t)b_bytes && (uintptr_t)b < (uintptr_t)a + (uintptr_t)a_bytes;
+}
+lv_status lv_compensate_device_async(lv_handle h, const lv_state32* path, int32_t ns, const lv_state32* Xt2, const float* d_xyz,
+                                     const double* d_t, const int64_t* d_n, int64_t n_max, float* d_xyz_out) {
+    if (!path || !Xt2 || !d_xyz || !d_t || !d_n || !d_xyz_out) { set_error("compensate async: null path, Xt2, xyz, t, count or output"); return LV_ERR_ARG; }
+    if (n_max < 1 || n_max > 0x7fffffff) { set_error("compensate async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (ns < 2) { set_error("compensate async: a path needs two states"); return LV_ERR_ARG; }
+    /* one thread reads a point and then writes the same point: in place is fine, a shifted overlap is not */
+    if ((d_xyz_out != d_xyz && ranges_overlap(d_xyz_out, 12 * n_max, d_xyz, 12 * n_max)) || ranges_overlap(d_xyz_out, 12 * n_max, d_t, 8 * n_max)) {
+        set_error("compensate async: the output range overlaps an input range");
+        return LV_ERR_ARG;
+    }
+    if (!h) { set_error("compensate async: null handle"); return LV_ERR_ARG; }
+    if (n_max > h->prm.max_points) { set_error("compensate async: n_max above max_points"); return LV_ERR_ARG; }
+    lv_status s = deskew_args_ok(h, path, ns, Xt2, d_xyz, d_t, n_max, d_xyz_out);
+    if (s != LV_OK) return s;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    return deskew_common(h, path, ns, Xt2, d_xyz, d_t, d_n, n_max, d_xyz_out);
 }
 lv_status lv_compensate(lv_handle h, const lv_state32* path, int32_t ns, const lv_state32* Xt2, const float* xyz,
                         const double* t, int64_t n, float* xyz_out) {
@@ -1089,7 +1188,7 @@ lv_status lv_compensate(lv_handle h, const lv_state32* path, int32_t ns, const l
     }
     LV_CUDA(cudaMemcpyAsync(h->d_deskew_in, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
     LV_CUDA(cudaMemcpyAsync(h->d_times, t, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
-    s = deskew_common(h, path, ns, Xt2, h->d_deskew_in, h->d_times, n, h->d_deskew_in);
+    s = deskew_common(h, path, ns, Xt2, h->d_deskew_in, h->d_times, nullptr, n, h->d_deskew_in);
     if (s != LV_OK) return s;
     LV_CUDA(cudaMemcpyAsync(xyz_out, h->d_deskew_in, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(cudaStreamSynchronize(h->stream));
@@ -1123,19 +1222,29 @@ lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_
     LV_CUDA(cudaSetDevice(h->prm.device));
     LV_CUDA(ds_reserve(h->ds, n));
     int launches = 0;
-    LV_CUDA(launch_voxelgrid(h->ds, d_xyz, n, leaf, d_xyz_out, h->stream, &launches));
+    /* the async form's kernels over the host-known count, then the count read back */
+    LV_CUDA(launch_voxelgrid(h->ds, d_xyz, nullptr, n, leaf, d_xyz_out, nullptr, nullptr, h->stream, &launches));
     h->prof.total_launches += launches;
     LV_CUDA(cudaStreamSynchronize(h->stream));
-    if (h->ds.h_count[1]) {
-        /* pcl::VoxelGrid::applyFilter warns "Leaf size is too small for the input dataset. Integer indices would overflow."
-         * and hands the input on unchanged; Compensator::voxelgrid_downsample carries on with it.  Same here. */
-        set_error("voxel grid: leaf size too small for the extent of the cloud (cell index overflows): input passed through");
-        LV_CUDA(cudaMemcpyAsync(d_xyz_out, d_xyz, sizeof(float) * 3 * (size_t)n, cudaMemcpyDeviceToDevice, h->stream));
-        LV_CUDA(cudaStreamSynchronize(h->stream));
-        *n_out = n;
-        return LV_OK;
-    }
+    /* the pass-through (input copied, count n) is done on the device; the host keeps PCL's warning */
+    if (h->ds.h_count[1]) set_error("voxel grid: leaf size too small for the extent of the cloud (cell index overflows): input passed through");
     *n_out = h->ds.h_count[0];
+    return LV_OK;
+}
+lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf,
+                                               float* d_xyz_out, int64_t* d_n_out) {
+    if (!d_xyz || !d_n || !d_xyz_out || !d_n_out) { set_error("voxel grid async: null input, count, output or output count"); return LV_ERR_ARG; }
+    if (n_max < 1 || n_max > 0x7fffffff) { set_error("voxel grid async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!(leaf > 0.f)) { set_error("voxel grid async: leaf size must be positive"); return LV_ERR_ARG; }
+    /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids */
+    if (ranges_overlap(d_xyz, 12 * n_max, d_xyz_out, 12 * n_max)) { set_error("voxel grid async: the output range overlaps the input range"); return LV_ERR_ARG; }
+    if (!h) { set_error("voxel grid async: null handle"); return LV_ERR_ARG; }
+    if (n_max > h->prm.max_points) { set_error("voxel grid async: n_max above max_points"); return LV_ERR_ARG; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(ds_reserve(h->ds, n_max));
+    int launches = 0;
+    LV_CUDA(launch_voxelgrid(h->ds, d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, &h->d_async->err, h->stream, &launches));
+    h->prof.total_launches += launches;
     return LV_OK;
 }
 lv_status lv_voxelgrid_downsample(lv_handle h, const float* xyz, int64_t n, float leaf, float* xyz_out, int64_t* n_out) {
@@ -1175,10 +1284,11 @@ lv_status lv_temporal_downsample(lv_handle h, const float* xyz, int64_t n, int32
 }
 
 /* ---- Accumulator::process ------------------------------------------------------------------------ */
-lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
-                                  int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
-                                  int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
-                                  int32_t* d_idx, int64_t* n_out) {
+/* the argument checks and the launches of both forms: d_n_out NULL = the synchronous form (*n_out read back) */
+static lv_status process_cloud_impl(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
+                                    int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
+                                    int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                    int32_t* d_idx, int64_t* n_out, int64_t* d_n_out) {
     /* every check before the first device call */
     if (n_out) *n_out = 0;
     if (!layout || !d_data || !d_xyz || !d_time || !n_out) { set_error("process cloud: null layout, data, xyz, time or n_out"); return LV_ERR_ARG; }
@@ -1194,13 +1304,21 @@ lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_clou
             return LV_ERR_ARG;
         }
     if (!h) { set_error("process cloud: null handle"); return LV_ERR_ARG; }
-    if (cloud_bound(n, downsample_rate) == 0) return LV_OK;      /* nothing can be kept */
+    if (cloud_bound(n, downsample_rate) == 0) {                  /* nothing can be kept */
+        if (d_n_out) {
+            LV_CUDA(cudaSetDevice(h->prm.device));
+            LV_CUDA(cudaMemsetAsync(d_n_out, 0, sizeof(int64_t), h->stream));
+        }
+        return LV_OK;
+    }
     LV_CUDA(cudaSetDevice(h->prm.device));
     LV_CUDA(ds_reserve(h->ds, n));
     const CloudArgs a = {d_data, n, *layout, type, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time, downsample_rate, min_dist};
     int launches = 0;
-    LV_CUDA(launch_process_cloud(h->ds, a, CloudOut{d_xyz, d_time, d_intensity, d_range, d_idx}, h->stream, &launches));
+    LV_CUDA(launch_process_cloud(h->ds, a, CloudOut{d_xyz, d_time, d_intensity, d_range, d_idx}, d_n_out, d_n_out ? &h->d_async->err : nullptr,
+                                 h->stream, &launches));
     h->prof.total_launches += launches;
+    if (d_n_out) return LV_OK;
     LV_CUDA(cudaStreamSynchronize(h->stream));
     if (h->ds.h_count[1]) {
         set_error("process cloud: a kept point's timestamp is NaN (the time sort has no order for it)");
@@ -1208,6 +1326,43 @@ lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_clou
     }
     *n_out = h->ds.h_count[0];
     return LV_OK;
+}
+lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
+                                  int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
+                                  int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                  int32_t* d_idx, int64_t* n_out) {
+    return process_cloud_impl(h, type, layout, d_data, data_bytes, n, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time,
+                              downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range, d_idx, n_out, nullptr);
+}
+lv_status lv_process_cloud_device_async(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
+                                        int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
+                                        int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity,
+                                        float* d_range, int32_t* d_idx, int64_t* d_n_out) {
+    int64_t unused = 0;                                           /* the count stays on the device */
+    if (!d_n_out) { set_error("process cloud: null layout, data, xyz, time or n_out"); return LV_ERR_ARG; }
+    return process_cloud_impl(h, type, layout, d_data, data_bytes, n, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time,
+                              downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range, d_idx, &unused, d_n_out);
+}
+
+/* the deferred errors of the _async calls (AsyncWords::err) and the map's flags; clears the former */
+lv_status lv_async_status(lv_handle h) {
+    if (!h) return LV_ERR_ARG;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(cudaMemcpyAsync(&h->h_async->err, &h->d_async->err, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaMemsetAsync(&h->d_async->err, 0, sizeof(uint32_t), h->stream));
+    LV_CUDA(map_fetch_counters(h->map, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    const uint32_t err = h->h_async->err;
+    if (err) {
+        std::string msg;
+        if (err & kAsyncCloudNaN) msg += "process cloud: a kept point's timestamp is NaN (the time sort has no order for it); ";
+        if (err & kAsyncDeskewPath) msg += "compensate: a timestamp lies outside the path or the points are not time-sorted; ";
+        if (err & kAsyncCount) msg += "a device point count lies outside [0, n_max] (clamped); ";
+        msg.resize(msg.size() - 2);
+        set_error(msg);
+        return LV_ERR_ARG;
+    }
+    return map_status_from_mirror(h);
 }
 
 lv_status lv_synchronize(lv_handle h) {

@@ -44,7 +44,8 @@ __global__ void __launch_bounds__(256) lv_cloud_flag_kernel(CloudArgs a, uint8_t
 }
 
 __global__ void __launch_bounds__(256) lv_cloud_key_kernel(CloudArgs a, const int32_t* __restrict__ sel, int* __restrict__ count,
-                                                           int64_t bound, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+                                                           int64_t bound, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                           uint32_t* __restrict__ err) {
     const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= bound) return;
     if (j >= count[0]) {                      /* padding: sorts behind every kept point */
@@ -55,7 +56,10 @@ __global__ void __launch_bounds__(256) lv_cloud_key_kernel(CloudArgs a, const in
     const int32_t i = sel[j];
     const double begin = wire_begin_time(a.type, a.layout, a.data, a.n, a.stamp_us, a.stamp_beginning);
     const double t = wire_time(a.type, a.layout, cloud_point(a, i), a.offset_beginning, a.full_rotation_time, begin);
-    if (isnan(t)) count[1] = 1;
+    if (isnan(t)) {
+        count[1] = 1;
+        if (err) atomicOr(err, kAsyncCloudNaN);
+    }
     keys[j] = time_key(t);
     vals[j] = (uint32_t)i;
 }
@@ -63,8 +67,9 @@ __global__ void __launch_bounds__(256) lv_cloud_key_kernel(CloudArgs a, const in
 __global__ void __launch_bounds__(256) lv_cloud_gather_kernel(CloudArgs a, const uint32_t* __restrict__ order, const int* __restrict__ count,
                                                               float* __restrict__ xyz, double* __restrict__ time,
                                                               float* __restrict__ intensity, float* __restrict__ range,
-                                                              int32_t* __restrict__ idx) {
+                                                              int32_t* __restrict__ idx, int64_t* __restrict__ n_out) {
     const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0 && n_out) *n_out = count[0];
     if (r >= count[0]) return;
     const uint32_t i = order[r];
     const uint8_t* p = cloud_point(a, i);
@@ -80,19 +85,20 @@ __global__ void __launch_bounds__(256) lv_cloud_gather_kernel(CloudArgs a, const
 
 int64_t cloud_bound(int64_t n, int rate) { return rate <= 1 ? n : n / rate; }
 
-cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const CloudOut& o, cudaStream_t st, int* launches) {
+cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err, cudaStream_t st,
+                                 int* launches) {
     const int64_t bound = cloud_bound(a.n, a.rate);
     lv_cloud_flag_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, st>>>(a, s.flags, s.count);
     size_t tmp = s.tmp_bytes;
     cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags, s.sel, s.count, (int)a.n, st);
     if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)((bound + 255) / 256);
-    lv_cloud_key_kernel<<<grid, 256, 0, st>>>(a, s.sel, s.count, bound, s.keys64, s.vals);
+    lv_cloud_key_kernel<<<grid, 256, 0, st>>>(a, s.sel, s.count, bound, s.keys64, s.vals, err);
     tmp = s.tmp_bytes;
     e = cub::DeviceRadixSort::SortPairs(s.tmp, tmp, s.keys64, s.keys64_sorted, s.vals, s.vals_sorted, (int)bound, 0, 64, st);
     if (e != cudaSuccess) return e;
-    lv_cloud_gather_kernel<<<grid, 256, 0, st>>>(a, s.vals_sorted, s.count, o.xyz, o.time, o.intensity, o.range, o.idx);
-    cudaMemcpyAsync(s.h_count, s.count, 2 * sizeof(int), cudaMemcpyDeviceToHost, st);
+    lv_cloud_gather_kernel<<<grid, 256, 0, st>>>(a, s.vals_sorted, s.count, o.xyz, o.time, o.intensity, o.range, o.idx, d_n_out);
+    if (!d_n_out) cudaMemcpyAsync(s.h_count, s.count, 2 * sizeof(int), cudaMemcpyDeviceToHost, st);   /* the synchronous form reads them */
     if (launches) *launches += 6;
     return cudaGetLastError();
 }

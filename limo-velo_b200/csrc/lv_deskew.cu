@@ -14,7 +14,8 @@ namespace lv {
 enum { kDeskewThreads = 256, kMaxPathStates = 256 };
 
 __global__ void __launch_bounds__(kDeskewThreads) lv_deskew_kernel(const lv_state32* path, int ns, const Rt32 back,
-                                                                   const float* xyz, const double* t, int64_t n, float* out) {
+                                                                   const float* xyz, const double* t, const int64_t* d_n, int64_t n_max,
+                                                                   float* out) {
     __shared__ lv_state32 s_path[kMaxPathStates];
     {
         const uint32_t* src = reinterpret_cast<const uint32_t*>(path);
@@ -24,7 +25,7 @@ __global__ void __launch_bounds__(kDeskewThreads) lv_deskew_kernel(const lv_stat
     }
     __syncthreads();
     const int64_t i = (int64_t)blockIdx.x * kDeskewThreads + threadIdx.x;
-    if (i >= n) return;
+    if (i >= device_count(d_n, n_max, nullptr)) return;
     const float p[3] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2]};
     float q[3];
     deskew_point(s_path, ns, back, p, t[i], q);
@@ -32,22 +33,26 @@ __global__ void __launch_bounds__(kDeskewThreads) lv_deskew_kernel(const lv_stat
 }
 
 /* 1 where a timestamp lies outside [t_lo, t_hi] or is smaller than its predecessor (the reference asserts both) */
-__global__ void lv_deskew_check_kernel(const double* t, int64_t n, double t_lo, double t_hi, int* bad) {
+__global__ void lv_deskew_check_kernel(const double* t, const int64_t* d_n, int64_t n_max, double t_lo, double t_hi, int* bad,
+                                       uint32_t* err) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= device_count(d_n, n_max, err)) return;
     const double v = t[i];
-    if (!(v >= t_lo && v <= t_hi) || (i > 0 && v < t[i - 1])) *bad = 1;
+    if (!(v >= t_lo && v <= t_hi) || (i > 0 && v < t[i - 1])) {
+        *bad = 1;
+        if (err) atomicOr(err, kAsyncDeskewPath);
+    }
 }
 
 int deskew_max_states() { return kMaxPathStates; }
 
-cudaError_t launch_deskew(const lv_state32* d_path, int ns, const lv_state32& Xt2, double t_lo, double t_hi,
-                          const float* d_xyz, const double* d_t, int64_t n, float* d_out, int* d_bad, cudaStream_t st) {
+cudaError_t launch_deskew(const lv_state32* d_path, int ns, const lv_state32& Xt2, double t_lo, double t_hi, const float* d_xyz,
+                          const double* d_t, const int64_t* d_n, int64_t n_max, float* d_out, int* d_bad, uint32_t* err, cudaStream_t st) {
     const Rt32 back = deskew_back(Xt2);
-    const unsigned grid = (unsigned)((n + kDeskewThreads - 1) / kDeskewThreads);
+    const unsigned grid = (unsigned)((n_max + kDeskewThreads - 1) / kDeskewThreads);
     cudaMemsetAsync(d_bad, 0, sizeof(int), st);
-    lv_deskew_check_kernel<<<grid, kDeskewThreads, 0, st>>>(d_t, n, t_lo, t_hi, d_bad);
-    lv_deskew_kernel<<<grid, kDeskewThreads, 0, st>>>(d_path, ns, back, d_xyz, d_t, n, d_out);
+    lv_deskew_check_kernel<<<grid, kDeskewThreads, 0, st>>>(d_t, d_n, n_max, t_lo, t_hi, d_bad, err);
+    lv_deskew_kernel<<<grid, kDeskewThreads, 0, st>>>(d_path, ns, back, d_xyz, d_t, d_n, n_max, d_out);
     return cudaGetLastError();
 }
 

@@ -25,17 +25,20 @@ namespace lv {
 struct GridBox {          /* written by the bounding-box kernel, read by the key kernel */
     int mn[3], mx[3];     /* floats in an order-preserving int encoding */
     int overflow;         /* PCL refuses when the cell count exceeds INT32_MAX */
+    int64_t n;            /* points of the cloud (<= the host bound the grids and the sort are sized for) */
 };
 
 __device__ __forceinline__ int f2ord(float f) { const int i = __float_as_int(f); return i ^ ((i >> 31) & 0x7fffffff); }
 __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i ^ ((i >> 31) & 0x7fffffff)); }
 
-__global__ void lv_ds_box_init_kernel(GridBox* b) {
+__global__ void lv_ds_box_init_kernel(GridBox* b, const int64_t* d_n, int64_t n_max, uint32_t* err) {
     if (threadIdx.x < 3) { b->mn[threadIdx.x] = 0x7fffffff; b->mx[threadIdx.x] = (int)0x80000000; }
     if (threadIdx.x == 3) b->overflow = 0;
+    if (threadIdx.x == 0) b->n = device_count(d_n, n_max, err);
 }
 
-__global__ void __launch_bounds__(256) lv_ds_box_kernel(const float* __restrict__ xyz, int64_t n, GridBox* b) {   /* getMinMax3D */
+__global__ void __launch_bounds__(256) lv_ds_box_kernel(const float* __restrict__ xyz, GridBox* b) {   /* getMinMax3D */
+    const int64_t n = b->n;
     int mn[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff}, mx[3] = {(int)0x80000000, (int)0x80000000, (int)0x80000000};
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
 #pragma unroll
@@ -55,10 +58,18 @@ __global__ void __launch_bounds__(256) lv_ds_box_kernel(const float* __restrict_
     }
 }
 
-/* voxel_grid.hpp: min_b = floor(min_p * inv), div_b = floor(max_p * inv) - min_b + 1, idx = ijk . (1, div0, div0 div1) */
-__global__ void __launch_bounds__(256) lv_ds_keys_kernel(const float* __restrict__ xyz, int64_t n, float inv, GridBox* b,
+/* voxel_grid.hpp: min_b = floor(min_p * inv), div_b = floor(max_p * inv) - min_b + 1, idx = ijk . (1, div0, div0 div1).
+ * Slots [b->n, n_max) get the padding key 0xFFFFFFFF: no cell index reaches it (cells <= INT32_MAX), and the stable sort
+ * keeps a real key that ties with it in front, so the first b->n sorted pairs are those of a sort over b->n points. */
+__global__ void __launch_bounds__(256) lv_ds_keys_kernel(const float* __restrict__ xyz, int64_t n_max, float inv, GridBox* b,
                                                          uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t n = b->n;
+    if (i >= n && i < n_max) {
+        keys[i] = 0xFFFFFFFFu;
+        vals[i] = (uint32_t)i;
+        return;
+    }
     int minb[3], divb[3];
     long long cells = 1;
 #pragma unroll
@@ -78,17 +89,19 @@ __global__ void __launch_bounds__(256) lv_ds_keys_kernel(const float* __restrict
     vals[i] = (uint32_t)i;
 }
 
-__global__ void __launch_bounds__(256) lv_ds_heads_kernel(const uint32_t* __restrict__ keys, int64_t n, uint8_t* __restrict__ head) {
+__global__ void __launch_bounds__(256) lv_ds_heads_kernel(const uint32_t* __restrict__ keys, int64_t n_max, const GridBox* b,
+                                                          uint8_t* __restrict__ head) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) head[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1 : 0;
+    if (i < n_max) head[i] = (i < b->n && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
 }
 
 /* one thread per leaf: AccumulatorXYZ (xyz += p in sorted order), centroid = xyz / n */
 __global__ void __launch_bounds__(256) lv_ds_centroid_kernel(const float* __restrict__ xyz, const uint32_t* __restrict__ vals,
                                                              const uint32_t* __restrict__ starts, const int* __restrict__ n_runs,
-                                                             int64_t n, float* __restrict__ out) {
+                                                             const GridBox* __restrict__ b, float* __restrict__ out) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     const int runs = *n_runs;
+    const int64_t n = b->n;
     if (r >= runs) return;
     const uint32_t s = starts[r], e = r + 1 < runs ? starts[r + 1] : (uint32_t)n;
     float sx = 0.f, sy = 0.f, sz = 0.f;
@@ -98,6 +111,22 @@ __global__ void __launch_bounds__(256) lv_ds_centroid_kernel(const float* __rest
     }
     const float cnt = (float)(e - s);
     out[3 * (size_t)r] = fdiv(sx, cnt); out[3 * (size_t)r + 1] = fdiv(sy, cnt); out[3 * (size_t)r + 2] = fdiv(sz, cnt);
+}
+
+/* the output count, and PCL's pass-through: when the cell index overflows, pcl::VoxelGrid::applyFilter warns "Leaf size is too
+ * small for the input dataset. Integer indices would overflow." and hands the input on unchanged (Compensator::voxelgrid_downsample
+ * carries on with it): the input is copied over the centroids and the count is the input's.  count[0] becomes the output count. */
+__global__ void __launch_bounds__(256) lv_ds_finish_kernel(const float* __restrict__ xyz, const GridBox* __restrict__ b, int* __restrict__ count,
+                                                           float* __restrict__ out, int64_t* __restrict__ n_out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t n = b->n;
+    const bool pass = b->overflow && n > 0;
+    if (i == 0) {
+        const int64_t m = n == 0 ? 0 : (pass ? n : (int64_t)count[0]);
+        count[0] = (int)m;
+        if (n_out) *n_out = m;
+    }
+    if (pass && i < 3 * n) out[i] = xyz[i];
 }
 
 /* temporal_downsample: keep = (rate <= 1 or (i + 1) % rate == 0) and min_dist < |p| (lv_wire.h) */
@@ -158,26 +187,28 @@ void ds_free(DownsampleScratch& s) {
     s = DownsampleScratch();
 }
 
-/* enqueues everything; afterwards s.h_count[0] = number of leaves, s.h_count[1] = overflow flag (after a stream sync) */
-cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, int64_t n, float leaf, float* d_out, cudaStream_t st,
-                             int* launches) {
-    const unsigned grid = (unsigned)((n + 255) / 256);
+cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf, float* d_out,
+                             int64_t* d_n_out, uint32_t* err, cudaStream_t st, int* launches) {
+    const unsigned grid = (unsigned)((n_max + 255) / 256);
     GridBox* box = static_cast<GridBox*>(s.box);
     const float inv = fdiv(1.0f, leaf);
-    lv_ds_box_init_kernel<<<1, 32, 0, st>>>(box);
-    lv_ds_box_kernel<<<grid < kNumSMs * 4u ? grid : kNumSMs * 4u, 256, 0, st>>>(d_xyz, n, box);
-    lv_ds_keys_kernel<<<grid, 256, 0, st>>>(d_xyz, n, inv, box, s.keys, s.vals);
+    lv_ds_box_init_kernel<<<1, 32, 0, st>>>(box, d_n, n_max, err);
+    lv_ds_box_kernel<<<grid < kNumSMs * 4u ? grid : kNumSMs * 4u, 256, 0, st>>>(d_xyz, box);
+    lv_ds_keys_kernel<<<grid, 256, 0, st>>>(d_xyz, n_max, inv, box, s.keys, s.vals);
     size_t tmp = s.tmp_bytes;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(s.tmp, tmp, s.keys, s.keys_sorted, s.vals, s.vals_sorted, (int)n, 0, 32, st);
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(s.tmp, tmp, s.keys, s.keys_sorted, s.vals, s.vals_sorted, (int)n_max, 0, 32, st);
     if (e != cudaSuccess) return e;
-    lv_ds_heads_kernel<<<grid, 256, 0, st>>>(s.keys_sorted, n, s.flags);
+    lv_ds_heads_kernel<<<grid, 256, 0, st>>>(s.keys_sorted, n_max, box, s.flags);
     tmp = s.tmp_bytes;
-    e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags, s.sel, s.count, (int)n, st);
+    e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags, s.sel, s.count, (int)n_max, st);
     if (e != cudaSuccess) return e;
-    lv_ds_centroid_kernel<<<grid, 256, 0, st>>>(d_xyz, s.vals_sorted, reinterpret_cast<const uint32_t*>(s.sel), s.count, n, d_out);
-    cudaMemcpyAsync(&s.h_count[0], s.count, sizeof(int), cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(&s.h_count[1], &box->overflow, sizeof(int), cudaMemcpyDeviceToHost, st);
-    if (launches) *launches += 10;
+    lv_ds_centroid_kernel<<<grid, 256, 0, st>>>(d_xyz, s.vals_sorted, reinterpret_cast<const uint32_t*>(s.sel), s.count, box, d_out);
+    lv_ds_finish_kernel<<<(unsigned)((3 * n_max + 255) / 256), 256, 0, st>>>(d_xyz, box, s.count, d_out, d_n_out);
+    if (!d_n_out) {                           /* the synchronous form reads the count and the warning flag */
+        cudaMemcpyAsync(&s.h_count[0], s.count, sizeof(int), cudaMemcpyDeviceToHost, st);
+        cudaMemcpyAsync(&s.h_count[1], &box->overflow, sizeof(int), cudaMemcpyDeviceToHost, st);
+    }
+    if (launches) *launches += 11;
     return cudaGetLastError();
 }
 

@@ -15,6 +15,35 @@ namespace lv {
 
 /* SMs of one H100 SXM: fixed grids that stride over device-side work are sized in multiples of it */
 enum { kNumSMs = 132 };
+
+/* The stream-ordered (_async) entry points report errors through one device word of the handle, read and cleared by
+ * lv_async_status.  Bits: */
+enum : uint32_t { kAsyncCloudNaN = 1u, kAsyncDeskewPath = 2u, kAsyncCount = 4u };
+/* device words of the async tick: the deferred errors and what lv_correct_device_async decided */
+struct AsyncWords {
+    uint32_t err;              /* kAsync* bits since the last lv_async_status              */
+    int32_t time_set;          /* 1: an async update ran since the last fetch; time_updated is its time */
+    double time_updated;
+};
+#ifdef __CUDACC__
+/* a count in device memory (NULL: the host-known n_max) clamped to [0, n_max]; one thread flags a count outside it */
+__device__ __forceinline__ int64_t device_count(const int64_t* d_n, int64_t n_max, uint32_t* err) {
+    if (!d_n) return n_max;
+    const int64_t v = *d_n;
+    if (v >= 0 && v <= n_max) return v;
+    if (err && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(err, kAsyncCount);
+    return v < 0 ? 0 : n_max;
+}
+#endif
+
+/* what lv_correct_device_async hands the begin kernel (all zero / NULL for the synchronous forms) */
+struct UpdateGate {
+    const int64_t* n = nullptr;              /* device count of the sweep (NULL: the host-known n) */
+    int64_t min_points = 0;                  /* main.cpp:81 MAX_POINTS2MATCH: fewer points -> LV_TOO_FEW_POINTS, no update */
+    const uint32_t* map_counters = nullptr;  /* non-NULL: LV_EMPTY_MAP when the map holds no point (host cannot know it) */
+    AsyncWords* words = nullptr;             /* non-NULL: the time of an update that runs goes to words->time_updated */
+    double time = 0.0;
+};
 /* the fit kernel's grid: 4 blocks of kMeasureThreads resident per SM is ample; one partial row per block */
 enum { kMeasureThreads = 128, kPartialStride = 96, kStepThreads = 512, kPartialGroup = 32, kMeasureGridCap = kNumSMs * 4 };
 inline int partial_groups(int grid) { return (grid + kPartialGroup - 1) / kPartialGroup; }
@@ -88,7 +117,6 @@ struct MapBuffers {
     int64_t cap;               /* max_map_points, then what the last growth sized for (tables and arena) */
     int64_t add_cap;           /* most points one build / add can take                        */
     int64_t max_points;        /* lv_params.max_points: add_cap never drops below it          */
-    int64_t n_inserted;        /* ids handed out so far                                       */
     bool empty;                /* nothing was ever added (Mapper::exists, Mapper.cpp:32-34)   */
     cudaStream_t stream;       /* the stream the buffers were allocated on (stream-ordered)   */
 };
@@ -111,11 +139,22 @@ void map_free(MapBuffers& b);
 cudaError_t map_grow(MapBuffers& b, int64_t cap, cudaStream_t st, int* launches);
 /* empty the map (table, block table, counters); asynchronous */
 cudaError_t map_clear(MapBuffers& b, cudaStream_t st, int* launches);
-/* KD_TREE::Build (downsample = 0 on an empty map) / Add_Points: n points in DEVICE memory; asynchronous, no host round trip */
-cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample, cudaStream_t st, int* launches);
+/* the count of an add that lives in device memory (lv_correct_device_async -> lv_map_add_last_sweep): the add takes
+ * *n points (clamped to the host bound), none when *n < max(min_points, 1) (main.cpp:81 breaks before map.add); with
+ * build_if_empty an add that finds the map without points builds it (no downsampling, Mapper.cpp:26) */
+struct MapAddCount {
+    const int64_t* n = nullptr;
+    int64_t min_points = 0;
+    int build_if_empty = 0;
+    uint32_t* err = nullptr;
+};
+/* KD_TREE::Build (downsample = 0 on an empty map) / Add_Points: n points in DEVICE memory (or *cnt.n of them, n = the
+ * host-known bound the sort runs over); asynchronous, no host round trip */
+cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample, cudaStream_t st, int* launches,
+                    const MapAddCount& cnt = MapAddCount(), const UpdateCtrl* to_world = nullptr);
 /* the sweep (LiDAR frame, device) transformed by the state in d_ctrl->x, then map_add: main.cpp:99-105 without leaving the GPU */
 cudaError_t map_add_sweep(MapBuffers& b, const UpdateCtrl* d_ctrl, const float* d_xyz_lidar, int64_t n, int downsample, cudaStream_t st,
-                          int* launches);
+                          int* launches, const MapAddCount& cnt = MapAddCount());
 cudaError_t map_fetch_counters(MapBuffers& b, cudaStream_t st);
 cudaError_t map_points_sorted(MapBuffers& b, float* host_out, int64_t cap, int64_t* n_out, cudaStream_t st);
 VoxelMapView map_view(const MapBuffers& b);
@@ -129,7 +168,8 @@ struct MeasureProbe { void (*at)(void* ctx, int stage); void* ctx; };
  * the shape of the level-0 search kernel (search_group() in lv_measure.cu). */
 cudaError_t launch_measure(const MeasureArgs& a, int grid, cudaStream_t st, const MeasureProbe* probe = nullptr,
                            int reuse = 0, int pdl = 0);
-cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n, uint32_t* counters, cudaStream_t st);
+cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n, uint32_t* counters, const UpdateGate& gate,
+                               cudaStream_t st);
 const void* ieskf_begin_kernel_ptr();
 void measure_init();                          /* constant tables; call once before any capture           */
 cudaError_t launch_ieskf_step(UpdateCtrl* c, const IeskfParams& prm, const double* partials, int n_partials,
@@ -156,8 +196,11 @@ struct DownsampleScratch {
 };
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n);
 void ds_free(DownsampleScratch& s);
-cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, int64_t n, float leaf, float* d_out, cudaStream_t st,
-                             int* launches);
+/* the voxel grid over d_n ? *d_n : n_max points (the sort runs over n_max, padding keys last), the PCL cell-index overflow
+ * pass-through decided on the device; afterwards s.count[0] = output count (also written to *d_n_out when non-NULL),
+ * s.h_count[0] / [1] = output count / overflow flag after a stream sync */
+cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf, float* d_out,
+                             int64_t* d_n_out, uint32_t* err, cudaStream_t st, int* launches);
 cudaError_t launch_temporal(DownsampleScratch& s, const float* d_xyz, int64_t n, int rate, double min_dist, float* d_out,
                             int32_t* d_idx_out, cudaStream_t st, int* launches);
 
@@ -177,13 +220,16 @@ struct CloudOut { float* xyz; double* time; float* intensity; float* range; int3
 /* most points the decimator can keep: the slots the sort runs over */
 int64_t cloud_bound(int64_t n, int rate);
 /* enqueues everything (needs ds_reserve(s, n) and cloud_bound > 0); afterwards s.h_count[0] = points kept, s.h_count[1] = 1 if a
- * kept point's time is NaN (after a stream sync) */
-cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const CloudOut& o, cudaStream_t st, int* launches);
+ * kept point's time is NaN (after a stream sync).  d_n_out (may be NULL) receives the count on the device; err (may be NULL)
+ * gets kAsyncCloudNaN for a NaN time */
+cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err, cudaStream_t st,
+                                 int* launches);
 
-/* lv_deskew.cu: Compensator::compensate.  d_bad (one int) is set when a timestamp is out of range / out of order */
+/* lv_deskew.cu: Compensator::compensate over d_n ? *d_n : n_max points.  d_bad (one int) is set when a timestamp is out of
+ * range / out of order; err (may be NULL) gets kAsyncDeskewPath then too */
 int deskew_max_states();
-cudaError_t launch_deskew(const lv_state32* d_path, int ns, const lv_state32& Xt2, double t_lo, double t_hi,
-                          const float* d_xyz, const double* d_t, int64_t n, float* d_out, int* d_bad, cudaStream_t st);
+cudaError_t launch_deskew(const lv_state32* d_path, int ns, const lv_state32& Xt2, double t_lo, double t_hi, const float* d_xyz,
+                          const double* d_t, const int64_t* d_n, int64_t n_max, float* d_out, int* d_bad, uint32_t* err, cudaStream_t st);
 
 }  // namespace lv
 #endif

@@ -35,27 +35,39 @@ __global__ void __launch_bounds__(256) lv_map_clear_kernel(uint4* table, uint32_
     if (i0 < (size_t)kMapCounters) counters[i0] = i0 == (size_t)kCtrArenaTop ? 16u : 0u;   /* position 0 is never handed out */
 }
 
-__global__ void lv_map_begin_kernel(uint32_t* counters) {
-    if (threadIdx.x == 0) { counters[kCtrTouched] = 0u; counters[kCtrDirty] = 0u; }
+/* the add's point count (n, or the device count of MapAddCount), its first id and whether it builds the map */
+__global__ void lv_map_begin_kernel(uint32_t* counters, int64_t n, const int64_t* d_n, int64_t min_points, int build_if_empty,
+                                    uint32_t* err) {
+    if (threadIdx.x == 0) {
+        counters[kCtrTouched] = 0u;
+        counters[kCtrDirty] = 0u;
+        int64_t k = device_count(d_n, n, err);
+        if (d_n && k < (min_points > 1 ? min_points : 1)) k = 0;              /* main.cpp:81: the tick breaks before map.add */
+        counters[kCtrAddN] = (uint32_t)k;
+        counters[kCtrIdBase] = counters[kCtrIds];                            /* a new point gets id_base + its index in the batch */
+        counters[kCtrIds] += (uint32_t)k;
+        counters[kCtrBuild] = (build_if_empty && counters[kCtrPoints] == 0u) ? 1u : 0u;
+    }
 }
 
+/* slots past the add's count get the key of a point that cannot be stored: the merge skips them */
 __global__ void __launch_bounds__(256) lv_map_keys_kernel(const VoxelMapRW m, const float* __restrict__ xyz, uint32_t n,
                                                            uint32_t* __restrict__ skeys, uint32_t* __restrict__ svals) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    skeys[i] = map_point_key(m, xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2]);
+    skeys[i] = i < m.counters[kCtrAddN] ? map_point_key(m, xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2]) : 0xFFFFFFFFu;
     svals[i] = i;
 }
 
 __global__ void __launch_bounds__(128) lv_map_merge_kernel(const VoxelMapRW m, const uint32_t* __restrict__ skeys,
                                                             const uint32_t* __restrict__ svals, uint32_t n,
-                                                            const float* __restrict__ xyz, uint32_t id_base, int downsample) {
+                                                            const float* __restrict__ xyz, int downsample) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
     const uint32_t key = skeys[j];
     if (key == 0xFFFFFFFFu) return;                                          /* not storable (non-finite / table full) */
     if (j > 0 && (skeys[j - 1] >> kCellBits) == (key >> kCellBits)) return;  /* not the head of its voxel's run */
-    map_merge_run(m, skeys, svals, j, n, xyz, id_base, downsample);
+    map_merge_run(m, skeys, svals, j, n, xyz, m.counters[kCtrIdBase], m.counters[kCtrBuild] ? 0 : downsample);
 }
 
 __global__ void __launch_bounds__(256) lv_map_dilate_kernel(const VoxelMapRW m) {
@@ -167,13 +179,13 @@ __global__ void __launch_bounds__(256) lv_map_unpack_kernel(const float4* __rest
 
 /* main.cpp:99-105 on the device: the sweep (LiDAR frame) in world coordinates with the state the update just produced,
  * Xt2 * Xt2.I_Rt_L() * p in fp32 (State.cpp:79-89, RotTransl.cpp:36-48) — the very transform Mapper::match applies */
-__global__ void __launch_bounds__(256) lv_sweep_to_world_kernel(const UpdateCtrl* __restrict__ c, const float* __restrict__ xyz, uint32_t n,
-                                                                 float* __restrict__ out) {
+__global__ void __launch_bounds__(256) lv_sweep_to_world_kernel(const UpdateCtrl* __restrict__ c, const float* __restrict__ xyz,
+                                                                 const uint32_t* __restrict__ counters, float* __restrict__ out) {
     __shared__ Frame s_frame;
     if (threadIdx.x == 0) make_frame(c->x, &s_frame);
     __syncthreads();
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= counters[kCtrAddN]) return;
     float g[3];
     rt_apply(s_frame.lidar_to_world, xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2], g);
     out[3 * (size_t)i] = g[0]; out[3 * (size_t)i + 1] = g[1]; out[3 * (size_t)i + 2] = g[2];
@@ -353,24 +365,29 @@ VoxelMapView map_view(const MapBuffers& b) { return map_view_of(map_rw(b)); }
 
 cudaError_t map_clear(MapBuffers& b, cudaStream_t st, int* launches) {
     lv_map_clear_kernel<<<kNumSMs * 8, 256, 0, st>>>(b.table, b.slots, b.btable, b.bslots, b.counters);
-    b.n_inserted = 0;
     b.empty = true;
     if (launches) *launches += 1;
     return cudaGetLastError();
 }
 
-cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample, cudaStream_t st, int* launches) {
+cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample, cudaStream_t st, int* launches, const MapAddCount& cnt,
+                    const UpdateCtrl* to_world) {
     if (n <= 0) return cudaSuccess;
     if (n > b.add_cap) return cudaErrorInvalidValue;
     const VoxelMapRW m = map_rw(b);
     const uint32_t n32 = (uint32_t)n;
     const unsigned blocks = (unsigned)((n + 255) / 256);
-    lv_map_begin_kernel<<<1, 32, 0, st>>>(b.counters);
+    lv_map_begin_kernel<<<1, 32, 0, st>>>(b.counters, n, cnt.n, cnt.min_points, cnt.build_if_empty, cnt.err);
+    if (to_world) {
+        lv_sweep_to_world_kernel<<<blocks, 256, 0, st>>>(to_world, d_xyz, b.counters, b.stage_xyz);
+        d_xyz = b.stage_xyz;
+        if (launches) *launches += 1;
+    }
     lv_map_keys_kernel<<<blocks, 256, 0, st>>>(m, d_xyz, n32, b.skeys, b.svals);
     size_t tmp = b.sort_tmp_bytes;
     cudaError_t e = cub::DeviceRadixSort::SortPairs(b.sort_tmp, tmp, b.skeys, b.skeys_alt, b.svals, b.svals_alt, (int)n, 0, b.sort_bits, st);
     if (e != cudaSuccess) return e;
-    lv_map_merge_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(m, b.skeys_alt, b.svals_alt, n32, d_xyz, (uint32_t)b.n_inserted, downsample);
+    lv_map_merge_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(m, b.skeys_alt, b.svals_alt, n32, d_xyz, downsample);
     /* touched <= n voxels, dirty <= 27 n: fixed grids striding over the device-side counts */
     uint64_t dil = ((uint64_t)n * 27 + 255) / 256;
     dil = dil < 1 ? 1 : (dil > kNumSMs * 8u ? kNumSMs * 8u : dil);
@@ -378,19 +395,14 @@ cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample
     uint64_t hal = ((uint64_t)n * 27 + 7) / 8;
     hal = hal < 1 ? 1 : (hal > kNumSMs * 64u ? kNumSMs * 64u : hal);
     lv_map_halo_kernel<<<(unsigned)hal, 256, 0, st>>>(m);
-    b.n_inserted += n;
     b.empty = false;
     if (launches) *launches += 5 + 4;   /* + histogram and onesweep passes of the sort (approximate) */
     return cudaGetLastError();
 }
 
 cudaError_t map_add_sweep(MapBuffers& b, const UpdateCtrl* d_ctrl, const float* d_xyz_lidar, int64_t n, int downsample, cudaStream_t st,
-                          int* launches) {
-    if (n <= 0) return cudaSuccess;
-    if (n > b.add_cap) return cudaErrorInvalidValue;
-    lv_sweep_to_world_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_ctrl, d_xyz_lidar, (uint32_t)n, b.stage_xyz);
-    if (launches) *launches += 1;
-    return map_add(b, b.stage_xyz, n, b.empty ? 0 : downsample, st, launches);
+                          int* launches, const MapAddCount& cnt) {
+    return map_add(b, d_xyz_lidar, n, b.empty ? 0 : downsample, st, launches, cnt, d_ctrl);
 }
 
 /* device counters -> pinned mirror; the caller synchronises the stream before reading b.h_counters */

@@ -588,17 +588,32 @@ __global__ void __launch_bounds__(kStepThreads) lv_reduce_partials_kernel(const 
     if (threadIdx.x == 0) out[156] = (double)nm;
 }
 
+/* with gate.n the sweep's count comes from device memory (n is then its host-known bound); an update the gate stops finishes
+ * here with a status, the state untouched: every later kernel of the update sees done = 1 */
 __global__ void __launch_bounds__(256) lv_ieskf_begin_kernel(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n,
-                                                             uint32_t* counters) {
+                                                             uint32_t* counters, const UpdateGate gate) {
     pdl_trigger();
     if (counters && threadIdx.x < kCounters) counters[threadIdx.x] = 0u;    /* work-list lengths of the measurement kernels */
+    const int k = (int)device_count(gate.n, n, gate.words ? &gate.words->err : nullptr);
     if (job && threadIdx.x == 0) {
         job->xyz = xyz;
-        job->n = n;
-        job->n_tiles = (n + kMeasureThreads - 1) / kMeasureThreads;
+        job->n = k;
+        job->n_tiles = (k + kMeasureThreads - 1) / kMeasureThreads;
     }
     ExecBlock ex;
     ieskf_begin(ex, c);
+    if (threadIdx.x == 0) {
+        if (gate.n && k < (gate.min_points > 1 ? gate.min_points : 1)) {      /* main.cpp:81 */
+            c->status = LV_TOO_FEW_POINTS;
+            c->done = 1;
+        } else if (gate.map_counters && gate.map_counters[kCtrPoints] == 0u) {  /* Localizator.cpp:24 */
+            c->status = LV_EMPTY_MAP;
+            c->done = 1;
+        } else if (gate.words) {
+            gate.words->time_updated = gate.time;                              /* Localizator.cpp:26 */
+            gate.words->time_set = 1;
+        }
+    }
 }
 
 /* Localizator::propagate_to (Localizator.cpp:59-75): every IMU sample between two sweeps through esekf::predict, one launch,
@@ -707,8 +722,9 @@ cudaError_t launch_measure(const MeasureArgs& a, int grid, cudaStream_t st, cons
     if (probe) probe->at(probe->ctx, 3);
     return cudaGetLastError();
 }
-cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n, uint32_t* counters, cudaStream_t st) {
-    lv_ieskf_begin_kernel<<<1, 256, 0, st>>>(c, job, xyz, n, counters);
+cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n, uint32_t* counters, const UpdateGate& gate,
+                               cudaStream_t st) {
+    lv_ieskf_begin_kernel<<<1, 256, 0, st>>>(c, job, xyz, n, counters, gate);
     return cudaGetLastError();
 }
 const void* ieskf_begin_kernel_ptr() { return (const void*)lv_ieskf_begin_kernel; }

@@ -52,7 +52,10 @@ enum {
     kMaxCellsPerVoxel = 3
 };
 /* device counters of the map (MapCounters index) */
-enum { kCtrArenaTop = 0, kCtrPoints, kCtrTouched, kCtrDirty, kCtrError, kCtrSlotsUsed, kCtrGather, kCtrBlocksUsed, kMapCounters = 16 };
+/* kCtrIds: ids handed out so far; kCtrIdBase: the first id of the add in flight; kCtrAddN: points of the add in flight;
+ * kCtrBuild: 1 when the add in flight builds the map (no downsampling) */
+enum { kCtrArenaTop = 0, kCtrPoints, kCtrTouched, kCtrDirty, kCtrError, kCtrSlotsUsed, kCtrGather, kCtrBlocksUsed,
+       kCtrIds, kCtrIdBase, kCtrAddN, kCtrBuild, kMapCounters = 16 };
 /* bits of kCtrError */
 enum { kErrTableFull = 1, kErrArenaFull = 2, kErrExtentTooLarge = 4, kErrListFull = 8, kErrBlockTableFull = 16 };
 
