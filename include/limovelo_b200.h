@@ -406,6 +406,49 @@ lv_status lv_correct_device_async(lv_handle h, const float* d_xyz, const int64_t
  * LV_ERR_ARG (lv_last_error names the stage), LV_ERR_CAPACITY or LV_OK.  Clears them; the handle stays usable.  Synchronises. */
 lv_status lv_async_status(lv_handle h);
 
+/* ---- the LiDAR buffer in HBM (Accumulator::BUFFER_L, include/Headers/Accumulator.hpp:3) ------------------------------------------
+ * main.cpp:61-79 localizes on a time window [t1, t2] that is usually much shorter than a message: Compensator::compensate(t1, t2)
+ * takes its points from the Accumulator's LiDAR buffer (Compensator.cpp:23 -> Accumulator::get_points -> get, Accumulator.hpp:61-74),
+ * which receive_lidar fills one processed message at a time (Accumulator.cpp:39-48) and clear_lidar empties from its old end
+ * (main.cpp:122, Buffer.cpp:66-70).  These calls keep that buffer on the device: a message goes lv_process_cloud_device_async ->
+ * scratch -> lv_lidar_push_device_async, a tick's window comes out of lv_lidar_get_points_device_async into the buffers that
+ * lv_compensate_device_async reads, and nothing about the buffer's fill state is known on the host.  Time management (t2, the
+ * delta schedule, the field-of-view check) stays with the caller.
+ * The results are the reference's bit for bit, quirks included: the buffer is in arrival order (a late or overlapping message
+ * leaves it unsorted, and get still runs its binary search with the reference's probe sequence), and of m points whose time
+ * equals t2 exactly only min(m, 2) are returned (the walk starts one before the last of them; t1 is inclusive, so the next
+ * window picks up the rest).  Point times that are NaN follow the reference's comparisons.  The buffer holds xyz (float) and
+ * time (double) per point: 20 bytes.  All calls are stream-ordered on the handle's stream.  Argument errors are LV_ERR_ARG
+ * before any device work, also with a null handle: null pointers, n_max outside [1, 2^31 - 1], a NaN time argument, a push, get
+ * or clear before lv_lidar_reserve, and ranges that overlap each other or the buffer.  lv_destroy releases the buffer. */
+/* sizes the buffer for `capacity` points (1 .. 2^30; the deque has no bound, so size it for empty_lidar_time of data plus the
+ * messages a tick may leave behind); the live points stay, in order.  LV_ERR_CAPACITY when more points are live than fit.
+ * Synchronises. */
+lv_status lv_lidar_reserve(lv_handle h, int64_t capacity);
+/* Accumulator::receive_lidar's `for (Point p : points) this->add(p);` (Accumulator.cpp:47): appends the *d_n points (clamped to
+ * [0, n_max]) of d_xyz (n x 3) / d_time in that order, the last one becoming content[0].  Points that do not fit are a deferred
+ * error (lv_async_status) and leave the buffer unchanged: nothing is dropped silently. */
+lv_status lv_lidar_push_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max);
+/* Accumulator::get_points(t1, t2) (Accumulator.cpp:93-95, Accumulator.hpp:61-74): the points of the window, oldest inserted first,
+ * into d_xyz (n_max x 3) / d_time (n_max); *d_n_out = their count.  A window of more than n_max points writes count 0 and is a
+ * deferred error: the tick that follows is gated off (LV_TOO_FEW_POINTS) and lv_async_status names the stage. */
+lv_status lv_lidar_get_points_device_async(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max,
+                                           int64_t* d_n_out);
+/* the same kernels, then the count read back into *n_out (host); a window above n_max returns LV_ERR_CAPACITY with *n_out = 0
+ * and lv_last_error() naming its size.  Synchronises. */
+lv_status lv_lidar_get_points_device(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* n_out);
+/* Accumulator::clear_lidar(t) (Accumulator.cpp:68-70, Buffer.cpp:66-70): drops the oldest points while t >= their time, stopping
+ * at the first one, in insertion order, that is newer than t */
+lv_status lv_lidar_clear_async(lv_handle h, double t);
+struct lv_lidar_info {
+    int64_t points;            /* live points: content.size()                                   */
+    int64_t capacity;          /* lv_lidar_reserve's capacity (0: not reserved)                  */
+    double oldest_time;        /* content.back().time  (NaN when empty)                          */
+    double newest_time;        /* content.front().time (NaN when empty)                          */
+};
+/* the buffer's fill state; synchronises */
+lv_status lv_lidar_info(lv_handle h, struct lv_lidar_info* out);
+
 /* ---- rosbag reader (format 2.0; replaces roscpp / `rosbag play` in front of Accumulator::receive_lidar / receive_imu,
  * src/main.cpp:27-39, src/Modules/Accumulator.cpp:39-60).  Sequential read of uncompressed bags (bz2 / lz4 chunks are
  * refused with LV_ERR_IO: `rosbag decompress` first).  Host code.                                                       */

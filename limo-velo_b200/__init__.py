@@ -62,6 +62,11 @@ class MapInfo(C.Structure):
                 ("error_flags", C.c_uint32), ("pad_", C.c_uint32)]
 
 
+class LidarInfo(C.Structure):
+    """struct lv_lidar_info: fill state of the LiDAR buffer"""
+    _fields_ = [("points", C.c_int64), ("capacity", C.c_int64), ("oldest_time", C.c_double), ("newest_time", C.c_double)]
+
+
 def build(verbose=False):
     """Compile liblimovelo_b200.so in-tree with nvcc for sm_90a (works without a GPU)."""
     cmd = ["make", "-C", _HERE, "-j8"]
@@ -143,6 +148,13 @@ def lib():
         L.lv_voxelgrid_downsample_device_async.argtypes = [vp, vp, vp, i64, C.c_float, vp, vp]
         L.lv_correct_device_async.argtypes = [vp, vp, vp, i64, i64, C.c_double]
         L.lv_async_status.argtypes = [vp]
+    if hasattr(L, "lv_lidar_reserve"):   # the LiDAR buffer; absent from older builds that tools/ab_bench.py may load
+        L.lv_lidar_reserve.argtypes = [vp, i64]
+        L.lv_lidar_push_device_async.argtypes = [vp, vp, vp, vp, i64]
+        L.lv_lidar_get_points_device_async.argtypes = [vp, C.c_double, C.c_double, vp, vp, i64, vp]
+        L.lv_lidar_get_points_device.argtypes = [vp, C.c_double, C.c_double, vp, vp, i64, C.POINTER(i64)]
+        L.lv_lidar_clear_async.argtypes = [vp, C.c_double]
+        L.lv_lidar_info.argtypes = [vp, C.POINTER(LidarInfo)]
     L.lv_synchronize.argtypes = [vp]
     L.lv_profile_enable.argtypes = [vp, C.c_int]
     L.lv_profile_get.argtypes = [vp, C.POINTER(Profile), C.c_int]
@@ -608,6 +620,37 @@ class Localizer:
         """the deferred errors of the async calls (cleared by the call): returns (status, lv_last_error text); synchronises"""
         st = self.L.lv_async_status(self.h)
         return st, (self.L.lv_last_error().decode() if st != OK else "")
+
+    # the LiDAR buffer (Accumulator::BUFFER_L) in HBM: raw device pointers, counts as int64 in device memory
+    def lidar_reserve(self, capacity):
+        """size the buffer for `capacity` points (the live points stay, in order); synchronises"""
+        return _check(self.L.lv_lidar_reserve(self.h, int(capacity)))
+
+    def lidar_push_async(self, d_xyz, d_time, d_n, n_max):
+        """Accumulator::receive_lidar's push of the *d_n processed points (e.g. lv_process_cloud_device_async's output)"""
+        return _check(self.L.lv_lidar_push_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_n), int(n_max)))
+
+    def lidar_get_points_async(self, t1, t2, d_xyz, d_time, n_max, d_n_out):
+        """Accumulator::get_points(t1, t2) into device buffers of n_max points; the count goes to d_n_out"""
+        return _check(self.L.lv_lidar_get_points_device_async(self.h, float(t1), float(t2), C.c_void_p(d_xyz), C.c_void_p(d_time),
+                                                              int(n_max), C.c_void_p(d_n_out)))
+
+    def lidar_get_points(self, t1, t2, d_xyz, d_time, n_max):
+        """the same, synchronising: returns the count (raises on a window above n_max)"""
+        n = C.c_int64(0)
+        _check(self.L.lv_lidar_get_points_device(self.h, float(t1), float(t2), C.c_void_p(d_xyz), C.c_void_p(d_time), int(n_max),
+                                                 C.byref(n)))
+        return n.value
+
+    def lidar_clear_async(self, t):
+        """Accumulator::clear_lidar(t)"""
+        return _check(self.L.lv_lidar_clear_async(self.h, float(t)))
+
+    def lidar_info(self):
+        """points, capacity, oldest_time, newest_time of the buffer as a dict; synchronises"""
+        out = LidarInfo()
+        _check(self.L.lv_lidar_info(self.h, C.byref(out)))
+        return {k: getattr(out, k) for k, _ in LidarInfo._fields_}
 
     def last_time_updated(self):
         return float(self.L.lv_last_time_updated(self.h))

@@ -18,6 +18,7 @@
 #include "../../include/limovelo_b200.h"
 #include "lv_host.h"
 #include "lv_internal.h"
+#include "lv_lidar_buffer.h"
 #include "lv_predict.h"
 #include "lv_wire.h"
 
@@ -77,6 +78,7 @@ struct lv_context {
     bool time_pending = false;         /* last_time_updated waits for the device's decision (next fetch) */
     bool map_unknown = false;          /* an async add may have left the map without points: the device checks it */
     cudaEvent_t path_copied = nullptr; /* the last H2D copy out of h_path (lv_compensate_device_async returns before it runs) */
+    LidarRing lidar;                   /* Accumulator::BUFFER_L (lv_lidar_reserve) */
     bool use_reuse = true;
     bool use_pdl = true;               /* programmatic dependent launch between the kernels of an update */
     /* Compensator (deskew) staging: lazily allocated */
@@ -336,6 +338,7 @@ void lv_destroy(lv_handle h) {
     if (h->ctrl_copied) cudaEventDestroy(h->ctrl_copied);
     if (h->path_copied) cudaEventDestroy(h->path_copied);
     cudaFree(h->d_async); cudaFreeHost(h->h_async);
+    cudaFree(h->lidar.xyz); cudaFree(h->lidar.time); cudaFree(h->lidar.words); cudaFreeHost(h->lidar.h_words);
     for (cudaEvent_t e : h->snap_ev) if (e) cudaEventDestroy(e);
     cudaFreeHost(h->h_snap);
     cudaFree(h->d_job); cudaFree(h->d_ref); cudaFree(h->d_redo); cudaFree(h->d_imu); cudaFreeHost(h->h_imu);
@@ -1358,11 +1361,150 @@ lv_status lv_async_status(lv_handle h) {
         if (err & kAsyncCloudNaN) msg += "process cloud: a kept point's timestamp is NaN (the time sort has no order for it); ";
         if (err & kAsyncDeskewPath) msg += "compensate: a timestamp lies outside the path or the points are not time-sorted; ";
         if (err & kAsyncCount) msg += "a device point count lies outside [0, n_max] (clamped); ";
+        if (err & kAsyncLidarFull) msg += "lidar push: the points do not fit the buffer's capacity (nothing appended; lv_lidar_reserve); ";
+        if (err & kAsyncLidarWindow) msg += "lidar get points: the window holds more than n_max points (count 0); ";
         msg.resize(msg.size() - 2);
         set_error(msg);
         return LV_ERR_ARG;
     }
     return map_status_from_mirror(h);
+}
+
+/* ---- Accumulator::BUFFER_L (lv_lidar_buffer.cu) ---------------------------------------------------------------------------------- */
+static bool overlaps_lidar(const lv_context* h, const void* p, int64_t bytes) {
+    return ranges_overlap(p, bytes, h->lidar.xyz, 12 * h->lidar.cap) || ranges_overlap(p, bytes, h->lidar.time, 8 * h->lidar.cap) ||
+           ranges_overlap(p, bytes, h->lidar.words, (int64_t)sizeof(LidarWords));
+}
+lv_status lv_lidar_reserve(lv_handle h, int64_t capacity) {
+    if (capacity < 1 || capacity > kLidarMaxCapacity) { set_error("lidar reserve: capacity outside [1, 2^30]"); return LV_ERR_ARG; }
+    if (!h) { set_error("lidar reserve: null handle"); return LV_ERR_ARG; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LidarRing& r = h->lidar;
+    if (!r.words) {
+        LidarWords *d = nullptr, *hw = nullptr;
+        LV_CUDA(cudaMalloc(&d, sizeof(LidarWords)));
+        if (cudaMallocHost(&hw, sizeof(LidarWords)) != cudaSuccess) { cudaFree(d); LV_CUDA(cudaGetLastError()); }
+        r.words = d;
+        r.h_words = hw;
+        LV_CUDA(cudaMemsetAsync(r.words, 0, sizeof(LidarWords), h->stream));
+    }
+    LV_CUDA(cudaMemcpyAsync(r.h_words, r.words, sizeof(LidarWords), cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    if (capacity == r.cap) return LV_OK;
+    const int64_t live = r.h_words->tail - r.h_words->head;
+    if (live > capacity) {
+        char buf[160];
+        snprintf(buf, sizeof(buf), "lidar reserve: %lld points are live, more than a capacity of %lld", (long long)live, (long long)capacity);
+        set_error(buf);
+        return LV_ERR_CAPACITY;
+    }
+    float* xyz = nullptr;
+    double* time = nullptr;
+    cudaError_t e = cudaMalloc(&xyz, sizeof(float) * 3 * (size_t)capacity);
+    if (e == cudaSuccess) e = cudaMalloc(&time, sizeof(double) * (size_t)capacity);
+    int launches = 0;
+    if (e == cudaSuccess) e = launch_lidar_move(r, live, xyz, time, capacity, h->stream, &launches);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) {                                       /* the buffer stays as it was */
+        cudaFree(xyz); cudaFree(time);
+        cudaGetLastError();
+        set_error(std::string("lidar reserve: ") + cudaGetErrorString(e));
+        return LV_ERR_CAPACITY;
+    }
+    h->prof.total_launches += launches;
+    cudaFree(r.xyz); cudaFree(r.time);
+    r.xyz = xyz;
+    r.time = time;
+    r.cap = capacity;
+    return LV_OK;
+}
+lv_status lv_lidar_push_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max) {
+    if (!d_xyz || !d_time || !d_n) { set_error("lidar push: null xyz, time or count"); return LV_ERR_ARG; }
+    if (n_max < 1 || n_max > 0x7fffffff) { set_error("lidar push: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!h) { set_error("lidar push: null handle"); return LV_ERR_ARG; }
+    if (!h->lidar.cap) { set_error("lidar push: the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
+    /* the kernel reads the count and the points while it writes the buffer */
+    if (overlaps_lidar(h, d_xyz, 12 * n_max) || overlaps_lidar(h, d_time, 8 * n_max) || overlaps_lidar(h, d_n, 8)) {
+        set_error("lidar push: an input range overlaps the buffer");
+        return LV_ERR_ARG;
+    }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    int launches = 0;
+    LV_CUDA(launch_lidar_push(h->lidar, d_xyz, d_time, d_n, n_max, &h->d_async->err, h->stream, &launches));
+    h->prof.total_launches += launches;
+    return LV_OK;
+}
+/* the checks and the launch of both forms of get: d_n_out NULL = the synchronous form */
+static lv_status lidar_get_impl(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, const void* count,
+                                int64_t* d_n_out) {
+    if (!d_xyz || !d_time || !count) { set_error("lidar get points: null xyz, time or count"); return LV_ERR_ARG; }
+    if (n_max < 1 || n_max > 0x7fffffff) { set_error("lidar get points: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (isnan(t1) || isnan(t2)) { set_error("lidar get points: t1 or t2 is NaN"); return LV_ERR_ARG; }
+    if (ranges_overlap(d_xyz, 12 * n_max, d_time, 8 * n_max) ||
+        (d_n_out && (ranges_overlap(d_n_out, 8, d_xyz, 12 * n_max) || ranges_overlap(d_n_out, 8, d_time, 8 * n_max)))) {
+        set_error("lidar get points: the output ranges overlap");
+        return LV_ERR_ARG;
+    }
+    if (!h) { set_error("lidar get points: null handle"); return LV_ERR_ARG; }
+    if (!h->lidar.cap) { set_error("lidar get points: the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
+    if (overlaps_lidar(h, d_xyz, 12 * n_max) || overlaps_lidar(h, d_time, 8 * n_max) || (d_n_out && overlaps_lidar(h, d_n_out, 8))) {
+        set_error("lidar get points: an output range overlaps the buffer");
+        return LV_ERR_ARG;
+    }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    int launches = 0;
+    LV_CUDA(launch_lidar_get(h->lidar, t1, t2, d_xyz, d_time, n_max, d_n_out, d_n_out ? &h->d_async->err : nullptr, h->stream, &launches));
+    h->prof.total_launches += launches;
+    return LV_OK;
+}
+lv_status lv_lidar_get_points_device_async(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* d_n_out) {
+    return lidar_get_impl(h, t1, t2, d_xyz, d_time, n_max, d_n_out, d_n_out);
+}
+lv_status lv_lidar_get_points_device(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* n_out) {
+    if (n_out) *n_out = 0;
+    lv_status s = lidar_get_impl(h, t1, t2, d_xyz, d_time, n_max, n_out, nullptr);
+    if (s != LV_OK) return s;
+    LidarRing& r = h->lidar;
+    LV_CUDA(cudaMemcpyAsync(r.h_words, r.words, sizeof(LidarWords), cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    if (r.h_words->window > n_max) {
+        char buf[160];
+        snprintf(buf, sizeof(buf), "lidar get points: the window holds %lld points, more than n_max = %lld", (long long)r.h_words->window,
+                 (long long)n_max);
+        set_error(buf);
+        return LV_ERR_CAPACITY;
+    }
+    *n_out = r.h_words->count;
+    return LV_OK;
+}
+lv_status lv_lidar_clear_async(lv_handle h, double t) {
+    if (isnan(t)) { set_error("lidar clear: t is NaN"); return LV_ERR_ARG; }
+    if (!h) { set_error("lidar clear: null handle"); return LV_ERR_ARG; }
+    if (!h->lidar.cap) { set_error("lidar clear: the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    int launches = 0;
+    LV_CUDA(launch_lidar_clear(h->lidar, t, h->stream, &launches));
+    h->prof.total_launches += launches;
+    return LV_OK;
+}
+lv_status lv_lidar_info(lv_handle h, struct lv_lidar_info* out) {
+    if (!h || !out) { set_error("lidar info: null handle or output"); return LV_ERR_ARG; }
+    const LidarRing& r = h->lidar;
+    out->points = 0;
+    out->capacity = r.cap;
+    out->oldest_time = out->newest_time = NAN;
+    if (!r.cap) return LV_OK;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(cudaMemcpyAsync(r.h_words, r.words, sizeof(LidarWords), cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    const int64_t head = r.h_words->head, tail = r.h_words->tail;
+    out->points = tail - head;
+    if (tail > head) {
+        LV_CUDA(cudaMemcpyAsync(&out->oldest_time, r.time + lidar_slot(head, r.cap), sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        LV_CUDA(cudaMemcpyAsync(&out->newest_time, r.time + lidar_slot(tail - 1, r.cap), sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        LV_CUDA(cudaStreamSynchronize(h->stream));
+    }
+    return LV_OK;
 }
 
 lv_status lv_synchronize(lv_handle h) {

@@ -18,7 +18,7 @@ enum { kNumSMs = 132 };
 
 /* The stream-ordered (_async) entry points report errors through one device word of the handle, read and cleared by
  * lv_async_status.  Bits: */
-enum : uint32_t { kAsyncCloudNaN = 1u, kAsyncDeskewPath = 2u, kAsyncCount = 4u };
+enum : uint32_t { kAsyncCloudNaN = 1u, kAsyncDeskewPath = 2u, kAsyncCount = 4u, kAsyncLidarFull = 8u, kAsyncLidarWindow = 16u };
 /* device words of the async tick: the deferred errors and what lv_correct_device_async decided */
 struct AsyncWords {
     uint32_t err;              /* kAsync* bits since the last lv_async_status              */
@@ -230,6 +230,32 @@ cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const
 int deskew_max_states();
 cudaError_t launch_deskew(const lv_state32* d_path, int ns, const lv_state32& Xt2, double t_lo, double t_hi, const float* d_xyz,
                           const double* d_t, const int64_t* d_n, int64_t n_max, float* d_out, int* d_bad, uint32_t* err, cudaStream_t st);
+
+/* lv_lidar_buffer.cu: Accumulator::BUFFER_L as a ring in HBM (index arithmetic: lv_lidar_buffer.h) */
+struct LidarWords {
+    int64_t head, tail;        /* live positions [head, tail); position p in slot p % cap          */
+    int64_t window;            /* points the last get's window holds (also when above its n_max)    */
+    int64_t count;             /* points the last get wrote (0 when the window was above n_max)     */
+    uint32_t ticket;           /* blocks of a push that have finished                               */
+    uint32_t pad;
+};
+struct LidarRing {
+    float* xyz = nullptr;      /* cap x 3 */
+    double* time = nullptr;    /* cap     */
+    int64_t cap = 0;           /* 0: not reserved yet */
+    LidarWords* words = nullptr;
+    LidarWords* h_words = nullptr;   /* pinned */
+};
+/* push *d_n (clamped to [0, n_max]) points; kAsyncLidarFull and nothing appended when they do not fit */
+cudaError_t launch_lidar_push(const LidarRing& r, const float* xyz, const double* time, const int64_t* d_n, int64_t n_max, uint32_t* err,
+                              cudaStream_t st, int* launches);
+/* Accumulator::get(BUFFER_L, t1, t2) into xyz / time; the count goes to words->count and to *d_n_out (may be NULL); a window
+ * above n_max writes count 0 and raises kAsyncLidarWindow (err may be NULL) */
+cudaError_t launch_lidar_get(const LidarRing& r, double t1, double t2, float* xyz, double* time, int64_t n_max, int64_t* d_n_out, uint32_t* err,
+                             cudaStream_t st, int* launches);
+cudaError_t launch_lidar_clear(const LidarRing& r, double t, cudaStream_t st, int* launches);
+/* copy the `live` live points of `from` into the arrays of a ring of capacity cap (the counters stay as they are) */
+cudaError_t launch_lidar_move(const LidarRing& from, int64_t live, float* xyz, double* time, int64_t cap, cudaStream_t st, int* launches);
 
 }  // namespace lv
 #endif

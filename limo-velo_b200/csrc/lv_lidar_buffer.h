@@ -1,0 +1,62 @@
+/*
+ * lv_lidar_buffer.h — index arithmetic of the device LiDAR buffer: Accumulator::BUFFER_L (include/Headers/Accumulator.hpp:3)
+ * with Buffer::push / clear(t) (src/Objects/Buffer.cpp:26-28,66-70) and Accumulator::get (Accumulator.hpp:61-74).
+ *
+ * The reference keeps a std::deque<Point> that Buffer::push grows at the FRONT: content[0] is the newest point inserted, and
+ * across messages the order is arrival order, not time order.  The device keeps a ring of `cap` slots and two monotonically
+ * increasing 64-bit counters head <= tail: position p (head <= p < tail) lives in slot p % cap, and
+ *
+ *     content[k] = ring[tail - 1 - k],   size = tail - head,   content.back() = ring[head].
+ *
+ * Everything here compiles for the device (lv_lidar_buffer.cu) and for the host (tests/cpu_shim_buffer, test-only), so the
+ * kernels and the host build share the probe sequence of the binary search and the predicates of the walk and of clear.
+ * Comparisons are written exactly as in the reference, so a NaN point time behaves as it does there.
+ */
+#ifndef LV_LIDAR_BUFFER_H_
+#define LV_LIDAR_BUFFER_H_
+
+#include <stdint.h>
+
+#include "lv_hd.h"
+
+namespace lv {
+
+/* the largest ring: the reference's indices are `int`, and (low + high) of its binary search must not overflow */
+enum : int64_t { kLidarMaxCapacity = (int64_t)1 << 30 };
+
+LV_HD int64_t lidar_slot(int64_t p, int64_t cap) { return p % cap; }
+/* ring position of content[k] */
+LV_HD int64_t lidar_pos(int64_t tail, int64_t k) { return tail - 1 - k; }
+/* Buffer::push of n points keeps the ring's content only if they fit */
+LV_HD bool lidar_fits(int64_t head, int64_t tail, int64_t n, int64_t cap) { return tail + n - head <= cap; }
+
+/* Algorithms::binary_search(content, t, desc = true) (include/Headers/Utils.hpp:9-23), probe for probe: on content that is
+ * not sorted (a late or overlapping message) the answer depends on exactly which elements it reads */
+LV_HD int64_t lidar_binary_search(const double* time, int64_t cap, int64_t head, int64_t tail, double t) {
+    int64_t low = 0, high = (tail - head) - 1;
+    while (high >= low) {
+        const int64_t mid = (low + high) / 2;
+        (time[lidar_slot(lidar_pos(tail, mid), cap)] < t) ? high = mid - 1 : low = mid + 1;
+    }
+    if (--high < 0) return 0;
+    return high;
+}
+
+/* Accumulator::get: the walk starts at k_t2 = max(0, binary_search(content, t2)), i.e. at this ring position; on an empty
+ * buffer it is head - 1 (nothing to walk) */
+LV_HD int64_t lidar_window_top(const double* time, int64_t cap, int64_t head, int64_t tail, double t2) {
+    int64_t k = lidar_binary_search(time, cap, head, tail, t2);
+    if (k < 0) k = 0;
+    return lidar_pos(tail, k);
+}
+/* `if (t1 > cnt.time) break;` — the walk goes from the top to lower positions: it stops at the highest position <= top
+ * for which this holds */
+LV_HD bool lidar_breaks(double time, double t1) { return t1 > time; }
+/* `if (t2 >= cnt.time) result.push_front(cnt);` — kept points come out in ascending position (oldest inserted first) */
+LV_HD bool lidar_keeps(double time, double t2) { return t2 >= time; }
+/* Buffer::clear(t): `while (size > 0 and t >= back().time) pop_back();` — head advances to the lowest position for which
+ * this fails (a NaN time stops it, as it stops the loop) */
+LV_HD bool lidar_pops(double time, double t) { return t >= time; }
+
+}  // namespace lv
+#endif

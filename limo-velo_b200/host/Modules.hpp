@@ -196,10 +196,38 @@ class Compensator {
     Context& ctx;
 };
 
-/* Plain time-ordered buffers (Accumulator.hpp:61-74), fed by a reader instead of ROS callbacks. */
+/* Plain time-ordered buffers (Accumulator.hpp:61-74), fed by a reader instead of ROS callbacks; with a Context the LiDAR buffer
+ * (BUFFER_L) lives in HBM instead (lv_lidar_*), so the tick reads like main.cpp:61-122:
+ *
+ *     accum.receive_lidar_device(msg);                                  // Accumulator.cpp:39-48: process -> push, on the device
+ *     ... t2, delta, t1 = max(t2 - delta, loc.last_time_updated); if (t2 - t1 < delta - 1e-6) break;   (host, main.cpp:61-71)
+ *     accum.get_points_device(t1, t2, d_xyz, d_time, n_max, d_n);        // Compensator.cpp:23
+ *     lv_compensate_device_async(...); lv_voxelgrid_downsample_device_async(...); lv_correct_device_async(...); ...
+ *     accum.clear_lidar(t2 - empty_lidar_time);                         // main.cpp:122
+ */
 class Accumulator {
    public:
+    Accumulator() = default;
+    explicit Accumulator(Context& c, int64_t lidar_capacity) : ctx(&c) { check(lv_lidar_reserve(c.h, lidar_capacity), "Accumulator"); }
     void receive_lidar(const Points& sweep) { points = sweep; }                /* Accumulator.cpp:39-48 */
+    /* Accumulator::receive_lidar on the message's bytes in device memory: Accumulator::process (lv_process_cloud_device_async into
+     * the caller's scratch d_xyz / d_time / d_n, room for msg_n points) -> every point pushed onto BUFFER_L; no host wait */
+    struct DeviceMessage {
+        lv_lidar_type type; const lv_cloud_layout* layout; const uint8_t* d_data; int64_t data_bytes, n; uint64_t stamp_us;
+        int stamp_beginning, offset_beginning; double full_rotation_time; int32_t downsample_rate; double min_dist;
+    };
+    void receive_lidar_device(const DeviceMessage& m, float* d_xyz, double* d_time, int64_t* d_n) {
+        check(lv_process_cloud_device_async(ctx->h, m.type, m.layout, m.d_data, m.data_bytes, m.n, m.stamp_us, m.stamp_beginning,
+                                            m.offset_beginning, m.full_rotation_time, m.downsample_rate, m.min_dist, d_xyz, d_time,
+                                            nullptr, nullptr, nullptr, d_n),
+              "Accumulator::receive_lidar_device");
+        if (m.n > 0) check(lv_lidar_push_device_async(ctx->h, d_xyz, d_time, d_n, m.n), "Accumulator::receive_lidar_device");
+    }
+    /* Accumulator::get_points(t1, t2) (Accumulator.hpp:61-74) into device buffers of n_max points; the count goes to *d_n_out */
+    void get_points_device(double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* d_n_out) {
+        check(lv_lidar_get_points_device_async(ctx->h, t1, t2, d_xyz, d_time, n_max, d_n_out), "Accumulator::get_points_device");
+    }
+    void clear_lidar(double t) { check(lv_lidar_clear_async(ctx->h, t), "Accumulator::clear_lidar"); }   /* Accumulator.cpp:68-70 */
     void receive_imu(const IMU& imu) { imus.push_back(imu); }
     IMUs get_imus(double t1, double t2) {
         IMUs out;
@@ -208,6 +236,9 @@ class Accumulator {
     }
     Points points;
     IMUs imus;
+
+   private:
+    Context* ctx = nullptr;
 };
 
 }  // namespace lv

@@ -58,3 +58,21 @@ for lidar in ("velodyne", "ouster"):
                   T.host_process(lv, lidar, pts, T.STAMP_US, False, True, 0.1, 4, 3.0), lidar)
 loc.close()
 print("sanitize target: process cloud ok", flush=True)
+
+# the LiDAR buffer (lv_lidar_*): a ring that wraps, ties at t2, a late message, clears, against the restatement
+import lidar_buffer_ref as R
+from test_gpu_lidar_buffer import DeviceBuffer, same_window, velodyne_message
+loc = lv.Localizer(lv.default_params(max_points=1 << 13, max_map_points=1 << 13))
+dev, ref = DeviceBuffer(loc, 2000, n_max=4096), R.LidarBuffer()
+for j in range(8):
+    xyz, t = velodyne_message(rng, 1.0 + 0.01 * j - (0.03 if j == 5 else 0.0), 8)
+    if ref.size() + len(t) > 2000:
+        ref.clear(1.0 + 0.01 * j - 0.02)
+        loc.lidar_clear_async(1.0 + 0.01 * j - 0.02)
+    dev.push(xyz, t)
+    ref.push_message(xyz, t)
+    same_window(lv, dev, ref, float(t[0]), float(t[-1]), j)
+assert loc.async_status() == (lv.OK, "")
+dev.close()
+loc.close()
+print("sanitize target: lidar buffer ok", flush=True)
