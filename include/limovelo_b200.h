@@ -402,6 +402,23 @@ lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, 
  * (main.cpp:81 breaks before map.add), the first tick's build included; its growth bound (lv_map_set_growth) uses n_max. */
 lv_status lv_correct_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int64_t min_points,
                                   double time);
+/* ---- the tick's output and mapping step (main.cpp:88-117) without a host wait.  Stream-ordered like the calls above: counts in
+ * device memory, n_max in [1, min(max_points, 2^31 - 1)], argument errors LV_ERR_ARG before any device work (a null handle too),
+ * deferred errors through lv_async_status.  Whether to publish, map online or map offline (mapping_online, high_quality_publish,
+ * Mapper::hasToMap with full_rotation_time) stays with the caller, as does the time management. */
+/* `Xt2 * Xt2.I_Rt_L() * points` (main.cpp:91-93, 111; State.cpp:79-89) in fp32 with the filter state on the device: the state the
+ * preceding update left, or the propagated state when there was none (an empty map, Localizator.cpp:24).  The same arithmetic and
+ * the same kernel as lv_map_add_last_sweep's transform and Mapper::match's.  *d_n points (clamped to [0, n_max]) of d_xyz_lidar
+ * (n_max x 3) go to d_xyz_world; *d_n_out = their count, or 0 when the preceding lv_correct_device_async's gate stopped the tick
+ * (main.cpp:81 breaks before publishing), the rule lv_map_add_last_sweep follows.  d_xyz_world may equal d_xyz_lidar and d_n_out
+ * may equal d_n; other overlaps of the outputs with the inputs are refused.  Two launches. */
+lv_status lv_sweep_to_world_device_async(lv_handle h, const float* d_xyz_lidar, const int64_t* d_n, int64_t n_max, float* d_xyz_world,
+                                         int64_t* d_n_out);
+/* Mapper::add (Mapper.cpp:22-30) of *d_n points (clamped to [0, n_max]) of d_xyz (device, world frame): nothing when the count is
+ * 0; a map without points is built without downsampling, else Add_Points with the 0.2 m rule when downsample != 0.  No gate of its
+ * own.  Content, point ids, order and lv_map_info counters equal those of lv_map_add_device with the count on the host; the growth
+ * bound (lv_map_set_growth) uses n_max. */
+lv_status lv_map_add_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int downsample);
 /* the deferred errors of the _async calls since the last lv_async_status, and the map's capacity flags (as lv_map_status):
  * LV_ERR_ARG (lv_last_error names the stage), LV_ERR_CAPACITY or LV_OK.  Clears them; the handle stays usable.  Synchronises. */
 lv_status lv_async_status(lv_handle h);

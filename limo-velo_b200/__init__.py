@@ -155,6 +155,9 @@ def lib():
         L.lv_lidar_get_points_device.argtypes = [vp, C.c_double, C.c_double, vp, vp, i64, C.POINTER(i64)]
         L.lv_lidar_clear_async.argtypes = [vp, C.c_double]
         L.lv_lidar_info.argtypes = [vp, C.POINTER(LidarInfo)]
+    if hasattr(L, "lv_sweep_to_world_device_async"):   # the tick's output and mapping step; absent from older builds
+        L.lv_sweep_to_world_device_async.argtypes = [vp, vp, vp, i64, vp, vp]
+        L.lv_map_add_device_async.argtypes = [vp, vp, vp, i64, C.c_int]
     L.lv_synchronize.argtypes = [vp]
     L.lv_profile_enable.argtypes = [vp, C.c_int]
     L.lv_profile_get.argtypes = [vp, C.POINTER(Profile), C.c_int]
@@ -615,6 +618,15 @@ class Localizer:
         map is empty, else LV_OK (the update's own status is fetched later, e.g. by last_logs)"""
         return _check(self.L.lv_correct_device_async(self.h, C.c_void_p(d_ptr), C.c_void_p(d_n), int(n_max), int(min_points),
                                                      float(time)), allow=(EMPTY_MAP,))
+
+    def sweep_to_world_async(self, d_xyz_lidar, d_n, n_max, d_xyz_world, d_n_out):
+        """Xt2 * Xt2.I_Rt_L() * the *d_n points with the filter state on the device; the count goes to d_n_out (0 on a gated tick)"""
+        return _check(self.L.lv_sweep_to_world_device_async(self.h, C.c_void_p(d_xyz_lidar), C.c_void_p(d_n), int(n_max),
+                                                            C.c_void_p(d_xyz_world), C.c_void_p(d_n_out)))
+
+    def map_add_device_async(self, d_xyz, d_n, n_max, downsample=True):
+        """Mapper::add of the *d_n world-frame points of a device buffer (built un-downsampled on an empty map)"""
+        return _check(self.L.lv_map_add_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_n), int(n_max), int(downsample)))
 
     def async_status(self):
         """the deferred errors of the async calls (cleared by the call): returns (status, lv_last_error text); synchronises"""

@@ -535,22 +535,23 @@ lv_status lv_map_info(lv_handle h, struct lv_map_info* out) {
     return LV_OK;
 }
 
-static lv_status map_build_device_impl(lv_context* h, const float* d_xyz, int64_t m) {
+/* m, n: the points, or with cnt.n the host bound of their device count */
+static lv_status map_build_device_impl(lv_context* h, const float* d_xyz, int64_t m, const MapAddCount& cnt = MapAddCount()) {
     EventPair ep;
     const bool pr = prof_begin(h, 2, &ep);
     int launches = 0;
     LV_CUDA(map_clear(h->map, h->stream, &launches));
-    LV_CUDA(map_add(h->map, d_xyz, m, 0, h->stream, &launches));              /* Build: no downsampling (Mapper.cpp:68-71) */
+    LV_CUDA(map_add(h->map, d_xyz, m, 0, h->stream, &launches, cnt));         /* Build: no downsampling (Mapper.cpp:68-71) */
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
     snap_reset_cleared(h);
     return snap_after_add(h, m);
 }
-static lv_status map_add_device_impl(lv_context* h, const float* d_xyz, int64_t n, int downsample) {
+static lv_status map_add_device_impl(lv_context* h, const float* d_xyz, int64_t n, int downsample, const MapAddCount& cnt = MapAddCount()) {
     EventPair ep;
     const bool pr = prof_begin(h, 2, &ep);
     int launches = 0;
-    LV_CUDA(map_add(h->map, d_xyz, n, downsample ? 1 : 0, h->stream, &launches));
+    LV_CUDA(map_add(h->map, d_xyz, n, downsample ? 1 : 0, h->stream, &launches, cnt));
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
     return snap_after_add(h, n);
@@ -621,9 +622,29 @@ lv_status lv_map_add_device(lv_handle h, const float* d_xyz, int64_t n, int down
     if (h->map.empty) return map_build_device_impl(h, d_xyz, n);
     return map_add_device_impl(h, d_xyz, n, downsample);
 }
+lv_status lv_map_add_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int downsample) {
+    if (!d_xyz || !d_n) { set_error("map add async: null points or count"); return LV_ERR_ARG; }
+    if (n_max < 1 || n_max > 0x7fffffff) { set_error("map add async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!h) { set_error("map add async: null handle"); return LV_ERR_ARG; }
+    if (n_max > h->prm.max_points) { set_error("map add async: n_max above max_points"); return LV_ERR_ARG; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    const bool build = h->map.empty;
+    lv_status s = grow_before_add(h, n_max, build);
+    if (s != LV_OK) return s;
+    /* Mapper.cpp:22-30: *d_n points, none when it is 0; a map without points (also one an earlier device count left empty) is
+     * built without downsampling.  The add capacity is at least max_points, so n_max always fits. */
+    MapAddCount cnt;
+    cnt.n = d_n;
+    cnt.build_if_empty = 1;
+    cnt.err = &h->d_async->err;
+    if (!build) return map_add_device_impl(h, d_xyz, n_max, downsample, cnt);
+    h->map_unknown = true;                                        /* a count of 0 leaves the build without a point */
+    return map_build_device_impl(h, d_xyz, n_max, cnt);
+}
 
 /* ---- the tick on the device: main.cpp:99-105 ------------------------------------------------- */
 static lv_status upload_state(lv_context* h, const double* x, const double* P);
+static bool ranges_overlap(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes);
 /* n: the sweep's points, or with cnt.n the host bound of its device count */
 static lv_status add_sweep_impl(lv_context* h, const float* d_xyz_lidar, int64_t n, int downsample, const MapAddCount& cnt = MapAddCount()) {
     if (h->state_dirty) {                                         /* the transform uses the device copy of the state */
@@ -663,6 +684,34 @@ lv_status lv_map_add_last_sweep(lv_handle h, int downsample) {
     cnt.build_if_empty = 1;
     cnt.err = &h->d_async->err;
     return add_sweep_impl(h, h->last_sweep, h->last_sweep_n, downsample, cnt);
+}
+lv_status lv_sweep_to_world_device_async(lv_handle h, const float* d_xyz_lidar, const int64_t* d_n, int64_t n_max, float* d_xyz_world,
+                                         int64_t* d_n_out) {
+    if (!d_xyz_lidar || !d_n || !d_xyz_world || !d_n_out) { set_error("sweep to world: null input, count, output or output count"); return LV_ERR_ARG; }
+    if (n_max < 1 || n_max > 0x7fffffff) { set_error("sweep to world: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    /* one thread reads a point and then writes the same point: in place is fine, a shifted overlap is not.  The counts are read
+     * and written by one thread before any point: the output count may equal the input count, but not lie among the points. */
+    const int64_t b = 12 * n_max;
+    if ((d_xyz_world != d_xyz_lidar && ranges_overlap(d_xyz_world, b, d_xyz_lidar, b)) || ranges_overlap(d_n_out, 8, d_xyz_lidar, b) ||
+        ranges_overlap(d_n_out, 8, d_xyz_world, b) || ranges_overlap(d_n, 8, d_xyz_world, b) ||
+        (d_n_out != d_n && ranges_overlap(d_n_out, 8, d_n, 8))) {
+        set_error("sweep to world: an output range overlaps another range");
+        return LV_ERR_ARG;
+    }
+    if (!h) { set_error("sweep to world: null handle"); return LV_ERR_ARG; }
+    if (n_max > h->prm.max_points) { set_error("sweep to world: n_max above max_points"); return LV_ERR_ARG; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    if (h->state_dirty) {                                         /* the transform uses the device copy of the state */
+        lv_status s = upload_state(h, h->x, h->P);
+        if (s != LV_OK) return s;
+        h->state_dirty = false;
+    }
+    /* after lv_correct_device_async its gate decides for the whole tick, as for lv_map_add_last_sweep */
+    int launches = 0;
+    LV_CUDA(launch_sweep_to_world(h->d_ctrl, d_xyz_lidar, d_n, n_max, h->last_sweep_dn, h->last_sweep_n, h->last_sweep_min, d_xyz_world, d_n_out,
+                                  &h->d_async->world_n, &h->d_async->err, h->stream, &launches));
+    h->prof.total_launches += launches;
+    return LV_OK;
 }
 
 /* ---- state ----------------------------------------------------------------------------------- */

@@ -24,6 +24,8 @@ struct AsyncWords {
     uint32_t err;              /* kAsync* bits since the last lv_async_status              */
     int32_t time_set;          /* 1: an async update ran since the last fetch; time_updated is its time */
     double time_updated;
+    uint32_t world_n;          /* the count lv_sweep_to_world_device_async's transform reads */
+    uint32_t pad;
 };
 #ifdef __CUDACC__
 /* a count in device memory (NULL: the host-known n_max) clamped to [0, n_max]; one thread flags a count outside it */
@@ -155,6 +157,12 @@ cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample
 /* the sweep (LiDAR frame, device) transformed by the state in d_ctrl->x, then map_add: main.cpp:99-105 without leaving the GPU */
 cudaError_t map_add_sweep(MapBuffers& b, const UpdateCtrl* d_ctrl, const float* d_xyz_lidar, int64_t n, int downsample, cudaStream_t st,
                           int* launches, const MapAddCount& cnt = MapAddCount());
+/* main.cpp:91-93 (lv_sweep_to_world_device_async): *d_n points (clamped to [0, n_max]) of d_xyz (LiDAR frame) transformed by the
+ * state in d_ctrl->x into d_out (may equal d_xyz); *d_n_out and *count (a device word the transform reads) = that count, or 0 when
+ * gate_n is given and its count (clamped to [0, gate_max]) is below max(gate_min, 1) (main.cpp:81 breaks before publishing) */
+cudaError_t launch_sweep_to_world(const UpdateCtrl* d_ctrl, const float* d_xyz, const int64_t* d_n, int64_t n_max, const int64_t* gate_n,
+                                  int64_t gate_max, int64_t gate_min, float* d_out, int64_t* d_n_out, uint32_t* count, uint32_t* err,
+                                  cudaStream_t st, int* launches);
 cudaError_t map_fetch_counters(MapBuffers& b, cudaStream_t st);
 cudaError_t map_points_sorted(MapBuffers& b, float* host_out, int64_t cap, int64_t* n_out, cudaStream_t st);
 VoxelMapView map_view(const MapBuffers& b);

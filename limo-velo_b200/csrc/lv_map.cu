@@ -177,15 +177,16 @@ __global__ void __launch_bounds__(256) lv_map_unpack_kernel(const float4* __rest
     xyz[3 * (size_t)i] = p.x; xyz[3 * (size_t)i + 1] = p.y; xyz[3 * (size_t)i + 2] = p.z;
 }
 
-/* main.cpp:99-105 on the device: the sweep (LiDAR frame) in world coordinates with the state the update just produced,
- * Xt2 * Xt2.I_Rt_L() * p in fp32 (State.cpp:79-89, RotTransl.cpp:36-48) — the very transform Mapper::match applies */
-__global__ void __launch_bounds__(256) lv_sweep_to_world_kernel(const UpdateCtrl* __restrict__ c, const float* __restrict__ xyz,
-                                                                 const uint32_t* __restrict__ counters, float* __restrict__ out) {
+/* main.cpp:91-93,99-105 on the device: a cloud (LiDAR frame) in world coordinates with the state the update just produced,
+ * Xt2 * Xt2.I_Rt_L() * p in fp32 (State.cpp:79-89, RotTransl.cpp:36-48) — the very transform Mapper::match applies.
+ * *count points: the map add's (kCtrAddN) or lv_sweep_to_world_device_async's (lv_world_count_kernel).  xyz may equal out. */
+__global__ void __launch_bounds__(256) lv_sweep_to_world_kernel(const UpdateCtrl* __restrict__ c, const float* xyz,
+                                                                 const uint32_t* __restrict__ count, float* out) {
     __shared__ Frame s_frame;
     if (threadIdx.x == 0) make_frame(c->x, &s_frame);
     __syncthreads();
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= counters[kCtrAddN]) return;
+    if (i >= *count) return;
     float g[3];
     rt_apply(s_frame.lidar_to_world, xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2], g);
     out[3 * (size_t)i] = g[0]; out[3 * (size_t)i + 1] = g[1]; out[3 * (size_t)i + 2] = g[2];
@@ -379,7 +380,7 @@ cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample
     const unsigned blocks = (unsigned)((n + 255) / 256);
     lv_map_begin_kernel<<<1, 32, 0, st>>>(b.counters, n, cnt.n, cnt.min_points, cnt.build_if_empty, cnt.err);
     if (to_world) {
-        lv_sweep_to_world_kernel<<<blocks, 256, 0, st>>>(to_world, d_xyz, b.counters, b.stage_xyz);
+        lv_sweep_to_world_kernel<<<blocks, 256, 0, st>>>(to_world, d_xyz, b.counters + kCtrAddN, b.stage_xyz);
         d_xyz = b.stage_xyz;
         if (launches) *launches += 1;
     }
@@ -403,6 +404,25 @@ cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample
 cudaError_t map_add_sweep(MapBuffers& b, const UpdateCtrl* d_ctrl, const float* d_xyz_lidar, int64_t n, int downsample, cudaStream_t st,
                           int* launches, const MapAddCount& cnt) {
     return map_add(b, d_xyz_lidar, n, b.empty ? 0 : downsample, st, launches, cnt, d_ctrl);
+}
+
+/* one thread reads every count before it writes: d_n_out may equal d_n or the gate's count */
+__global__ void lv_world_count_kernel(const int64_t* d_n, int64_t n_max, const int64_t* gate_n, int64_t gate_max, int64_t gate_min,
+                                      uint32_t* count, int64_t* d_n_out, uint32_t* err) {
+    if (threadIdx.x != 0) return;
+    int64_t k = device_count(d_n, n_max, err);
+    if (gate_n && device_count(gate_n, gate_max, nullptr) < (gate_min > 1 ? gate_min : 1)) k = 0;   /* main.cpp:81 */
+    *count = (uint32_t)k;
+    *d_n_out = k;
+}
+
+cudaError_t launch_sweep_to_world(const UpdateCtrl* d_ctrl, const float* d_xyz, const int64_t* d_n, int64_t n_max, const int64_t* gate_n,
+                                  int64_t gate_max, int64_t gate_min, float* d_out, int64_t* d_n_out, uint32_t* count, uint32_t* err,
+                                  cudaStream_t st, int* launches) {
+    lv_world_count_kernel<<<1, 32, 0, st>>>(d_n, n_max, gate_n, gate_max, gate_min, count, d_n_out, err);
+    lv_sweep_to_world_kernel<<<(unsigned)((n_max + 255) / 256), 256, 0, st>>>(d_ctrl, d_xyz, count, d_out);
+    if (launches) *launches += 2;
+    return cudaGetLastError();
 }
 
 /* device counters -> pinned mirror; the caller synchronises the stream before reading b.h_counters */

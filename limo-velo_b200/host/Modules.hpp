@@ -84,6 +84,20 @@ class Mapper {
         check(lv_map_add_last_sweep(ctx.h, downsample ? 1 : 0), "Mapper::add_corrected_sweep");
         last_map_time = time;
     }
+    /* Mapper::add of a device cloud whose count is on the device (lv_map_add_device_async), e.g. main.cpp:111-114's
+     * global_full_ds_compensated.  The reference skips an empty cloud without touching last_map_time; the host does not know the
+     * count here, so last_map_time becomes `time` either way (a full rotation of LiDAR data is not empty in practice). */
+    void add_device(const float* d_xyz, const int64_t* d_n, int64_t n_max, double time, bool downsample = true) {
+        check(lv_map_add_device_async(ctx.h, d_xyz, d_n, n_max, downsample ? 1 : 0), "Mapper::add_device");
+        last_map_time = time;
+    }
+    /* Mapper.cpp:58-61: with mapping_online false, whether the tick at t maps the last full rotation */
+    double full_rotation_time = 0.1;                                            /* Config.full_rotation_time (YAML) */
+    bool hasToMap(double t) { return has_to_map(last_map_time, t, full_rotation_time); }
+    static bool has_to_map(double& last_map_time, double t, double full_rotation_time) {
+        if (last_map_time < 0) last_map_time = t;
+        return t - last_map_time >= full_rotation_time;
+    }
     /* the ikd-Tree has no capacity (ikd_Tree.cpp:478-573): grow the device map now to hold `points`, or let it grow by itself
      * before the adds that may not fit, up to `max_points` (0: off) — lv_map_reserve / lv_map_set_growth */
     void reserve(int64_t points) { check(lv_map_reserve(ctx.h, points), "Mapper::reserve"); }
@@ -143,6 +157,12 @@ class Localizator {
         if (s != LV_TOO_FEW_MATCHES) check(s, "Localizator::correct");
         last_time_updated = time;
         return n_evals;
+    }
+    /* `Xt2 * Xt2.I_Rt_L() * points` (main.cpp:91-93, 111) on the device with the state the last correct left there
+     * (lv_sweep_to_world_device_async): global_ds_compensated and global_compensated for the publishers, or the full rotation of
+     * the offline map add.  *d_n_out = 0 when the MAX_POINTS2MATCH gate of correct_device_async stopped the tick. */
+    void to_world_device(const float* d_xyz_lidar, const int64_t* d_n, int64_t n_max, float* d_xyz_world, int64_t* d_n_out) {
+        check(lv_sweep_to_world_device_async(ctx.h, d_xyz_lidar, d_n, n_max, d_xyz_world, d_n_out), "Localizator::to_world_device");
     }
     State latest_state() {                                                     /* Localizator.cpp:77-98 */
         State s;

@@ -3,7 +3,10 @@
  * reader: propagate_to -> compensate -> downsample -> correct -> map.add, with LIMO-Velo's module
  * names (Modules.hpp) on top of liblimovelo_b200.so.
  *
- *   limovelo_synth <config.yaml> [sweeps=10] [map_points=200000] [rings=64] [azimuths=1024] [downsample_leaf=0]
+ *   limovelo_synth <config.yaml> [sweeps=10] [map_points=200000] [rings=64] [azimuths=1024] [downsample_leaf=0] [mapping_online=1]
+ *
+ * mapping_online=0 runs main.cpp:106-117 instead of the online map add: once per full_rotation_time the last full rotation goes to
+ * the world frame, through the voxel grid (when a leaf is given) and into the map, on the device.
  */
 #include <math.h>
 #include <stdio.h>
@@ -15,11 +18,15 @@
 #include "Modules.hpp"
 
 int main(int argc, char** argv) {
-    if (argc < 2) { fprintf(stderr, "usage: %s config.yaml [sweeps] [map_points] [rings] [azimuths] [downsample_leaf]\n", argv[0]); return 2; }
+    if (argc < 2) {
+        fprintf(stderr, "usage: %s config.yaml [sweeps] [map_points] [rings] [azimuths] [downsample_leaf] [mapping_online]\n", argv[0]);
+        return 2;
+    }
     const int sweeps = argc > 2 ? atoi(argv[2]) : 10;
     const int64_t map_points = argc > 3 ? atoll(argv[3]) : 200000;
     const int rings = argc > 4 ? atoi(argv[4]) : 64, azimuths = argc > 5 ? atoi(argv[5]) : 1024;
     const float leaf = argc > 6 ? (float)atof(argv[6]) : 0.f;
+    const bool mapping_online = argc > 7 ? atoi(argv[7]) != 0 : true;
     try {
         lv_params prm;
         lv_default_params(&prm);
@@ -48,6 +55,13 @@ int main(int argc, char** argv) {
         lv::check(lv_get_state(ctx.h, nullptr, P0), "P0");
 
         std::vector<float> sw(3 * (size_t)rings * azimuths);
+        /* mapping offline: the full rotation (device), its world-frame copy and its voxel grid, each with a device count */
+        const int64_t n_sweep = (int64_t)rings * azimuths;
+        float* d_full = (float*)lv_device_alloc(ctx.h, 12 * n_sweep);
+        float* d_world = (float*)lv_device_alloc(ctx.h, 12 * n_sweep);
+        float* d_ds = (float*)lv_device_alloc(ctx.h, 12 * n_sweep);
+        int64_t* d_counts = (int64_t*)lv_device_alloc(ctx.h, 3 * sizeof(int64_t));
+        if (!d_full || !d_world || !d_ds || !d_counts) throw std::runtime_error("device buffers for mapping offline");
         for (int k = 0; k < sweeps; ++k) {
             const double t2 = 0.1 * (k + 1);
             lv_synth_pose(world, 10.0 + 1.5 * (k + 1), &prm, truth);   /* 15 m/s at 10 Hz */
@@ -79,13 +93,28 @@ int main(int argc, char** argv) {
             const int evals = loc.correct(ds, t2);                    /* main.cpp:84 */
             /* main.cpp:101-105: the sweep joins the map in the world frame of the corrected state, under the 0.2 m rule —
              * on the device, with the state the update left there (no copy of the sweep, no copy of the state) */
-            map.add_corrected_sweep(t2, true);
+            if (mapping_online) map.add_corrected_sweep(t2, true);
+            else if (map.hasToMap(t2)) {                              /* main.cpp:106-117 */
+                /* the synthetic sweep is one full rotation, deskewed at t2: [t2 - full_rotation_time, t2] */
+                const int64_t n_full = (int64_t)accum.points.size();
+                lv::check(lv_memcpy_h2d(ctx.h, d_full, sw.data(), 12 * n_full), "full rotation");
+                lv::check(lv_memcpy_h2d(ctx.h, d_counts, &n_full, sizeof(int64_t)), "full rotation");
+                loc.to_world_device(d_full, d_counts, n_sweep, d_world, d_counts + 1);
+                if (leaf > 0.f) {
+                    lv::check(lv_voxelgrid_downsample_device_async(ctx.h, d_world, d_counts + 1, n_sweep, leaf, d_ds, d_counts + 2),
+                              "Compensator::downsample");
+                    map.add_device(d_ds, d_counts + 2, n_sweep, t2, true);
+                } else {
+                    map.add_device(d_world, d_counts + 1, n_sweep, t2, true);
+                }
+            }
             const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
             lv::State X = loc.latest_state();
             const double err = sqrt(pow(X.x[0] - truth[0], 2) + pow(X.x[1] - truth[1], 2) + pow(X.x[2] - truth[2], 2));
             printf("sweep %2d  t=%.1f  points=%zu  evals=%d  Nm=%lld  correct()+map.add()=%.3f ms  |pos error|=%.4f m  map=%d\n", k, t2, ds.size(), evals,
                    evals ? (long long)loc.logs[evals - 1].n_matches : 0LL, ms, err, map.size());
         }
+        for (void* p : {(void*)d_full, (void*)d_world, (void*)d_ds, (void*)d_counts}) lv_device_free(ctx.h, p);
         lv_synth_world_destroy(world);
     } catch (const std::exception& e) {
         fprintf(stderr, "limovelo_synth: %s\n", e.what());
