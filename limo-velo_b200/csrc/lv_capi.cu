@@ -43,7 +43,9 @@ static void set_error(const std::string& s) { g_last_error = s; }
         }                                                                                        \
     } while (0)
 
-struct EventPair { cudaEvent_t a, b; int kind; int upd; int slot; };   /* kind 0 measure, 1 solve, 2 build, 3 search, 4 search-upper, 5 fit */
+/* what an event pair times; search, search-upper and fit are in the order of launch_measure's probe stages 0, 1, 2 */
+enum ProfKind { kProfSolve, kProfMap, kProfSearch, kProfSearchUpper, kProfFit, kProfReuse };
+struct EventPair { cudaEvent_t a, b; ProfKind kind; int upd; int slot; };
 enum { kNevalsRing = 4096 };
 
 struct lv_context {
@@ -68,10 +70,13 @@ struct lv_context {
      * the update), so the next refill of the pinned buffer waits for this event, not for the whole stream */
     cudaEvent_t imu_copied = nullptr;
     cudaEvent_t ctrl_copied = nullptr;
-    int64_t last_sweep_n = 0;          /* points of the sweep d_sweep holds (lv_correct / lv_measure*), for lv_map_add_last_sweep */
-    const float* last_sweep = nullptr; /* device pointer of the sweep of the last update */
-    const int64_t* last_sweep_dn = nullptr;   /* lv_correct_device_async: its device count (last_sweep_n is then the bound) ... */
-    int64_t last_sweep_min = 0;               /* ... and its min_points */
+    /* the sweep of the last update (correct_enqueue), for lv_map_add_last_sweep and lv_sweep_to_world_device_async */
+    struct TickSweep {
+        const float* xyz = nullptr;    /* device pointer */
+        int64_t n = 0;                 /* its points, or with d_n the host bound of its device count */
+        const int64_t* d_n = nullptr;  /* lv_correct_device_async: the device count ... */
+        int64_t min_points = 0;        /* ... and its MAX_POINTS2MATCH gate */
+    } tick;
     /* the async tick: deferred errors and the time of the last update that ran (lv_correct_device_async) */
     AsyncWords* d_async = nullptr;
     AsyncWords* h_async = nullptr;     /* pinned */
@@ -152,22 +157,21 @@ static lv_status drain_events(lv_context* h) {
         /* launches enqueued after the update had already finished return immediately: keep them apart */
         const bool idle = e.upd >= 0 && e.slot >= h->h_nevals[e.upd % kNevalsRing];
         if (idle) { h->prof.idle_ms += ms; h->prof.idle_launches++; }
-        else if (e.kind == 0) { h->prof.measure_ms += ms; h->prof.measure_launches++; }
-        else if (e.kind == 3) {
+        else if (e.kind == kProfSearch) {
             h->prof.search_ms += ms; h->prof.measure_ms += ms; h->prof.measure_launches++;
             if (e.slot <= 0) { h->prof.search_first_ms += ms; h->prof.search_first_launches++; }
         }
-        else if (e.kind == 4) { h->prof.search_upper_ms += ms; h->prof.measure_ms += ms; }
-        else if (e.kind == 5) { h->prof.fit_ms += ms; h->prof.measure_ms += ms; }
-        else if (e.kind == 6) { h->prof.reuse_ms += ms; h->prof.measure_ms += ms; }
-        else if (e.kind == 1) { h->prof.solve_ms += ms; h->prof.solve_launches++; }
+        else if (e.kind == kProfSearchUpper) { h->prof.search_upper_ms += ms; h->prof.measure_ms += ms; }
+        else if (e.kind == kProfFit) { h->prof.fit_ms += ms; h->prof.measure_ms += ms; }
+        else if (e.kind == kProfReuse) { h->prof.reuse_ms += ms; h->prof.measure_ms += ms; }
+        else if (e.kind == kProfSolve) { h->prof.solve_ms += ms; h->prof.solve_launches++; }
         else { h->prof.build_ms += ms; h->prof.build_launches++; }
         h->pool.push_back(e);
     }
     h->pending.clear();
     return LV_OK;
 }
-static bool prof_begin(lv_context* h, int kind, EventPair* ep) {
+static bool prof_begin(lv_context* h, ProfKind kind, EventPair* ep) {
     if (!h->profile) return false;
     if (h->pending.size() > 2048) drain_events(h);
     if (h->pool.empty()) {
@@ -228,25 +232,73 @@ static cudaError_t ensure(T** p, size_t count) {
     return cudaMalloc(p, sizeof(T) * count);
 }
 
+/* argument checks of the _async forms; `what` names the call in the message */
+static bool n_max_ok(const char* what, int64_t n_max) {
+    if (n_max >= 1 && n_max <= 0x7fffffff) return true;
+    set_error(std::string(what) + ": n_max outside [1, 2^31 - 1]");
+    return false;
+}
+static bool handle_ok(const char* what, const lv_context* h, int64_t n_max) {
+    if (!h) { set_error(std::string(what) + ": null handle"); return false; }
+    if (n_max > h->prm.max_points) { set_error(std::string(what) + ": n_max above max_points"); return false; }
+    return true;
+}
+/* the byte ranges share a byte (ranges that only touch do not) */
+static bool ranges_overlap(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes) {
+    return (uintptr_t)a < (uintptr_t)b + (uintptr_t)b_bytes && (uintptr_t)b < (uintptr_t)a + (uintptr_t)a_bytes;
+}
+
 extern "C" {
 
 const char* lv_last_error(void) { return g_last_error.c_str(); }
 const char* lv_version(void) { return "limovelo_b200 0.1 (sm_90a)"; }
 int64_t lv_result_bytes(void) { return (int64_t)sizeof(UpdateCtrl); }
 
-/* every failure after `new lv_context` goes through here: nothing of a half-built context survives */
-#define LV_CREATE_CUDA(call)                                                                     \
-    do {                                                                                         \
-        cudaError_t e__ = (call);                                                                \
-        if (e__ != cudaSuccess) {                                                                \
-            char buf__[512];                                                                     \
-            snprintf(buf__, sizeof(buf__), "%s:%d: %s -> %s", __FILE__, __LINE__, #call,         \
-                     cudaGetErrorString(e__));                                                   \
-            lv_destroy(h);                                                                       \
-            set_error(buf__);                                                                    \
-            return LV_ERR_CUDA;                                                                  \
-        }                                                                                        \
-    } while (0)
+/* the stream and the buffers of a new context; lv_create destroys the context when this fails */
+static lv_status create_buffers(lv_context* h) {
+    const lv_params* p = &h->prm;
+    if (p->stream) { h->stream = (cudaStream_t)p->stream; h->own_stream = false; }
+    else { LV_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
+    LV_CUDA(map_alloc(h->map, p->max_map_points, p->max_points, p->voxel_size, p->map_downsample_size, h->stream));
+    { int l = 0; LV_CUDA(map_clear(h->map, h->stream, &l)); }
+    LV_CUDA(cudaMalloc(&h->d_sweep, sizeof(float) * 3 * p->max_points));
+    LV_CUDA(cudaMalloc(&h->d_nn_a, sizeof(int4) * p->max_points));
+    LV_CUDA(cudaMalloc(&h->d_nn_b, sizeof(int2) * p->max_points));
+    LV_CUDA(cudaMalloc(&h->d_hard_list, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
+    LV_CUDA(cudaMalloc(&h->d_ref, sizeof(float4) * p->max_points));
+    LV_CUDA(cudaMalloc(&h->d_redo, sizeof(uint32_t) * (p->max_points + 64)));   /* + one block of slack: read speculatively */
+    /* hand-over buffers start defined: lv_search_kernel<.., LIST> reads redo_list[] before it knows the list's length, and a
+     * first update's reuse kernel must not see stale neighbours (also keeps compute-sanitizer initcheck quiet) */
+    LV_CUDA(cudaMemset(h->d_redo, 0, sizeof(uint32_t) * (p->max_points + 64)));
+    LV_CUDA(cudaMemset(h->d_nn_a, 0xFF, sizeof(int4) * p->max_points));
+    LV_CUDA(cudaMemset(h->d_nn_b, 0xFF, sizeof(int2) * p->max_points));
+    LV_CUDA(cudaMemset(h->d_ref, 0, sizeof(float4) * p->max_points));
+    LV_CUDA(cudaMemset(h->d_hard_list, 0, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
+    h->use_reuse = getenv("LV_NO_REUSE") == nullptr;
+    h->use_pdl = getenv("LV_NO_PDL") == nullptr;
+    LV_CUDA(cudaMalloc(&h->d_job, sizeof(MeasureJob)));
+    measure_init();
+    h->use_graph = getenv("LV_NO_GRAPH") == nullptr;
+    LV_CUDA(cudaMalloc(&h->d_ctrl, sizeof(UpdateCtrl)));
+    LV_CUDA(cudaMemset(h->d_ctrl, 0, sizeof(UpdateCtrl)));
+    LV_CUDA(cudaMallocHost(&h->h_ctrl, sizeof(UpdateCtrl)));
+    LV_CUDA(cudaEventCreateWithFlags(&h->imu_copied, cudaEventDisableTiming));
+    LV_CUDA(cudaEventCreateWithFlags(&h->ctrl_copied, cudaEventDisableTiming));
+    LV_CUDA(cudaEventCreateWithFlags(&h->path_copied, cudaEventDisableTiming));
+    LV_CUDA(cudaMalloc(&h->d_async, sizeof(AsyncWords)));
+    LV_CUDA(cudaMemset(h->d_async, 0, sizeof(AsyncWords)));
+    LV_CUDA(cudaMallocHost(&h->h_async, sizeof(AsyncWords)));
+    LV_CUDA(cudaMalloc(&h->d_partials, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
+    LV_CUDA(cudaMemset(h->d_partials, 0, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
+    LV_CUDA(cudaMalloc(&h->d_group_rows, sizeof(double) * kPartialStride * 32));
+    LV_CUDA(cudaMemset(h->d_group_rows, 0, sizeof(double) * kPartialStride * 32));
+    LV_CUDA(cudaMalloc(&h->d_group_tickets, sizeof(uint32_t) * 32));
+    LV_CUDA(cudaMemset(h->d_group_tickets, 0, sizeof(uint32_t) * 32));
+    LV_CUDA(cudaMalloc(&h->d_reduced, sizeof(double) * 160));
+    LV_CUDA(cudaMallocHost(&h->h_reduced, sizeof(double) * 160));
+    LV_CUDA(cudaMallocHost(&h->h_nevals, sizeof(int32_t) * kNevalsRing));
+    return LV_OK;
+}
 
 lv_status lv_create(const lv_params* p, lv_handle* out) {
     if (!p || !out) return LV_ERR_ARG;
@@ -278,46 +330,8 @@ lv_status lv_create(const lv_params* p, lv_handle* out) {
     memset(h->logs, 0, sizeof(h->logs));
     memset(&h->map, 0, sizeof(h->map));
     fill_iprm(h);
-    if (p->stream) { h->stream = (cudaStream_t)p->stream; h->own_stream = false; }
-    else { LV_CREATE_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
-    LV_CREATE_CUDA(map_alloc(h->map, p->max_map_points, p->max_points, p->voxel_size, p->map_downsample_size, h->stream));
-    { int l = 0; LV_CREATE_CUDA(map_clear(h->map, h->stream, &l)); }
-    LV_CREATE_CUDA(cudaMalloc(&h->d_sweep, sizeof(float) * 3 * p->max_points));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_nn_a, sizeof(int4) * p->max_points));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_nn_b, sizeof(int2) * p->max_points));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_hard_list, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_ref, sizeof(float4) * p->max_points));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_redo, sizeof(uint32_t) * (p->max_points + 64)));   /* + one block of slack: read speculatively */
-    /* hand-over buffers start defined: lv_search_kernel<.., LIST> reads redo_list[] before it knows the list's length, and a
-     * first update's reuse kernel must not see stale neighbours (also keeps compute-sanitizer initcheck quiet) */
-    LV_CREATE_CUDA(cudaMemset(h->d_redo, 0, sizeof(uint32_t) * (p->max_points + 64)));
-    LV_CREATE_CUDA(cudaMemset(h->d_nn_a, 0xFF, sizeof(int4) * p->max_points));
-    LV_CREATE_CUDA(cudaMemset(h->d_nn_b, 0xFF, sizeof(int2) * p->max_points));
-    LV_CREATE_CUDA(cudaMemset(h->d_ref, 0, sizeof(float4) * p->max_points));
-    LV_CREATE_CUDA(cudaMemset(h->d_hard_list, 0, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
-    h->use_reuse = getenv("LV_NO_REUSE") == nullptr;
-    h->use_pdl = getenv("LV_NO_PDL") == nullptr;
-    LV_CREATE_CUDA(cudaMalloc(&h->d_job, sizeof(MeasureJob)));
-    measure_init();
-    h->use_graph = getenv("LV_NO_GRAPH") == nullptr;
-    LV_CREATE_CUDA(cudaMalloc(&h->d_ctrl, sizeof(UpdateCtrl)));
-    LV_CREATE_CUDA(cudaMemset(h->d_ctrl, 0, sizeof(UpdateCtrl)));
-    LV_CREATE_CUDA(cudaMallocHost(&h->h_ctrl, sizeof(UpdateCtrl)));
-    LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->imu_copied, cudaEventDisableTiming));
-    LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->ctrl_copied, cudaEventDisableTiming));
-    LV_CREATE_CUDA(cudaEventCreateWithFlags(&h->path_copied, cudaEventDisableTiming));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_async, sizeof(AsyncWords)));
-    LV_CREATE_CUDA(cudaMemset(h->d_async, 0, sizeof(AsyncWords)));
-    LV_CREATE_CUDA(cudaMallocHost(&h->h_async, sizeof(AsyncWords)));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_partials, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
-    LV_CREATE_CUDA(cudaMemset(h->d_partials, 0, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_group_rows, sizeof(double) * kPartialStride * 32));
-    LV_CREATE_CUDA(cudaMemset(h->d_group_rows, 0, sizeof(double) * kPartialStride * 32));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_group_tickets, sizeof(uint32_t) * 32));
-    LV_CREATE_CUDA(cudaMemset(h->d_group_tickets, 0, sizeof(uint32_t) * 32));
-    LV_CREATE_CUDA(cudaMalloc(&h->d_reduced, sizeof(double) * 160));
-    LV_CREATE_CUDA(cudaMallocHost(&h->h_reduced, sizeof(double) * 160));
-    LV_CREATE_CUDA(cudaMallocHost(&h->h_nevals, sizeof(int32_t) * kNevalsRing));
+    const lv_status s = create_buffers(h);
+    if (s != LV_OK) { lv_destroy(h); return s; }                 /* nothing of a half-built context survives */
     /* default filter state: identity pose, P = I (esekf constructor); callers normally follow
      * with lv_init_state or lv_set_state */
     for (int i = 0; i < LV_STATE_LEN; ++i) h->x[i] = 0;
@@ -385,7 +399,7 @@ static lv_status map_grow_to(lv_context* h, int64_t cap) {
         return LV_ERR_CAPACITY;
     }
     EventPair ep;
-    const bool pr = prof_begin(h, 2, &ep);
+    const bool pr = prof_begin(h, kProfMap, &ep);
     const int64_t old_cap = h->map.cap;
     int launches = 0;
     const cudaError_t e = map_grow(h->map, cap, h->stream, &launches);
@@ -535,47 +549,52 @@ lv_status lv_map_info(lv_handle h, struct lv_map_info* out) {
     return LV_OK;
 }
 
-/* m, n: the points, or with cnt.n the host bound of their device count */
-static lv_status map_build_device_impl(lv_context* h, const float* d_xyz, int64_t m, const MapAddCount& cnt = MapAddCount()) {
-    EventPair ep;
-    const bool pr = prof_begin(h, 2, &ep);
-    int launches = 0;
-    LV_CUDA(map_clear(h->map, h->stream, &launches));
-    LV_CUDA(map_add(h->map, d_xyz, m, 0, h->stream, &launches, cnt));         /* Build: no downsampling (Mapper.cpp:68-71) */
-    if (pr) prof_end(h, &ep);
-    count_map_launches(h, launches);
-    snap_reset_cleared(h);
-    return snap_after_add(h, m);
+static lv_status upload_state(lv_context* h, const double* x, const double* P);
+/* the host mirror into d_ctrl when it is the newer copy (lv_set_state, lv_init_state, lv_predict) */
+static lv_status sync_device_state(lv_context* h) {
+    if (!h->state_dirty) return LV_OK;
+    const lv_status s = upload_state(h, h->x, h->P);
+    if (s == LV_OK) h->state_dirty = false;
+    return s;
 }
-static lv_status map_add_device_impl(lv_context* h, const float* d_xyz, int64_t n, int downsample, const MapAddCount& cnt = MapAddCount()) {
+
+/* Mapper::add on the device, every form, from its argument checks on: n points of xyz, or with cnt.n the host bound of their
+ * device count.  Points on the host (on_host) are staged once the add is known to fit.  `build` empties the map first and
+ * adds without downsampling (KD_TREE::Build, Mapper.cpp:68-71), and its points must fit the map's capacity; any other add
+ * must fit one add's scratch.  An add that finds the map without points builds it (Mapper.cpp:26): emptied first too, except
+ * a sweep (to_world: its points transformed by the state on the device), which adds without downsampling to the map as it
+ * stands. */
+static lv_status map_enqueue(lv_context* h, const float* xyz, bool on_host, int64_t n, bool build, int downsample,
+                             const MapAddCount& cnt = MapAddCount(), bool to_world = false) {
+    if (!h || (!xyz && n > 0)) return LV_ERR_ARG;
+    if (n <= 0) return LV_OK;                                    /* Mapper.cpp:23 */
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    const bool empty = h->map.empty;
+    const bool clears = build || (empty && !to_world);
+    lv_status s = to_world ? sync_device_state(h) : LV_OK;
+    if (s != LV_OK) return s;
+    s = grow_before_add(h, n, clears);
+    if (s != LV_OK) return s;
+    if (build ? n > h->map.cap : n > h->map.add_cap)
+        return capacity_error(h, build ? "map capacity exceeded" : "more points than one lv_map_add can take (max_map_points)");
+    if (on_host) {
+        LV_CUDA(cudaMemcpyAsync(h->map.stage_xyz, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
+        xyz = h->map.stage_xyz;
+    }
+    if (cnt.n && empty) h->map_unknown = true;                   /* a device count of 0 leaves the map without a point */
     EventPair ep;
-    const bool pr = prof_begin(h, 2, &ep);
+    const bool pr = prof_begin(h, kProfMap, &ep);
     int launches = 0;
-    LV_CUDA(map_add(h->map, d_xyz, n, downsample ? 1 : 0, h->stream, &launches, cnt));
+    if (clears) LV_CUDA(map_clear(h->map, h->stream, &launches));
+    LV_CUDA(map_add(h->map, xyz, n, (!build && !empty && downsample) ? 1 : 0, h->stream, &launches, cnt, to_world ? h->d_ctrl : nullptr));
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
+    if (clears) snap_reset_cleared(h);
     return snap_after_add(h, n);
 }
 
-lv_status lv_map_build(lv_handle h, const float* xyz, int64_t m) {
-    if (!h || (!xyz && m > 0)) return LV_ERR_ARG;
-    if (m <= 0) return LV_OK;                                    /* Mapper.cpp:23 */
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    lv_status s = grow_before_add(h, m, true);
-    if (s != LV_OK) return s;
-    if (m > h->map.cap) return capacity_error(h, "map capacity exceeded");
-    LV_CUDA(cudaMemcpyAsync(h->map.stage_xyz, xyz, sizeof(float) * 3 * m, cudaMemcpyHostToDevice, h->stream));
-    return map_build_device_impl(h, h->map.stage_xyz, m);
-}
-lv_status lv_map_build_device(lv_handle h, const float* d_xyz, int64_t m) {
-    if (!h || (!d_xyz && m > 0)) return LV_ERR_ARG;
-    if (m <= 0) return LV_OK;
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    lv_status s = grow_before_add(h, m, true);
-    if (s != LV_OK) return s;
-    if (m > h->map.cap) return capacity_error(h, "map capacity exceeded");
-    return map_build_device_impl(h, d_xyz, m);
-}
+lv_status lv_map_build(lv_handle h, const float* xyz, int64_t m) { return map_enqueue(h, xyz, true, m, true, 0); }
+lv_status lv_map_build_device(lv_handle h, const float* d_xyz, int64_t m) { return map_enqueue(h, d_xyz, false, m, true, 0); }
 int64_t lv_map_size(lv_handle h) {
     if (!h || h->map.empty) return 0;
     if (cudaSetDevice(h->prm.device) != cudaSuccess) return -1;
@@ -600,95 +619,48 @@ int64_t lv_map_points(lv_handle h, float* out, int64_t cap) {
 }
 
 lv_status lv_map_add(lv_handle h, const float* xyz, int64_t n, int downsample) {
-    if (!h || (!xyz && n > 0)) return LV_ERR_ARG;
-    if (n <= 0) return LV_OK;                                    /* Mapper.cpp:23 */
-    if (h->map.empty) return lv_map_build(h, xyz, n);            /* Mapper.cpp:26 */
-    if (!h->grow_limit && n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    lv_status s = grow_before_add(h, n, false);
-    if (s != LV_OK) return s;
-    if (n > h->map.add_cap) return capacity_error(h, "more points than one lv_map_add can take (max_map_points)");
-    LV_CUDA(cudaMemcpyAsync(h->map.stage_xyz, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
-    return map_add_device_impl(h, h->map.stage_xyz, n, downsample);
+    return map_enqueue(h, xyz, true, n, h && h->map.empty, downsample);   /* Mapper.cpp:26: lv_map_build on a map without points */
 }
 lv_status lv_map_add_device(lv_handle h, const float* d_xyz, int64_t n, int downsample) {
-    if (!h || (!d_xyz && n > 0)) return LV_ERR_ARG;
-    if (n <= 0) return LV_OK;
-    if (!h->grow_limit && n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    lv_status s = grow_before_add(h, n, h->map.empty);
-    if (s != LV_OK) return s;
-    if (n > h->map.add_cap) return capacity_error(h, "more points than one lv_map_add can take (max_map_points)");
-    if (h->map.empty) return map_build_device_impl(h, d_xyz, n);
-    return map_add_device_impl(h, d_xyz, n, downsample);
+    return map_enqueue(h, d_xyz, false, n, false, downsample);
 }
 lv_status lv_map_add_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int downsample) {
     if (!d_xyz || !d_n) { set_error("map add async: null points or count"); return LV_ERR_ARG; }
-    if (n_max < 1 || n_max > 0x7fffffff) { set_error("map add async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
-    if (!h) { set_error("map add async: null handle"); return LV_ERR_ARG; }
-    if (n_max > h->prm.max_points) { set_error("map add async: n_max above max_points"); return LV_ERR_ARG; }
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    const bool build = h->map.empty;
-    lv_status s = grow_before_add(h, n_max, build);
-    if (s != LV_OK) return s;
+    if (!n_max_ok("map add async", n_max) || !handle_ok("map add async", h, n_max)) return LV_ERR_ARG;
     /* Mapper.cpp:22-30: *d_n points, none when it is 0; a map without points (also one an earlier device count left empty) is
      * built without downsampling.  The add capacity is at least max_points, so n_max always fits. */
     MapAddCount cnt;
     cnt.n = d_n;
     cnt.build_if_empty = 1;
     cnt.err = &h->d_async->err;
-    if (!build) return map_add_device_impl(h, d_xyz, n_max, downsample, cnt);
-    h->map_unknown = true;                                        /* a count of 0 leaves the build without a point */
-    return map_build_device_impl(h, d_xyz, n_max, cnt);
+    return map_enqueue(h, d_xyz, false, n_max, false, downsample, cnt);
 }
 
 /* ---- the tick on the device: main.cpp:99-105 ------------------------------------------------- */
-static lv_status upload_state(lv_context* h, const double* x, const double* P);
-static bool ranges_overlap(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes);
-/* n: the sweep's points, or with cnt.n the host bound of its device count */
-static lv_status add_sweep_impl(lv_context* h, const float* d_xyz_lidar, int64_t n, int downsample, const MapAddCount& cnt = MapAddCount()) {
-    if (h->state_dirty) {                                         /* the transform uses the device copy of the state */
-        lv_status s = upload_state(h, h->x, h->P);
-        if (s != LV_OK) return s;
-        h->state_dirty = false;
-    }
-    lv_status s = grow_before_add(h, n, false);
-    if (s != LV_OK) return s;
-    if (n > h->map.add_cap) return capacity_error(h, "more points than one lv_map_add can take (max_map_points)");
-    EventPair ep;
-    const bool pr = prof_begin(h, 2, &ep);
-    int launches = 0;
-    if (cnt.n && h->map.empty) h->map_unknown = true;             /* the gate may leave the build without a point */
-    LV_CUDA(map_add_sweep(h->map, h->d_ctrl, d_xyz_lidar, n, downsample ? 1 : 0, h->stream, &launches, cnt));
-    if (pr) prof_end(h, &ep);
-    count_map_launches(h, launches);
-    return snap_after_add(h, n);
+/* how the tick's map add and world cloud count the sweep of the last update: after lv_correct_device_async its gate decides for
+ * the whole tick (*d_n points, none when it stopped the tick; a map that an earlier gated build left without points is built,
+ * Mapper.cpp:26); after the synchronous forms the host knows the count */
+static MapAddCount tick_count(const lv_context* h) {
+    MapAddCount c;
+    if (!h->tick.d_n) return c;
+    c.n = h->tick.d_n;
+    c.min_points = h->tick.min_points;
+    c.build_if_empty = 1;
+    c.err = &h->d_async->err;
+    return c;
 }
 lv_status lv_map_add_sweep_device(lv_handle h, const float* d_xyz_lidar, int64_t n, int downsample) {
-    if (!h || (!d_xyz_lidar && n > 0)) return LV_ERR_ARG;
-    if (n <= 0) return LV_OK;
-    if (!h->grow_limit && n > h->map.add_cap) { set_error("more points than one lv_map_add can take (max_map_points)"); return LV_ERR_CAPACITY; }
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    return add_sweep_impl(h, d_xyz_lidar, n, downsample);
+    return map_enqueue(h, d_xyz_lidar, false, n, false, downsample, MapAddCount(), true);
 }
 lv_status lv_map_add_last_sweep(lv_handle h, int downsample) {
     if (!h) return LV_ERR_ARG;
-    if (!h->last_sweep || h->last_sweep_n <= 0) { set_error("no sweep has been corrected yet"); return LV_ERR_ARG; }
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    if (!h->last_sweep_dn) return add_sweep_impl(h, h->last_sweep, h->last_sweep_n, downsample);
-    /* after lv_correct_device_async: *d_n points, none when its gate stopped the tick; a map that an earlier gated build left
-     * without points is built (the reference's map does not exist yet, Mapper.cpp:26) */
-    MapAddCount cnt;
-    cnt.n = h->last_sweep_dn;
-    cnt.min_points = h->last_sweep_min;
-    cnt.build_if_empty = 1;
-    cnt.err = &h->d_async->err;
-    return add_sweep_impl(h, h->last_sweep, h->last_sweep_n, downsample, cnt);
+    if (!h->tick.xyz || h->tick.n <= 0) { set_error("no sweep has been corrected yet"); return LV_ERR_ARG; }
+    return map_enqueue(h, h->tick.xyz, false, h->tick.n, false, downsample, tick_count(h), true);
 }
 lv_status lv_sweep_to_world_device_async(lv_handle h, const float* d_xyz_lidar, const int64_t* d_n, int64_t n_max, float* d_xyz_world,
                                          int64_t* d_n_out) {
     if (!d_xyz_lidar || !d_n || !d_xyz_world || !d_n_out) { set_error("sweep to world: null input, count, output or output count"); return LV_ERR_ARG; }
-    if (n_max < 1 || n_max > 0x7fffffff) { set_error("sweep to world: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!n_max_ok("sweep to world", n_max)) return LV_ERR_ARG;
     /* one thread reads a point and then writes the same point: in place is fine, a shifted overlap is not.  The counts are read
      * and written by one thread before any point: the output count may equal the input count, but not lie among the points. */
     const int64_t b = 12 * n_max;
@@ -698,17 +670,13 @@ lv_status lv_sweep_to_world_device_async(lv_handle h, const float* d_xyz_lidar, 
         set_error("sweep to world: an output range overlaps another range");
         return LV_ERR_ARG;
     }
-    if (!h) { set_error("sweep to world: null handle"); return LV_ERR_ARG; }
-    if (n_max > h->prm.max_points) { set_error("sweep to world: n_max above max_points"); return LV_ERR_ARG; }
+    if (!handle_ok("sweep to world", h, n_max)) return LV_ERR_ARG;
     LV_CUDA(cudaSetDevice(h->prm.device));
-    if (h->state_dirty) {                                         /* the transform uses the device copy of the state */
-        lv_status s = upload_state(h, h->x, h->P);
-        if (s != LV_OK) return s;
-        h->state_dirty = false;
-    }
-    /* after lv_correct_device_async its gate decides for the whole tick, as for lv_map_add_last_sweep */
+    const lv_status s = sync_device_state(h);                     /* the transform uses the device copy of the state */
+    if (s != LV_OK) return s;
+    const MapAddCount gate = tick_count(h);
     int launches = 0;
-    LV_CUDA(launch_sweep_to_world(h->d_ctrl, d_xyz_lidar, d_n, n_max, h->last_sweep_dn, h->last_sweep_n, h->last_sweep_min, d_xyz_world, d_n_out,
+    LV_CUDA(launch_sweep_to_world(h->d_ctrl, d_xyz_lidar, d_n, n_max, gate.n, h->tick.n, gate.min_points, d_xyz_world, d_n_out,
                                   &h->d_async->world_n, &h->d_async->err, h->stream, &launches));
     h->prof.total_launches += launches;
     return LV_OK;
@@ -761,11 +729,8 @@ lv_status lv_propagate_device(lv_handle h, const double* acc, const double* gyro
         LV_CUDA(cudaMalloc(&h->d_imu, sizeof(double) * 7 * kImuBatch));
         LV_CUDA(cudaMallocHost(&h->h_imu, sizeof(double) * 7 * kImuBatch));
     }
-    if (h->state_dirty) {                                         /* the host mirror is newer (lv_set_state / lv_predict): bring it over */
-        lv_status s = upload_state(h, h->x, h->P);
-        if (s != LV_OK) return s;
-        h->state_dirty = false;
-    }
+    const lv_status s = sync_device_state(h);                     /* the host mirror may be newer (lv_set_state / lv_predict) */
+    if (s != LV_OK) return s;
     const PredictNoise noise = {h->prm.covariance_gyroscope, h->prm.covariance_acceleration, h->prm.covariance_bias_gyroscope,
                                 h->prm.covariance_bias_acceleration};
     for (int32_t s0 = 0; s0 < k; s0 += kImuBatch) {
@@ -817,7 +782,7 @@ static cudaError_t launch_measure_timed(lv_context* h, const MeasureArgs& a, int
         if (c->on) prof_end(c->h, &c->ep);
         c->on = false;
         if (stage != 3) {         /* 4: reuse kernel follows, 0: search, 1: search-upper, 2: fit, 3: end */
-            c->on = prof_begin(c->h, stage == 4 ? 6 : 3 + stage, &c->ep);
+            c->on = prof_begin(c->h, stage == 4 ? kProfReuse : (ProfKind)(kProfSearch + stage), &c->ep);
             c->ep.upd = c->upd; c->ep.slot = c->slot;
         }
     };
@@ -870,13 +835,9 @@ static lv_status build_update_graph(lv_context* h, int64_t cap, lv_context::Upda
 }
 
 /* n: the sweep's points, or with gate.n the host bound of its device count (the graph bucket is chosen by it) */
-static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n, UpdateGate gate = UpdateGate()) {
-    if (h->state_dirty) {
-        lv_status s = upload_state(h, h->x, h->P);
-        if (s != LV_OK) return s;
-        h->state_dirty = false;
-    }
-    if (h->map_unknown) gate.map_counters = h->map.counters;     /* an async build may have added nothing */
+static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n, UpdateGate gate) {
+    const lv_status s = sync_device_state(h);
+    if (s != LV_OK) return s;
     if (h->profile || !h->use_graph) return enqueue_update_kernels(h, d_xyz, n, gate.n != nullptr, false, gate);
     int64_t cap = 4096;
     while (cap < n) cap <<= 1;
@@ -917,7 +878,7 @@ static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64
         EventPair ep;
         bool pr;
         LV_CUDA(launch_measure_timed(h, a, grid, capture ? 0 : 1, e /* evaluation index: > 0 = reuse + work list */, (int)(h->update_seq % kNevalsRing), e, pdl));
-        pr = prof_begin(h, 1, &ep);
+        pr = prof_begin(h, kProfSolve, &ep);
         ep.upd = (int)(h->update_seq % kNevalsRing); ep.slot = e;
         LV_CUDA(launch_ieskf_step(h->d_ctrl, h->iprm, h->d_group_rows, partial_groups(grid), h->stream, pdl));
         if (pr) prof_end(h, &ep);
@@ -961,17 +922,43 @@ static lv_status fetch_results(lv_context* h) {
     return (lv_status)c->status;
 }
 
+/* Localizator::correct (Localizator.cpp:22-27) enqueued, every form: the sweep's n points, or with d_n its device count (n is
+ * then the bound) and the MAX_POINTS2MATCH gate min_points (main.cpp:81).  The sweep is recorded even on an empty map: the
+ * first tick's lv_map_add_last_sweep builds the map from it.  Who decides last_time_updated: with `fetched` (lv_correct, which
+ * fetches the results at once) the caller, from the status; otherwise the host now, unless only the device knows whether the
+ * update runs (a device count, or a map an async build may have left without points): then the device, read at the next fetch. */
+static lv_status correct_enqueue(lv_context* h, const float* d_xyz, int64_t n, const int64_t* d_n, int64_t min_points, double time,
+                                 bool fetched) {
+    h->tick = {d_xyz, n, d_n, min_points};
+    if (h->map.empty) return LV_EMPTY_MAP;                        /* Localizator.cpp:24: the state is left as it is */
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    UpdateGate gate;
+    gate.n = d_n;
+    gate.min_points = min_points;
+    if (h->map_unknown) gate.map_counters = h->map.counters;      /* an async build may have added nothing */
+    const bool device_time = d_n || (h->map_unknown && !fetched);
+    if (device_time) {
+        gate.words = h->d_async;
+        gate.time = time;
+    } else if (!fetched && h->time_pending) {                     /* this time supersedes what an earlier async update recorded */
+        LV_CUDA(cudaMemsetAsync(&h->d_async->time_set, 0, sizeof(int32_t), h->stream));
+    }
+    const lv_status s = enqueue_update(h, d_xyz, n, gate);
+    if (fetched) return s;
+    h->time_pending = device_time;
+    if (!device_time) h->last_time_updated = time;
+    h->pending_fetch = true;
+    return s;
+}
+
 lv_status lv_correct(lv_handle h, const float* xyz, int64_t n, double time, lv_iter_log* logs, int32_t* n_evals,
                      double* x_out, double* P_out) {
     if (!h || !xyz || n <= 0) return LV_ERR_ARG;
     if (n_evals) *n_evals = 0;
     if (n > h->prm.max_points) { set_error("sweep capacity exceeded"); return LV_ERR_CAPACITY; }
     LV_CUDA(cudaSetDevice(h->prm.device));
-    /* the sweep is uploaded and recorded even on an empty map: the first tick's lv_map_add_last_sweep builds the map from it */
     LV_CUDA(cudaMemcpyAsync(h->d_sweep, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
-    h->last_sweep = h->d_sweep; h->last_sweep_n = n; h->last_sweep_dn = nullptr;
-    if (h->map.empty) return LV_EMPTY_MAP;                       /* Localizator.cpp:24: the state is left as it is */
-    lv_status s = enqueue_update(h, h->d_sweep, n);
+    lv_status s = correct_enqueue(h, h->d_sweep, n, nullptr, 0, time, true);
     if (s != LV_OK) return s;
     s = fetch_results(h);
     if (s != LV_EMPTY_MAP) h->last_time_updated = time;          /* Localizator.cpp:26 (LV_EMPTY_MAP: an async build added nothing) */
@@ -984,42 +971,15 @@ lv_status lv_correct(lv_handle h, const float* xyz, int64_t n, double time, lv_i
 
 lv_status lv_correct_device(lv_handle h, const float* d_xyz, int64_t n, double time) {
     if (!h || !d_xyz || n <= 0) return LV_ERR_ARG;
-    h->last_sweep = d_xyz; h->last_sweep_n = n; h->last_sweep_dn = nullptr;   /* recorded on an empty map too (see lv_correct) */
-    if (h->map.empty) return LV_EMPTY_MAP;
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    UpdateGate gate;
-    if (h->map_unknown) {                                         /* whether the update runs is the device's decision */
-        gate.words = h->d_async;
-        gate.time = time;
-    } else if (h->time_pending) {                                 /* this time supersedes what an earlier async update recorded */
-        LV_CUDA(cudaMemsetAsync(&h->d_async->time_set, 0, sizeof(int32_t), h->stream));
-    }
-    lv_status s = enqueue_update(h, d_xyz, n, gate);
-    h->time_pending = h->map_unknown;
-    if (!h->map_unknown) h->last_time_updated = time;
-    h->pending_fetch = true;
-    return s;
+    return correct_enqueue(h, d_xyz, n, nullptr, 0, time, false);
 }
 
 lv_status lv_correct_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int64_t min_points, double time) {
     if (!d_xyz || !d_n) { set_error("correct async: null sweep or count"); return LV_ERR_ARG; }
-    if (n_max < 1 || n_max > 0x7fffffff) { set_error("correct async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!n_max_ok("correct async", n_max)) return LV_ERR_ARG;
     if (min_points < 0) { set_error("correct async: negative min_points"); return LV_ERR_ARG; }
-    if (!h) { set_error("correct async: null handle"); return LV_ERR_ARG; }
-    if (n_max > h->prm.max_points) { set_error("correct async: n_max above max_points"); return LV_ERR_ARG; }
-    /* recorded on an empty map too: lv_map_add_last_sweep builds the map from *d_n points unless the gate stops the tick */
-    h->last_sweep = d_xyz; h->last_sweep_n = n_max; h->last_sweep_dn = d_n; h->last_sweep_min = min_points;
-    if (h->map.empty) return LV_EMPTY_MAP;                        /* Localizator.cpp:24 */
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    UpdateGate gate;
-    gate.n = d_n;
-    gate.min_points = min_points;
-    gate.words = h->d_async;
-    gate.time = time;
-    lv_status s = enqueue_update(h, d_xyz, n_max, gate);
-    h->time_pending = true;
-    h->pending_fetch = true;
-    return s;
+    if (!handle_ok("correct async", h, n_max)) return LV_ERR_ARG;
+    return correct_enqueue(h, d_xyz, n_max, d_n, min_points, time, false);
 }
 
 lv_status lv_last_logs(lv_handle h, lv_iter_log* logs, int32_t* n_evals) {
@@ -1189,14 +1149,18 @@ static lv_status deskew_common(lv_context* h, const lv_state32* path, int32_t ns
     h->prof.total_launches += 2;
     return LV_OK;
 }
-static lv_status deskew_args_ok(lv_context* h, const lv_state32* path, int32_t ns, const lv_state32* Xt2, const void* a,
-                                const void* b, int64_t n, const void* c) {
-    if (!h || !path || !Xt2 || !a || !b || !c || n <= 0 || ns < 2) return LV_ERR_ARG;
+/* the path's checks, with the sweep's capacity between them (the async form has checked n against max_points already) */
+static lv_status deskew_path_ok(const lv_context* h, const lv_state32* path, int32_t ns, int64_t n) {
     if (ns > deskew_max_states()) { set_error("deskew path too long"); return LV_ERR_CAPACITY; }
     if (n > h->prm.max_points) { set_error("sweep capacity exceeded"); return LV_ERR_CAPACITY; }
     for (int32_t s = 1; s < ns; ++s)
         if (!(path[s - 1].time <= path[s].time)) { set_error("deskew path not sorted by time"); return LV_ERR_ARG; }
     return LV_OK;
+}
+static lv_status deskew_args_ok(const lv_context* h, const lv_state32* path, int32_t ns, const lv_state32* Xt2, const void* a,
+                                const void* b, int64_t n, const void* c) {
+    if (!h || !path || !Xt2 || !a || !b || !c || n <= 0 || ns < 2) return LV_ERR_ARG;
+    return deskew_path_ok(h, path, ns, n);
 }
 lv_status lv_compensate_device(lv_handle h, const lv_state32* path, int32_t ns, const lv_state32* Xt2,
                                const float* d_xyz, const double* d_t, int64_t n, float* d_xyz_out) {
@@ -1209,22 +1173,18 @@ lv_status lv_compensate_device(lv_handle h, const lv_state32* path, int32_t ns, 
     if (*h->h_bad) { set_error("deskew: a timestamp lies outside the path or the points are not time-sorted"); return LV_ERR_ARG; }
     return LV_OK;
 }
-static bool ranges_overlap(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes) {
-    return (uintptr_t)a < (uintptr_t)b + (uintptr_t)b_bytes && (uintptr_t)b < (uintptr_t)a + (uintptr_t)a_bytes;
-}
 lv_status lv_compensate_device_async(lv_handle h, const lv_state32* path, int32_t ns, const lv_state32* Xt2, const float* d_xyz,
                                      const double* d_t, const int64_t* d_n, int64_t n_max, float* d_xyz_out) {
     if (!path || !Xt2 || !d_xyz || !d_t || !d_n || !d_xyz_out) { set_error("compensate async: null path, Xt2, xyz, t, count or output"); return LV_ERR_ARG; }
-    if (n_max < 1 || n_max > 0x7fffffff) { set_error("compensate async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!n_max_ok("compensate async", n_max)) return LV_ERR_ARG;
     if (ns < 2) { set_error("compensate async: a path needs two states"); return LV_ERR_ARG; }
     /* one thread reads a point and then writes the same point: in place is fine, a shifted overlap is not */
     if ((d_xyz_out != d_xyz && ranges_overlap(d_xyz_out, 12 * n_max, d_xyz, 12 * n_max)) || ranges_overlap(d_xyz_out, 12 * n_max, d_t, 8 * n_max)) {
         set_error("compensate async: the output range overlaps an input range");
         return LV_ERR_ARG;
     }
-    if (!h) { set_error("compensate async: null handle"); return LV_ERR_ARG; }
-    if (n_max > h->prm.max_points) { set_error("compensate async: n_max above max_points"); return LV_ERR_ARG; }
-    lv_status s = deskew_args_ok(h, path, ns, Xt2, d_xyz, d_t, n_max, d_xyz_out);
+    if (!handle_ok("compensate async", h, n_max)) return LV_ERR_ARG;
+    const lv_status s = deskew_path_ok(h, path, ns, n_max);
     if (s != LV_OK) return s;
     LV_CUDA(cudaSetDevice(h->prm.device));
     return deskew_common(h, path, ns, Xt2, d_xyz, d_t, d_n, n_max, d_xyz_out);
@@ -1263,8 +1223,7 @@ static lv_status ds_stage(lv_context* h, int64_t n) {
 lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_t n, float leaf, float* d_xyz_out, int64_t* n_out) {
     /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids: an output
      * range that overlaps the input would be read after it is overwritten */
-    if (d_xyz && d_xyz_out && n > 0 && n <= 0x7fffffff && (uintptr_t)d_xyz_out < (uintptr_t)(d_xyz + 3 * n) &&
-        (uintptr_t)d_xyz < (uintptr_t)(d_xyz_out + 3 * n)) {
+    if (d_xyz && d_xyz_out && n > 0 && n <= 0x7fffffff && ranges_overlap(d_xyz_out, 12 * n, d_xyz, 12 * n)) {
         set_error("voxel grid: the output range overlaps the input range");
         return LV_ERR_ARG;
     }
@@ -1286,12 +1245,11 @@ lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_
 lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf,
                                                float* d_xyz_out, int64_t* d_n_out) {
     if (!d_xyz || !d_n || !d_xyz_out || !d_n_out) { set_error("voxel grid async: null input, count, output or output count"); return LV_ERR_ARG; }
-    if (n_max < 1 || n_max > 0x7fffffff) { set_error("voxel grid async: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!n_max_ok("voxel grid async", n_max)) return LV_ERR_ARG;
     if (!(leaf > 0.f)) { set_error("voxel grid async: leaf size must be positive"); return LV_ERR_ARG; }
     /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids */
     if (ranges_overlap(d_xyz, 12 * n_max, d_xyz_out, 12 * n_max)) { set_error("voxel grid async: the output range overlaps the input range"); return LV_ERR_ARG; }
-    if (!h) { set_error("voxel grid async: null handle"); return LV_ERR_ARG; }
-    if (n_max > h->prm.max_points) { set_error("voxel grid async: n_max above max_points"); return LV_ERR_ARG; }
+    if (!handle_ok("voxel grid async", h, n_max)) return LV_ERR_ARG;
     LV_CUDA(cudaSetDevice(h->prm.device));
     LV_CUDA(ds_reserve(h->ds, n_max));
     int launches = 0;
@@ -1351,7 +1309,7 @@ static lv_status process_cloud_impl(lv_handle h, lv_lidar_type type, const lv_cl
     const struct { const void* p; int64_t bytes; } outs[5] = {{d_xyz, 12 * n}, {d_time, 8 * n}, {d_intensity, 4 * n}, {d_range, 4 * n},
                                                             {d_idx, 4 * n}};
     for (const auto& o : outs)
-        if (o.p && n > 0 && (uintptr_t)o.p < (uintptr_t)d_data + (uintptr_t)data_bytes && (uintptr_t)d_data < (uintptr_t)o.p + (uintptr_t)o.bytes) {
+        if (o.p && n > 0 && ranges_overlap(o.p, o.bytes, d_data, data_bytes)) {
             set_error("process cloud: an output range overlaps the message bytes");
             return LV_ERR_ARG;
         }
@@ -1469,7 +1427,7 @@ lv_status lv_lidar_reserve(lv_handle h, int64_t capacity) {
 }
 lv_status lv_lidar_push_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max) {
     if (!d_xyz || !d_time || !d_n) { set_error("lidar push: null xyz, time or count"); return LV_ERR_ARG; }
-    if (n_max < 1 || n_max > 0x7fffffff) { set_error("lidar push: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!n_max_ok("lidar push", n_max)) return LV_ERR_ARG;
     if (!h) { set_error("lidar push: null handle"); return LV_ERR_ARG; }
     if (!h->lidar.cap) { set_error("lidar push: the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
     /* the kernel reads the count and the points while it writes the buffer */
@@ -1487,7 +1445,7 @@ lv_status lv_lidar_push_device_async(lv_handle h, const float* d_xyz, const doub
 static lv_status lidar_get_impl(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, const void* count,
                                 int64_t* d_n_out) {
     if (!d_xyz || !d_time || !count) { set_error("lidar get points: null xyz, time or count"); return LV_ERR_ARG; }
-    if (n_max < 1 || n_max > 0x7fffffff) { set_error("lidar get points: n_max outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!n_max_ok("lidar get points", n_max)) return LV_ERR_ARG;
     if (isnan(t1) || isnan(t2)) { set_error("lidar get points: t1 or t2 is NaN"); return LV_ERR_ARG; }
     if (ranges_overlap(d_xyz, 12 * n_max, d_time, 8 * n_max) ||
         (d_n_out && (ranges_overlap(d_n_out, 8, d_xyz, 12 * n_max) || ranges_overlap(d_n_out, 8, d_time, 8 * n_max)))) {

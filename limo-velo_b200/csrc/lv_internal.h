@@ -151,12 +151,10 @@ struct MapAddCount {
     uint32_t* err = nullptr;
 };
 /* KD_TREE::Build (downsample = 0 on an empty map) / Add_Points: n points in DEVICE memory (or *cnt.n of them, n = the
- * host-known bound the sort runs over); asynchronous, no host round trip */
+ * host-known bound the sort runs over); asynchronous, no host round trip.  With to_world the points are a sweep (LiDAR frame)
+ * transformed by the state in to_world->x first: main.cpp:99-105 without leaving the GPU */
 cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample, cudaStream_t st, int* launches,
                     const MapAddCount& cnt = MapAddCount(), const UpdateCtrl* to_world = nullptr);
-/* the sweep (LiDAR frame, device) transformed by the state in d_ctrl->x, then map_add: main.cpp:99-105 without leaving the GPU */
-cudaError_t map_add_sweep(MapBuffers& b, const UpdateCtrl* d_ctrl, const float* d_xyz_lidar, int64_t n, int downsample, cudaStream_t st,
-                          int* launches, const MapAddCount& cnt = MapAddCount());
 /* main.cpp:91-93 (lv_sweep_to_world_device_async): *d_n points (clamped to [0, n_max]) of d_xyz (LiDAR frame) transformed by the
  * state in d_ctrl->x into d_out (may equal d_xyz); *d_n_out and *count (a device word the transform reads) = that count, or 0 when
  * gate_n is given and its count (clamped to [0, gate_max]) is below max(gate_min, 1) (main.cpp:81 breaks before publishing) */

@@ -401,11 +401,6 @@ cudaError_t map_add(MapBuffers& b, const float* d_xyz, int64_t n, int downsample
     return cudaGetLastError();
 }
 
-cudaError_t map_add_sweep(MapBuffers& b, const UpdateCtrl* d_ctrl, const float* d_xyz_lidar, int64_t n, int downsample, cudaStream_t st,
-                          int* launches, const MapAddCount& cnt) {
-    return map_add(b, d_xyz_lidar, n, b.empty ? 0 : downsample, st, launches, cnt, d_ctrl);
-}
-
 /* one thread reads every count before it writes: d_n_out may equal d_n or the gate's count */
 __global__ void lv_world_count_kernel(const int64_t* d_n, int64_t n_max, const int64_t* gate_n, int64_t gate_max, int64_t gate_min,
                                       uint32_t* count, int64_t* d_n_out, uint32_t* err) {
