@@ -317,6 +317,12 @@ lv_status lv_voxelgrid_downsample(lv_handle h, const float* xyz, int64_t n, floa
  * d_xyz and d_xyz_out overlap                                                                              */
 lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_t n, float downsample_prec,
                                          float* d_xyz_out, int64_t* n_out);
+/* lv_voxelgrid_downsample_full_device_async on HOST buffers of n points (the outputs need room for n; time_out, intensity_out and
+ * range_out may be NULL); synchronises.  LV_ERR_ARG for a null handle or input, n outside [0, 2^31 - 1] or a leaf <= 0.  The
+ * overflow pass-through returns LV_OK with *n_out = n and PCL's warning in lv_last_error(), as lv_voxelgrid_downsample. */
+lv_status lv_voxelgrid_downsample_full(lv_handle h, const float* xyz, const double* time, const float* intensity, int64_t n,
+                                       float downsample_prec, float* xyz_out, double* time_out, float* intensity_out, float* range_out,
+                                       int64_t* n_out);
 
 /* ---- wire format of the LiDAR message (SURVEY 8f row 4, last item) --------------------------------------
  * PointCloudProcessor::msg2points (src/Utils/PointCloudProcessor.cpp:24-99) on the raw `data` of a
@@ -392,6 +398,18 @@ lv_status lv_compensate_device_async(lv_handle h, const lv_state32* path, int32_
  * device.  The n_max-point ranges of d_xyz and d_xyz_out must not overlap. */
 lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max,
                                                float downsample_prec, float* d_xyz_out, int64_t* d_n_out);
+/* Compensator::voxelgrid_downsample (Compensator.cpp:148-163) of full points, as the reference runs it on full_info::Points
+ * (Processor::fill -> pcl::VoxelGrid<full_info::Point> -> Point(const full_info::Point&), Point.cpp:21-25,164-168): per leaf the xyz
+ * centroid of lv_voxelgrid_downsample_device_async (bit for bit the same), intensity = the fp32 sum of the leaf's intensities in the
+ * same order divided by the count (CentroidPoint's AccumulatorIntensity), range = the fp32 norm of the centroid, time = 0 (no
+ * accumulator carries timestamp).  On a cell-index overflow PCL hands the input on: xyz, time and intensity are passed through,
+ * and range is the fp32 norm of each passed point, because Compensator.cpp:161 builds every output point with Point(p), whose
+ * set_attributes sets range = |p| (Point.cpp:166-169).  So range is always the norm of the output xyz, and no input range is
+ * taken.  The three inputs are required (time is read by the pass-through only); d_time_out, d_intensity_out and d_range_out may
+ * each be NULL.  No output range may overlap an input range or another output range (n_max points each, 8 bytes for a count). */
+lv_status lv_voxelgrid_downsample_full_device_async(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity,
+                                                    const int64_t* d_n, int64_t n_max, float downsample_prec, float* d_xyz_out,
+                                                    double* d_time_out, float* d_intensity_out, float* d_range_out, int64_t* d_n_out);
 /* main.cpp:81-88: `if (ds_compensated.size() < MAX_POINTS2MATCH) break; localizator.correct(ds_compensated, t2)` on *d_n points of
  * d_xyz (device, LiDAR frame).  Below max(min_points, 1) points the update does not run: state, P and last_time_updated are left
  * as they are and the status lv_last_logs fetches is LV_TOO_FEW_POINTS.  On a map the host knows to be empty it returns
@@ -419,6 +437,13 @@ lv_status lv_sweep_to_world_device_async(lv_handle h, const float* d_xyz_lidar, 
  * own.  Content, point ids, order and lv_map_info counters equal those of lv_map_add_device with the count on the host; the growth
  * bound (lv_map_set_growth) uses n_max. */
 lv_status lv_map_add_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, int downsample);
+/* Publishers::pointcloud's header stamp (Publishers.hpp:51-60 -> Processor::fill, PointCloudProcessor.cpp:125-133): starting from 0,
+ * the maximum over the *d_n (clamped to [0, n_max]) times of d_time of Conversions::sec2Microsec(t) = std::round(t * 1e6) as uint64
+ * (Utils.cpp:14-16: the product in double, rounded half away from zero), written to *d_stamp_us; 0 for a count of 0.  Specified
+ * for finite, non-negative times below 2^64 us only (the reference's conversion is undefined elsewhere).  The downsampled clouds'
+ * times are all 0 (lv_voxelgrid_downsample_full), so their stamp is 0, as in the reference; where the voxel grid passed its input
+ * through (cell-index overflow) the times are the input's and the stamp is their maximum.  One launch of one block. */
+lv_status lv_cloud_stamp_device_async(lv_handle h, const double* d_time, const int64_t* d_n, int64_t n_max, uint64_t* d_stamp_us);
 /* the deferred errors of the _async calls since the last lv_async_status, and the map's capacity flags (as lv_map_status):
  * LV_ERR_ARG (lv_last_error names the stage), LV_ERR_CAPACITY or LV_OK.  Clears them; the handle stays usable.  Synchronises. */
 lv_status lv_async_status(lv_handle h);
@@ -442,15 +467,31 @@ lv_status lv_async_status(lv_handle h);
  * messages a tick may leave behind); the live points stay, in order.  LV_ERR_CAPACITY when more points are live than fit.
  * Synchronises. */
 lv_status lv_lidar_reserve(lv_handle h, int64_t capacity);
+/* BUFFER_L holds whole Points (Accumulator.hpp:3,61-74): lv_lidar_reserve with two more float lanes per point, intensity and range
+ * (28 bytes per point), which lv_lidar_push_full_device_async fills and lv_lidar_get_points_full_device_async returns.  Live points
+ * keep their lanes across any later reserve (lv_lidar_reserve keeps the lanes of a ring that has them); points that arrived before
+ * the ring had lanes get intensity 0 and range 0, as does every point of a plain lv_lidar_push_device_async onto a ring with lanes.
+ * Synchronises. */
+lv_status lv_lidar_reserve_full(lv_handle h, int64_t capacity);
 /* Accumulator::receive_lidar's `for (Point p : points) this->add(p);` (Accumulator.cpp:47): appends the *d_n points (clamped to
  * [0, n_max]) of d_xyz (n x 3) / d_time in that order, the last one becoming content[0].  Points that do not fit are a deferred
  * error (lv_async_status) and leave the buffer unchanged: nothing is dropped silently. */
 lv_status lv_lidar_push_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max);
+/* the same with the points' intensity and range (n_max each), e.g. lv_process_cloud_device_async's d_intensity / d_range
+ * (Point.cpp:164-173: the message's intensity, Ouster reflectivity or Hesai uint8; the Ouster's range field, |p| otherwise).  LV_ERR_ARG
+ * on a ring without lanes (lv_lidar_reserve_full first). */
+lv_status lv_lidar_push_full_device_async(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity, const float* d_range,
+                                          const int64_t* d_n, int64_t n_max);
 /* Accumulator::get_points(t1, t2) (Accumulator.cpp:93-95, Accumulator.hpp:61-74): the points of the window, oldest inserted first,
  * into d_xyz (n_max x 3) / d_time (n_max); *d_n_out = their count.  A window of more than n_max points writes count 0 and is a
  * deferred error: the tick that follows is gated off (LV_TOO_FEW_POINTS) and lv_async_status names the stage. */
 lv_status lv_lidar_get_points_device_async(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max,
                                            int64_t* d_n_out);
+/* the same window (the same binary search, ties at t2, order and count) with its intensity and range into d_intensity / d_range
+ * (n_max each).  Deskew keeps the attributes and the order (RotTransl.cpp:43-48), so these lanes stay aligned with
+ * lv_compensate_device_async's output and lv_sweep_to_world_device_async's.  LV_ERR_ARG on a ring without lanes. */
+lv_status lv_lidar_get_points_full_device_async(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, float* d_intensity,
+                                                float* d_range, int64_t n_max, int64_t* d_n_out);
 /* the same kernels, then the count read back into *n_out (host); a window above n_max returns LV_ERR_CAPACITY with *n_out = 0
  * and lv_last_error() naming its size.  Synchronises. */
 lv_status lv_lidar_get_points_device(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* n_out);

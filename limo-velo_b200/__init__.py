@@ -158,6 +158,13 @@ def lib():
     if hasattr(L, "lv_sweep_to_world_device_async"):   # the tick's output and mapping step; absent from older builds
         L.lv_sweep_to_world_device_async.argtypes = [vp, vp, vp, i64, vp, vp]
         L.lv_map_add_device_async.argtypes = [vp, vp, vp, i64, C.c_int]
+    if hasattr(L, "lv_lidar_reserve_full"):   # full points (intensity, range) through the tick; absent from older builds
+        L.lv_lidar_reserve_full.argtypes = [vp, i64]
+        L.lv_lidar_push_full_device_async.argtypes = [vp, vp, vp, vp, vp, vp, i64]
+        L.lv_lidar_get_points_full_device_async.argtypes = [vp, C.c_double, C.c_double, vp, vp, vp, vp, i64, vp]
+        L.lv_voxelgrid_downsample_full.argtypes = [vp, vp, vp, vp, i64, C.c_float, vp, vp, vp, vp, C.POINTER(i64)]
+        L.lv_voxelgrid_downsample_full_device_async.argtypes = [vp, vp, vp, vp, vp, i64, C.c_float, vp, vp, vp, vp, vp]
+        L.lv_cloud_stamp_device_async.argtypes = [vp, vp, vp, i64, vp]
     L.lv_synchronize.argtypes = [vp]
     L.lv_profile_enable.argtypes = [vp, C.c_int]
     L.lv_profile_get.argtypes = [vp, C.POINTER(Profile), C.c_int]
@@ -533,6 +540,20 @@ class Localizer:
         _check(self.L.lv_voxelgrid_downsample(self.h, _f(xyz), C.c_int64(xyz.shape[0]), C.c_float(leaf), _f(out), C.byref(n)))
         return out[:n.value].copy()
 
+    def voxelgrid_downsample_full(self, xyz, time, intensity, leaf):
+        """Compensator::voxelgrid_downsample of full points (full_info::Point through pcl::VoxelGrid): returns (xyz, time, intensity,
+        range) of the leaves: the xyz centroids, time 0, the mean intensity and the centroid's norm (on an overflow: the input's xyz,
+        time and intensity, and each point's norm)"""
+        xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+        n = xyz.shape[0]
+        ins = (np.ascontiguousarray(time, np.float64), np.ascontiguousarray(intensity, np.float32))
+        assert all(a.shape == (n,) for a in ins)
+        out = (np.empty_like(xyz), np.empty(n), np.empty(n, np.float32), np.empty(n, np.float32))
+        m = C.c_int64(0)
+        _check(self.L.lv_voxelgrid_downsample_full(self.h, *(a.ctypes.data_as(C.c_void_p) for a in (xyz,) + ins), C.c_int64(n), C.c_float(leaf),
+                                                   *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
+        return tuple(a[:m.value].copy() for a in out)
+
     def voxelgrid_downsample_device(self, d_xyz, n, leaf, d_out):
         m = C.c_int64(0)
         _check(self.L.lv_voxelgrid_downsample_device(self.h, C.c_void_p(d_xyz), C.c_int64(n), C.c_float(leaf), C.c_void_p(d_out),
@@ -613,6 +634,19 @@ class Localizer:
         return _check(self.L.lv_voxelgrid_downsample_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_n), int(n_max), C.c_float(leaf),
                                                                   C.c_void_p(d_out), C.c_void_p(d_n_out)))
 
+    def voxelgrid_downsample_full_async(self, d_xyz, d_time, d_intensity, d_n, n_max, leaf, d_out, d_time_out, d_intensity_out,
+                                        d_range_out, d_n_out):
+        """lv_voxelgrid_downsample_device_async of full points: the leaves' xyz, time 0, mean intensity and centroid norm (an output
+        lane may be None)"""
+        return _check(self.L.lv_voxelgrid_downsample_full_device_async(
+            self.h, C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_n), int(n_max),
+            C.c_float(leaf), C.c_void_p(d_out), C.c_void_p(d_time_out), C.c_void_p(d_intensity_out), C.c_void_p(d_range_out),
+            C.c_void_p(d_n_out)))
+
+    def cloud_stamp_async(self, d_time, d_n, n_max, d_stamp_us):
+        """the published cloud's header stamp (max of round(t * 1e6), uint64 microseconds) of the *d_n times into d_stamp_us"""
+        return _check(self.L.lv_cloud_stamp_device_async(self.h, C.c_void_p(d_time), C.c_void_p(d_n), int(n_max), C.c_void_p(d_stamp_us)))
+
     def correct_device_async(self, d_ptr, d_n, n_max, min_points, time=0.0):
         """Localizator::correct on the *d_n points behind main.cpp:81's MAX_POINTS2MATCH gate; LV_EMPTY_MAP while the host knows the
         map is empty, else LV_OK (the update's own status is fetched later, e.g. by last_logs)"""
@@ -641,6 +675,21 @@ class Localizer:
     def lidar_push_async(self, d_xyz, d_time, d_n, n_max):
         """Accumulator::receive_lidar's push of the *d_n processed points (e.g. lv_process_cloud_device_async's output)"""
         return _check(self.L.lv_lidar_push_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_n), int(n_max)))
+
+    def lidar_reserve_full(self, capacity):
+        """size the buffer for `capacity` full points (xyz, time, intensity, range); synchronises"""
+        return _check(self.L.lv_lidar_reserve_full(self.h, int(capacity)))
+
+    def lidar_push_full_async(self, d_xyz, d_time, d_intensity, d_range, d_n, n_max):
+        """lidar_push_async with the points' intensity and range (a buffer reserved with lidar_reserve_full)"""
+        return _check(self.L.lv_lidar_push_full_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity),
+                                                             C.c_void_p(d_range), C.c_void_p(d_n), int(n_max)))
+
+    def lidar_get_points_full_async(self, t1, t2, d_xyz, d_time, d_intensity, d_range, n_max, d_n_out):
+        """lidar_get_points_async with the window's intensity and range"""
+        return _check(self.L.lv_lidar_get_points_full_device_async(self.h, float(t1), float(t2), C.c_void_p(d_xyz), C.c_void_p(d_time),
+                                                                   C.c_void_p(d_intensity), C.c_void_p(d_range), int(n_max),
+                                                                   C.c_void_p(d_n_out)))
 
     def lidar_get_points_async(self, t1, t2, d_xyz, d_time, n_max, d_n_out):
         """Accumulator::get_points(t1, t2) into device buffers of n_max points; the count goes to d_n_out"""

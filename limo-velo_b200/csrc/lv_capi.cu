@@ -97,6 +97,8 @@ struct lv_context {
     float* d_ds_in = nullptr;          /* staging for the host-buffer variants */
     float* d_ds_out = nullptr;
     int64_t ds_stage_cap = 0;
+    uint8_t* d_ds_lanes = nullptr;     /* attribute staging of lv_voxelgrid_downsample_full: 28 B per point (ds_stage_lanes) */
+    int64_t ds_lanes_cap = 0;
     double* d_reduced = nullptr;       /* 157 doubles */
     double* h_reduced = nullptr;       /* pinned */
     void* d_flush = nullptr;
@@ -353,11 +355,12 @@ void lv_destroy(lv_handle h) {
     if (h->path_copied) cudaEventDestroy(h->path_copied);
     cudaFree(h->d_async); cudaFreeHost(h->h_async);
     cudaFree(h->lidar.xyz); cudaFree(h->lidar.time); cudaFree(h->lidar.words); cudaFreeHost(h->lidar.h_words);
+    cudaFree(h->lidar.intensity); cudaFree(h->lidar.range);
     for (cudaEvent_t e : h->snap_ev) if (e) cudaEventDestroy(e);
     cudaFreeHost(h->h_snap);
     cudaFree(h->d_job); cudaFree(h->d_ref); cudaFree(h->d_redo); cudaFree(h->d_imu); cudaFreeHost(h->h_imu);
     cudaFree(h->d_path); cudaFreeHost(h->h_path); cudaFree(h->d_times); cudaFree(h->d_deskew_in); cudaFree(h->d_bad); cudaFreeHost(h->h_bad);
-    ds_free(h->ds); cudaFree(h->d_ds_in); cudaFree(h->d_ds_out);
+    ds_free(h->ds); cudaFree(h->d_ds_in); cudaFree(h->d_ds_out); cudaFree(h->d_ds_lanes);
     map_free(h->map);
     cudaFree(h->d_sweep); cudaFree(h->d_nn_a); cudaFree(h->d_nn_b); cudaFree(h->d_hard_list); cudaFree(h->d_ctrl); cudaFreeHost(h->h_ctrl); cudaFree(h->d_partials); cudaFree(h->d_group_rows); cudaFree(h->d_group_tickets);
     cudaFree(h->d_reduced); cudaFreeHost(h->h_reduced); cudaFreeHost(h->h_nevals); cudaFree(h->d_flush);
@@ -1220,6 +1223,21 @@ static lv_status ds_stage(lv_context* h, int64_t n) {
     h->ds_stage_cap = cap;
     return LV_OK;
 }
+/* the synchronous voxel grid of n > 0 device points (lanes: the full form's attributes): the async form's kernels over the
+ * host-known count, then the count read back */
+static lv_status voxelgrid_sync(lv_context* h, const float* d_xyz, int64_t n, float leaf, float* d_xyz_out, const VoxelLanes* lanes,
+                                int64_t* n_out) {
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(ds_reserve(h->ds, n));
+    int launches = 0;
+    LV_CUDA(launch_voxelgrid(h->ds, d_xyz, nullptr, n, leaf, d_xyz_out, nullptr, nullptr, h->stream, &launches, lanes));
+    h->prof.total_launches += launches;
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    /* the pass-through (input copied, count n) is done on the device; the host keeps PCL's warning */
+    if (h->ds.h_count[1]) set_error("voxel grid: leaf size too small for the extent of the cloud (cell index overflows): input passed through");
+    *n_out = h->ds.h_count[0];
+    return LV_OK;
+}
 lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_t n, float leaf, float* d_xyz_out, int64_t* n_out) {
     /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids: an output
      * range that overlaps the input would be read after it is overwritten */
@@ -1230,16 +1248,25 @@ lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_
     if (!h || !d_xyz || !d_xyz_out || !n_out || n < 0 || !(leaf > 0.f) || n > 0x7fffffff) return LV_ERR_ARG;
     *n_out = 0;
     if (n == 0) return LV_OK;
+    return voxelgrid_sync(h, d_xyz, n, leaf, d_xyz_out, nullptr, n_out);
+}
+/* the byte ranges of a full voxel grid's n points: inputs [0, 4) (xyz, time, intensity, count), outputs [4, 9); an output may not
+ * overlap an input or another output (the centroid kernel reads a leaf's inputs while other threads write) */
+static bool voxel_full_overlap(const void* const p[9], int64_t n) {
+    const int64_t bytes[9] = {12 * n, 8 * n, 4 * n, 8, 12 * n, 8 * n, 4 * n, 4 * n, 8};
+    for (int o = 4; o < 9; ++o)
+        for (int k = 0; k < o; ++k)
+            if (p[o] && p[k] && ranges_overlap(p[o], bytes[o], p[k], bytes[k])) return true;
+    return false;
+}
+/* the launch of both async voxel grids, after their argument checks */
+static lv_status voxelgrid_async(lv_context* h, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf, float* d_xyz_out,
+                                 int64_t* d_n_out, const VoxelLanes* lanes) {
     LV_CUDA(cudaSetDevice(h->prm.device));
-    LV_CUDA(ds_reserve(h->ds, n));
+    LV_CUDA(ds_reserve(h->ds, n_max));
     int launches = 0;
-    /* the async form's kernels over the host-known count, then the count read back */
-    LV_CUDA(launch_voxelgrid(h->ds, d_xyz, nullptr, n, leaf, d_xyz_out, nullptr, nullptr, h->stream, &launches));
+    LV_CUDA(launch_voxelgrid(h->ds, d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, &h->d_async->err, h->stream, &launches, lanes));
     h->prof.total_launches += launches;
-    LV_CUDA(cudaStreamSynchronize(h->stream));
-    /* the pass-through (input copied, count n) is done on the device; the host keeps PCL's warning */
-    if (h->ds.h_count[1]) set_error("voxel grid: leaf size too small for the extent of the cloud (cell index overflows): input passed through");
-    *n_out = h->ds.h_count[0];
     return LV_OK;
 }
 lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf,
@@ -1250,12 +1277,24 @@ lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, 
     /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids */
     if (ranges_overlap(d_xyz, 12 * n_max, d_xyz_out, 12 * n_max)) { set_error("voxel grid async: the output range overlaps the input range"); return LV_ERR_ARG; }
     if (!handle_ok("voxel grid async", h, n_max)) return LV_ERR_ARG;
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    LV_CUDA(ds_reserve(h->ds, n_max));
-    int launches = 0;
-    LV_CUDA(launch_voxelgrid(h->ds, d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, &h->d_async->err, h->stream, &launches));
-    h->prof.total_launches += launches;
-    return LV_OK;
+    return voxelgrid_async(h, d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, nullptr);
+}
+lv_status lv_voxelgrid_downsample_full_device_async(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity,
+                                                    const int64_t* d_n, int64_t n_max, float leaf, float* d_xyz_out, double* d_time_out,
+                                                    float* d_intensity_out, float* d_range_out, int64_t* d_n_out) {
+    if (!d_xyz || !d_time || !d_intensity || !d_n || !d_xyz_out || !d_n_out) {
+        set_error("voxel grid full: null xyz, time, intensity, count, output or output count");
+        return LV_ERR_ARG;
+    }
+    if (!n_max_ok("voxel grid full", n_max)) return LV_ERR_ARG;
+    if (!(leaf > 0.f)) { set_error("voxel grid full: leaf size must be positive"); return LV_ERR_ARG; }
+    const void* const p[9] = {d_xyz, d_time, d_intensity, d_n, d_xyz_out, d_time_out, d_intensity_out, d_range_out, d_n_out};
+    if (voxel_full_overlap(p, n_max)) { set_error("voxel grid full: an output range overlaps an input or another output"); return LV_ERR_ARG; }
+    if (!handle_ok("voxel grid full", h, n_max)) return LV_ERR_ARG;
+    VoxelLanes lanes;
+    lanes.time = d_time; lanes.intensity = d_intensity;
+    lanes.time_out = d_time_out; lanes.intensity_out = d_intensity_out; lanes.range_out = d_range_out;
+    return voxelgrid_async(h, d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, &lanes);
 }
 lv_status lv_voxelgrid_downsample(lv_handle h, const float* xyz, int64_t n, float leaf, float* xyz_out, int64_t* n_out) {
     if (!h || !xyz || !xyz_out || !n_out || n < 0 || !(leaf > 0.f) || n > 0x7fffffff) return LV_ERR_ARG;
@@ -1268,6 +1307,51 @@ lv_status lv_voxelgrid_downsample(lv_handle h, const float* xyz, int64_t n, floa
     s = lv_voxelgrid_downsample_device(h, h->d_ds_in, n, leaf, h->d_ds_out, n_out);
     if (s != LV_OK) return s;
     LV_CUDA(cudaMemcpyAsync(xyz_out, h->d_ds_out, sizeof(float) * 3 * (size_t)*n_out, cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    return LV_OK;
+}
+/* device staging of the full host form's attributes: in / out time, then in / out intensity and out range */
+static lv_status ds_stage_lanes(lv_context* h, int64_t n) {
+    if (n <= h->ds_lanes_cap) return LV_OK;
+    cudaFree(h->d_ds_lanes);
+    h->d_ds_lanes = nullptr;
+    h->ds_lanes_cap = 0;
+    const int64_t cap = n + n / 4 + 1024;
+    LV_CUDA(cudaMalloc(&h->d_ds_lanes, 28 * (size_t)cap));
+    h->ds_lanes_cap = cap;
+    return LV_OK;
+}
+lv_status lv_voxelgrid_downsample_full(lv_handle h, const float* xyz, const double* time, const float* intensity, int64_t n, float leaf,
+                                       float* xyz_out, double* time_out, float* intensity_out, float* range_out, int64_t* n_out) {
+    if (n_out) *n_out = 0;
+    if (!xyz || !time || !intensity || !xyz_out || !n_out) {
+        set_error("voxel grid full: null xyz, time, intensity, output or n_out");
+        return LV_ERR_ARG;
+    }
+    if (n < 0 || n > 0x7fffffff) { set_error("voxel grid full: n outside [0, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (!(leaf > 0.f)) { set_error("voxel grid full: leaf size must be positive"); return LV_ERR_ARG; }
+    if (!h) { set_error("voxel grid full: null handle"); return LV_ERR_ARG; }
+    if (n == 0) return LV_OK;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    lv_status s = ds_stage(h, n);
+    if (s == LV_OK) s = ds_stage_lanes(h, n);
+    if (s != LV_OK) return s;
+    const int64_t c = h->ds_lanes_cap;
+    VoxelLanes lanes;
+    double* t_in = reinterpret_cast<double*>(h->d_ds_lanes);
+    float* f = reinterpret_cast<float*>(t_in + 2 * c);
+    lanes.time = t_in; lanes.time_out = t_in + c;
+    lanes.intensity = f; lanes.intensity_out = f + c; lanes.range_out = f + 2 * c;
+    LV_CUDA(cudaMemcpyAsync(h->d_ds_in, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
+    LV_CUDA(cudaMemcpyAsync(t_in, time, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
+    LV_CUDA(cudaMemcpyAsync(f, intensity, sizeof(float) * n, cudaMemcpyHostToDevice, h->stream));
+    s = voxelgrid_sync(h, h->d_ds_in, n, leaf, h->d_ds_out, &lanes, n_out);
+    if (s != LV_OK) return s;
+    const size_t m = (size_t)*n_out;
+    LV_CUDA(cudaMemcpyAsync(xyz_out, h->d_ds_out, sizeof(float) * 3 * m, cudaMemcpyDeviceToHost, h->stream));
+    if (time_out) LV_CUDA(cudaMemcpyAsync(time_out, lanes.time_out, sizeof(double) * m, cudaMemcpyDeviceToHost, h->stream));
+    if (intensity_out) LV_CUDA(cudaMemcpyAsync(intensity_out, lanes.intensity_out, sizeof(float) * m, cudaMemcpyDeviceToHost, h->stream));
+    if (range_out) LV_CUDA(cudaMemcpyAsync(range_out, lanes.range_out, sizeof(float) * m, cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(cudaStreamSynchronize(h->stream));
     return LV_OK;
 }
@@ -1379,12 +1463,15 @@ lv_status lv_async_status(lv_handle h) {
 
 /* ---- Accumulator::BUFFER_L (lv_lidar_buffer.cu) ---------------------------------------------------------------------------------- */
 static bool overlaps_lidar(const lv_context* h, const void* p, int64_t bytes) {
-    return ranges_overlap(p, bytes, h->lidar.xyz, 12 * h->lidar.cap) || ranges_overlap(p, bytes, h->lidar.time, 8 * h->lidar.cap) ||
-           ranges_overlap(p, bytes, h->lidar.words, (int64_t)sizeof(LidarWords));
+    const LidarRing& r = h->lidar;
+    return ranges_overlap(p, bytes, r.xyz, 12 * r.cap) || ranges_overlap(p, bytes, r.time, 8 * r.cap) ||
+           ranges_overlap(p, bytes, r.words, (int64_t)sizeof(LidarWords)) ||
+           (r.intensity && (ranges_overlap(p, bytes, r.intensity, 4 * r.cap) || ranges_overlap(p, bytes, r.range, 4 * r.cap)));
 }
-lv_status lv_lidar_reserve(lv_handle h, int64_t capacity) {
-    if (capacity < 1 || capacity > kLidarMaxCapacity) { set_error("lidar reserve: capacity outside [1, 2^30]"); return LV_ERR_ARG; }
-    if (!h) { set_error("lidar reserve: null handle"); return LV_ERR_ARG; }
+/* lv_lidar_reserve (lanes: keep the ring's) and lv_lidar_reserve_full (lanes: always); `what` names the call in the messages */
+static lv_status lidar_resize(lv_handle h, int64_t capacity, bool full, const char* what) {
+    if (capacity < 1 || capacity > kLidarMaxCapacity) { set_error(std::string(what) + ": capacity outside [1, 2^30]"); return LV_ERR_ARG; }
+    if (!h) { set_error(std::string(what) + ": null handle"); return LV_ERR_ARG; }
     LV_CUDA(cudaSetDevice(h->prm.device));
     LidarRing& r = h->lidar;
     if (!r.words) {
@@ -1397,79 +1484,111 @@ lv_status lv_lidar_reserve(lv_handle h, int64_t capacity) {
     }
     LV_CUDA(cudaMemcpyAsync(r.h_words, r.words, sizeof(LidarWords), cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(cudaStreamSynchronize(h->stream));
-    if (capacity == r.cap) return LV_OK;
+    const bool lanes = full || r.intensity;
+    if (capacity == r.cap && lanes == (r.intensity != nullptr)) return LV_OK;
     const int64_t live = r.h_words->tail - r.h_words->head;
     if (live > capacity) {
         char buf[160];
-        snprintf(buf, sizeof(buf), "lidar reserve: %lld points are live, more than a capacity of %lld", (long long)live, (long long)capacity);
+        snprintf(buf, sizeof(buf), "%s: %lld points are live, more than a capacity of %lld", what, (long long)live, (long long)capacity);
         set_error(buf);
         return LV_ERR_CAPACITY;
     }
-    float* xyz = nullptr;
+    float *xyz = nullptr, *intensity = nullptr, *range = nullptr;
     double* time = nullptr;
     cudaError_t e = cudaMalloc(&xyz, sizeof(float) * 3 * (size_t)capacity);
     if (e == cudaSuccess) e = cudaMalloc(&time, sizeof(double) * (size_t)capacity);
+    if (e == cudaSuccess && lanes) e = cudaMalloc(&intensity, sizeof(float) * (size_t)capacity);
+    if (e == cudaSuccess && lanes) e = cudaMalloc(&range, sizeof(float) * (size_t)capacity);
     int launches = 0;
-    if (e == cudaSuccess) e = launch_lidar_move(r, live, xyz, time, capacity, h->stream, &launches);
+    if (e == cudaSuccess) e = launch_lidar_move(r, live, xyz, time, capacity, h->stream, &launches, intensity, range);
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
     if (e != cudaSuccess) {                                       /* the buffer stays as it was */
-        cudaFree(xyz); cudaFree(time);
+        cudaFree(xyz); cudaFree(time); cudaFree(intensity); cudaFree(range);
         cudaGetLastError();
-        set_error(std::string("lidar reserve: ") + cudaGetErrorString(e));
+        set_error(std::string(what) + ": " + cudaGetErrorString(e));
         return LV_ERR_CAPACITY;
     }
     h->prof.total_launches += launches;
-    cudaFree(r.xyz); cudaFree(r.time);
+    cudaFree(r.xyz); cudaFree(r.time); cudaFree(r.intensity); cudaFree(r.range);
     r.xyz = xyz;
     r.time = time;
+    r.intensity = intensity;
+    r.range = range;
     r.cap = capacity;
+    return LV_OK;
+}
+lv_status lv_lidar_reserve(lv_handle h, int64_t capacity) { return lidar_resize(h, capacity, false, "lidar reserve"); }
+lv_status lv_lidar_reserve_full(lv_handle h, int64_t capacity) { return lidar_resize(h, capacity, true, "lidar reserve full"); }
+/* the checks after the null-pointer check and the launch of both pushes: intensity / range NULL = the plain push */
+static lv_status lidar_push_impl(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity, const float* d_range,
+                                 const int64_t* d_n, int64_t n_max, const char* what) {
+    const std::string w(what);
+    if (!n_max_ok(what, n_max)) return LV_ERR_ARG;
+    if (!h) { set_error(w + ": null handle"); return LV_ERR_ARG; }
+    if (!h->lidar.cap) { set_error(w + ": the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
+    if (d_intensity && !h->lidar.intensity) { set_error(w + ": the buffer has no attribute lanes (lv_lidar_reserve_full first)"); return LV_ERR_ARG; }
+    /* the kernel reads the count and the points while it writes the buffer */
+    if (overlaps_lidar(h, d_xyz, 12 * n_max) || overlaps_lidar(h, d_time, 8 * n_max) || overlaps_lidar(h, d_n, 8) ||
+        (d_intensity && (overlaps_lidar(h, d_intensity, 4 * n_max) || overlaps_lidar(h, d_range, 4 * n_max)))) {
+        set_error(w + ": an input range overlaps the buffer");
+        return LV_ERR_ARG;
+    }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    int launches = 0;
+    LV_CUDA(launch_lidar_push(h->lidar, d_xyz, d_time, d_n, n_max, &h->d_async->err, h->stream, &launches, d_intensity, d_range));
+    h->prof.total_launches += launches;
     return LV_OK;
 }
 lv_status lv_lidar_push_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max) {
     if (!d_xyz || !d_time || !d_n) { set_error("lidar push: null xyz, time or count"); return LV_ERR_ARG; }
-    if (!n_max_ok("lidar push", n_max)) return LV_ERR_ARG;
-    if (!h) { set_error("lidar push: null handle"); return LV_ERR_ARG; }
-    if (!h->lidar.cap) { set_error("lidar push: the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
-    /* the kernel reads the count and the points while it writes the buffer */
-    if (overlaps_lidar(h, d_xyz, 12 * n_max) || overlaps_lidar(h, d_time, 8 * n_max) || overlaps_lidar(h, d_n, 8)) {
-        set_error("lidar push: an input range overlaps the buffer");
-        return LV_ERR_ARG;
-    }
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    int launches = 0;
-    LV_CUDA(launch_lidar_push(h->lidar, d_xyz, d_time, d_n, n_max, &h->d_async->err, h->stream, &launches));
-    h->prof.total_launches += launches;
-    return LV_OK;
+    return lidar_push_impl(h, d_xyz, d_time, nullptr, nullptr, d_n, n_max, "lidar push");
 }
-/* the checks and the launch of both forms of get: d_n_out NULL = the synchronous form */
-static lv_status lidar_get_impl(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, const void* count,
-                                int64_t* d_n_out) {
-    if (!d_xyz || !d_time || !count) { set_error("lidar get points: null xyz, time or count"); return LV_ERR_ARG; }
-    if (!n_max_ok("lidar get points", n_max)) return LV_ERR_ARG;
-    if (isnan(t1) || isnan(t2)) { set_error("lidar get points: t1 or t2 is NaN"); return LV_ERR_ARG; }
-    if (ranges_overlap(d_xyz, 12 * n_max, d_time, 8 * n_max) ||
-        (d_n_out && (ranges_overlap(d_n_out, 8, d_xyz, 12 * n_max) || ranges_overlap(d_n_out, 8, d_time, 8 * n_max)))) {
-        set_error("lidar get points: the output ranges overlap");
-        return LV_ERR_ARG;
-    }
-    if (!h) { set_error("lidar get points: null handle"); return LV_ERR_ARG; }
-    if (!h->lidar.cap) { set_error("lidar get points: the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
-    if (overlaps_lidar(h, d_xyz, 12 * n_max) || overlaps_lidar(h, d_time, 8 * n_max) || (d_n_out && overlaps_lidar(h, d_n_out, 8))) {
-        set_error("lidar get points: an output range overlaps the buffer");
-        return LV_ERR_ARG;
-    }
+lv_status lv_lidar_push_full_device_async(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity, const float* d_range,
+                                          const int64_t* d_n, int64_t n_max) {
+    if (!d_xyz || !d_time || !d_intensity || !d_range || !d_n) { set_error("lidar push full: null xyz, time, intensity, range or count"); return LV_ERR_ARG; }
+    return lidar_push_impl(h, d_xyz, d_time, d_intensity, d_range, d_n, n_max, "lidar push full");
+}
+/* the checks and the launch of every form of get: d_n_out NULL = the synchronous form; intensity / range NULL = a plain get */
+static lv_status lidar_get_impl(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, float* d_intensity, float* d_range, int64_t n_max,
+                                const void* count, int64_t* d_n_out, const char* what) {
+    const std::string w(what);
+    if (!d_xyz || !d_time || !count) { set_error(w + ": null xyz, time or count"); return LV_ERR_ARG; }
+    if (!n_max_ok(what, n_max)) return LV_ERR_ARG;
+    if (isnan(t1) || isnan(t2)) { set_error(w + ": t1 or t2 is NaN"); return LV_ERR_ARG; }
+    const void* const outs[5] = {d_xyz, d_time, d_n_out, d_intensity, d_range};
+    const int64_t bytes[5] = {12 * n_max, 8 * n_max, 8, 4 * n_max, 4 * n_max};
+    for (int a = 1; a < 5; ++a)
+        for (int b = 0; b < a; ++b)
+            if (outs[a] && outs[b] && ranges_overlap(outs[a], bytes[a], outs[b], bytes[b])) {
+                set_error(w + ": the output ranges overlap");
+                return LV_ERR_ARG;
+            }
+    if (!h) { set_error(w + ": null handle"); return LV_ERR_ARG; }
+    if (!h->lidar.cap) { set_error(w + ": the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
+    if (d_intensity && !h->lidar.intensity) { set_error(w + ": the buffer has no attribute lanes (lv_lidar_reserve_full first)"); return LV_ERR_ARG; }
+    for (int a = 0; a < 5; ++a)
+        if (outs[a] && overlaps_lidar(h, outs[a], bytes[a])) {
+            set_error(w + ": an output range overlaps the buffer");
+            return LV_ERR_ARG;
+        }
     LV_CUDA(cudaSetDevice(h->prm.device));
     int launches = 0;
-    LV_CUDA(launch_lidar_get(h->lidar, t1, t2, d_xyz, d_time, n_max, d_n_out, d_n_out ? &h->d_async->err : nullptr, h->stream, &launches));
+    LV_CUDA(launch_lidar_get(h->lidar, t1, t2, d_xyz, d_time, n_max, d_n_out, d_n_out ? &h->d_async->err : nullptr, h->stream, &launches,
+                             d_intensity, d_range));
     h->prof.total_launches += launches;
     return LV_OK;
 }
 lv_status lv_lidar_get_points_device_async(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* d_n_out) {
-    return lidar_get_impl(h, t1, t2, d_xyz, d_time, n_max, d_n_out, d_n_out);
+    return lidar_get_impl(h, t1, t2, d_xyz, d_time, nullptr, nullptr, n_max, d_n_out, d_n_out, "lidar get points");
+}
+lv_status lv_lidar_get_points_full_device_async(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, float* d_intensity,
+                                                float* d_range, int64_t n_max, int64_t* d_n_out) {
+    if (!d_intensity || !d_range) { set_error("lidar get points full: null intensity or range"); return LV_ERR_ARG; }
+    return lidar_get_impl(h, t1, t2, d_xyz, d_time, d_intensity, d_range, n_max, d_n_out, d_n_out, "lidar get points full");
 }
 lv_status lv_lidar_get_points_device(lv_handle h, double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* n_out) {
     if (n_out) *n_out = 0;
-    lv_status s = lidar_get_impl(h, t1, t2, d_xyz, d_time, n_max, n_out, nullptr);
+    lv_status s = lidar_get_impl(h, t1, t2, d_xyz, d_time, nullptr, nullptr, n_max, n_out, nullptr, "lidar get points");
     if (s != LV_OK) return s;
     LidarRing& r = h->lidar;
     LV_CUDA(cudaMemcpyAsync(r.h_words, r.words, sizeof(LidarWords), cudaMemcpyDeviceToHost, h->stream));
@@ -1491,6 +1610,21 @@ lv_status lv_lidar_clear_async(lv_handle h, double t) {
     LV_CUDA(cudaSetDevice(h->prm.device));
     int launches = 0;
     LV_CUDA(launch_lidar_clear(h->lidar, t, h->stream, &launches));
+    h->prof.total_launches += launches;
+    return LV_OK;
+}
+lv_status lv_cloud_stamp_device_async(lv_handle h, const double* d_time, const int64_t* d_n, int64_t n_max, uint64_t* d_stamp_us) {
+    if (!d_time || !d_n || !d_stamp_us) { set_error("cloud stamp: null time, count or stamp"); return LV_ERR_ARG; }
+    if (!n_max_ok("cloud stamp", n_max)) return LV_ERR_ARG;
+    /* one block reads the times and the count, then writes the stamp */
+    if (ranges_overlap(d_stamp_us, 8, d_time, 8 * n_max) || ranges_overlap(d_stamp_us, 8, d_n, 8)) {
+        set_error("cloud stamp: the stamp overlaps the times or the count");
+        return LV_ERR_ARG;
+    }
+    if (!handle_ok("cloud stamp", h, n_max)) return LV_ERR_ARG;
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    int launches = 0;
+    LV_CUDA(launch_cloud_stamp(d_time, d_n, n_max, d_stamp_us, &h->d_async->err, h->stream, &launches));
     h->prof.total_launches += launches;
     return LV_OK;
 }

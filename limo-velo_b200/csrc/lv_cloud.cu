@@ -12,7 +12,10 @@
  * The bytes of a kept point are read twice (flag + key, gather), those of a dropped point once (flag).  Every value is
  * assembled from single bytes (lv_wire.h): fields sit at any offset and the message at any address.  Byte offsets are
  * 64-bit: n < 2^31 points of up to 2^31 bytes each.
+ *
+ * Also Processor::fill's header stamp (PointCloudProcessor.cpp:125-133) of a cloud the publishers send: one block, a max-reduction.
  */
+#include <cub/block/block_reduce.cuh>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_select.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
@@ -100,6 +103,30 @@ cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const
     lv_cloud_gather_kernel<<<grid, 256, 0, st>>>(a, s.vals_sorted, s.count, o.xyz, o.time, o.intensity, o.range, o.idx, d_n_out);
     if (!d_n_out) cudaMemcpyAsync(s.h_count, s.count, 2 * sizeof(int), cudaMemcpyDeviceToHost, st);   /* the synchronous form reads them */
     if (launches) *launches += 6;
+    return cudaGetLastError();
+}
+
+/* `pcl.header.stamp = 0; for (p : points) stamp = max(stamp, Conversions::sec2Microsec(p.time));` with sec2Microsec =
+ * std::round(t * 1e6) converted to uint64 (Utils.cpp:14-16): the product unfused, round half away from zero */
+enum { kStampThreads = 1024 };
+__global__ void __launch_bounds__(kStampThreads) lv_cloud_stamp_kernel(const double* __restrict__ time, const int64_t* __restrict__ d_n,
+                                                                       int64_t n_max, unsigned long long* __restrict__ stamp, uint32_t* err) {
+    typedef cub::BlockReduce<unsigned long long, kStampThreads> Reduce;
+    __shared__ typename Reduce::TempStorage red;
+    const int64_t n = device_count(d_n, n_max, err);
+    unsigned long long m = 0;
+    for (int64_t i = threadIdx.x; i < n; i += kStampThreads) {
+        const unsigned long long us = (unsigned long long)round(dmul(time[i], 1e6));
+        m = us > m ? us : m;
+    }
+    const unsigned long long r = Reduce(red).Reduce(m, cub::Max());
+    if (threadIdx.x == 0) *stamp = r;
+}
+
+cudaError_t launch_cloud_stamp(const double* d_time, const int64_t* d_n, int64_t n_max, uint64_t* d_stamp_us, uint32_t* err, cudaStream_t st,
+                               int* launches) {
+    lv_cloud_stamp_kernel<<<1, kStampThreads, 0, st>>>(d_time, d_n, n_max, reinterpret_cast<unsigned long long*>(d_stamp_us), err);
+    if (launches) *launches += 1;
     return cudaGetLastError();
 }
 

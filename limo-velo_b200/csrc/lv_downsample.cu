@@ -9,6 +9,10 @@
  *              runs in ascending cell index (pcl/filters/impl/voxel_grid.hpp, applyFilter with
  *              downsample_all_data_ = true: CentroidPoint / AccumulatorXYZ: fp32 sum, divided by the count).
  *              PCL's std::sort leaves the order inside a leaf unspecified; here it is input order.
+ *              With attribute lanes (lv_voxelgrid_downsample_full) the centroid kernel's <true> instantiation also runs
+ *              AccumulatorIntensity (fp32 sum in the same order, / n), and writes what Point(const full_info::Point&)
+ *              (Point.cpp:21-25,164-168) makes of the leaf: time 0 (no accumulator) and range = |centroid| (fp32).
+ *              Compensator.cpp:161 builds every output point with Point(p), so range is always |output xyz|.
  * Everything stays on the device (the bounding box is consumed by the key kernel, not by the host); the host
  * reads back the output count and one status word.  Streaming integer/byte work: 12 B in per point, 12 B out per
  * leaf, a 32-bit key-value sort between.
@@ -95,29 +99,41 @@ __global__ void __launch_bounds__(256) lv_ds_heads_kernel(const uint32_t* __rest
     if (i < n_max) head[i] = (i < b->n && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
 }
 
-/* one thread per leaf: AccumulatorXYZ (xyz += p in sorted order), centroid = xyz / n */
+/* one thread per leaf: AccumulatorXYZ (xyz += p in sorted order), centroid = xyz / n; Full: the attribute lanes as well */
+template <bool Full>
 __global__ void __launch_bounds__(256) lv_ds_centroid_kernel(const float* __restrict__ xyz, const uint32_t* __restrict__ vals,
                                                              const uint32_t* __restrict__ starts, const int* __restrict__ n_runs,
-                                                             const GridBox* __restrict__ b, float* __restrict__ out) {
+                                                             const GridBox* __restrict__ b, float* __restrict__ out, VoxelLanes lanes) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     const int runs = *n_runs;
     const int64_t n = b->n;
     if (r >= runs) return;
     const uint32_t s = starts[r], e = r + 1 < runs ? starts[r + 1] : (uint32_t)n;
     float sx = 0.f, sy = 0.f, sz = 0.f;
+    float si = 0.f;
     for (uint32_t j = s; j < e; ++j) {
         const uint32_t p = vals[j];
         sx = fadd(sx, xyz[3 * (size_t)p]); sy = fadd(sy, xyz[3 * (size_t)p + 1]); sz = fadd(sz, xyz[3 * (size_t)p + 2]);
+        if (Full) si = fadd(si, lanes.intensity[p]);                 /* AccumulatorIntensity */
     }
     const float cnt = (float)(e - s);
     out[3 * (size_t)r] = fdiv(sx, cnt); out[3 * (size_t)r + 1] = fdiv(sy, cnt); out[3 * (size_t)r + 2] = fdiv(sz, cnt);
+    if (Full) {
+        const float cx = fdiv(sx, cnt), cy = fdiv(sy, cnt), cz = fdiv(sz, cnt);
+        if (lanes.intensity_out) lanes.intensity_out[r] = fdiv(si, cnt);
+        if (lanes.time_out) lanes.time_out[r] = 0.0;                     /* no accumulator for timestamp: value-initialised */
+        if (lanes.range_out) lanes.range_out[r] = wire_norm(cx, cy, cz);   /* set_attributes after set_XYZ: the centroid's norm */
+    }
 }
 
 /* the output count, and PCL's pass-through: when the cell index overflows, pcl::VoxelGrid::applyFilter warns "Leaf size is too
  * small for the input dataset. Integer indices would overflow." and hands the input on unchanged (Compensator::voxelgrid_downsample
- * carries on with it): the input is copied over the centroids and the count is the input's.  count[0] becomes the output count. */
+ * carries on with it): the input is copied over the centroids and the count is the input's.  count[0] becomes the output count.
+ * Full: time and intensity are passed through as well, and range is |p| of each passed point: Compensator.cpp:161 builds every
+ * output point with Point(p), whose set_attributes sets range = this->norm() (Point.cpp:21-25,166-169). */
+template <bool Full>
 __global__ void __launch_bounds__(256) lv_ds_finish_kernel(const float* __restrict__ xyz, const GridBox* __restrict__ b, int* __restrict__ count,
-                                                           float* __restrict__ out, int64_t* __restrict__ n_out) {
+                                                           float* __restrict__ out, int64_t* __restrict__ n_out, VoxelLanes lanes) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t n = b->n;
     const bool pass = b->overflow && n > 0;
@@ -127,6 +143,11 @@ __global__ void __launch_bounds__(256) lv_ds_finish_kernel(const float* __restri
         if (n_out) *n_out = m;
     }
     if (pass && i < 3 * n) out[i] = xyz[i];
+    if (Full && pass && i < n) {
+        if (lanes.time_out) lanes.time_out[i] = lanes.time[i];
+        if (lanes.intensity_out) lanes.intensity_out[i] = lanes.intensity[i];
+        if (lanes.range_out) lanes.range_out[i] = wire_norm(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2]);
+    }
 }
 
 /* temporal_downsample: keep = (rate <= 1 or (i + 1) % rate == 0) and min_dist < |p| (lv_wire.h) */
@@ -188,7 +209,7 @@ void ds_free(DownsampleScratch& s) {
 }
 
 cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf, float* d_out,
-                             int64_t* d_n_out, uint32_t* err, cudaStream_t st, int* launches) {
+                             int64_t* d_n_out, uint32_t* err, cudaStream_t st, int* launches, const VoxelLanes* lanes) {
     const unsigned grid = (unsigned)((n_max + 255) / 256);
     GridBox* box = static_cast<GridBox*>(s.box);
     const float inv = fdiv(1.0f, leaf);
@@ -202,8 +223,15 @@ cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, const int
     tmp = s.tmp_bytes;
     e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags, s.sel, s.count, (int)n_max, st);
     if (e != cudaSuccess) return e;
-    lv_ds_centroid_kernel<<<grid, 256, 0, st>>>(d_xyz, s.vals_sorted, reinterpret_cast<const uint32_t*>(s.sel), s.count, box, d_out);
-    lv_ds_finish_kernel<<<(unsigned)((3 * n_max + 255) / 256), 256, 0, st>>>(d_xyz, box, s.count, d_out, d_n_out);
+    const uint32_t* starts = reinterpret_cast<const uint32_t*>(s.sel);
+    const unsigned fgrid = (unsigned)((3 * n_max + 255) / 256);
+    if (lanes) {
+        lv_ds_centroid_kernel<true><<<grid, 256, 0, st>>>(d_xyz, s.vals_sorted, starts, s.count, box, d_out, *lanes);
+        lv_ds_finish_kernel<true><<<fgrid, 256, 0, st>>>(d_xyz, box, s.count, d_out, d_n_out, *lanes);
+    } else {
+        lv_ds_centroid_kernel<false><<<grid, 256, 0, st>>>(d_xyz, s.vals_sorted, starts, s.count, box, d_out, VoxelLanes());
+        lv_ds_finish_kernel<false><<<fgrid, 256, 0, st>>>(d_xyz, box, s.count, d_out, d_n_out, VoxelLanes());
+    }
     if (!d_n_out) {                           /* the synchronous form reads the count and the warning flag */
         cudaMemcpyAsync(&s.h_count[0], s.count, sizeof(int), cudaMemcpyDeviceToHost, st);
         cudaMemcpyAsync(&s.h_count[1], &box->overflow, sizeof(int), cudaMemcpyDeviceToHost, st);

@@ -202,11 +202,21 @@ struct DownsampleScratch {
 };
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n);
 void ds_free(DownsampleScratch& s);
+/* the attribute lanes of a full voxel grid (lv_voxelgrid_downsample_full): the inputs (intensity summed per leaf; time read by
+ * the overflow pass-through only; range is never read: every output's range is |output xyz|) and the outputs, any of which may
+ * be NULL */
+struct VoxelLanes {
+    const double* time = nullptr;
+    const float* intensity = nullptr;
+    double* time_out = nullptr;
+    float* intensity_out = nullptr;
+    float* range_out = nullptr;
+};
 /* the voxel grid over d_n ? *d_n : n_max points (the sort runs over n_max, padding keys last), the PCL cell-index overflow
  * pass-through decided on the device; afterwards s.count[0] = output count (also written to *d_n_out when non-NULL),
- * s.h_count[0] / [1] = output count / overflow flag after a stream sync */
+ * s.h_count[0] / [1] = output count / overflow flag after a stream sync.  lanes non-NULL: the full points' attributes too */
 cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf, float* d_out,
-                             int64_t* d_n_out, uint32_t* err, cudaStream_t st, int* launches);
+                             int64_t* d_n_out, uint32_t* err, cudaStream_t st, int* launches, const VoxelLanes* lanes = nullptr);
 cudaError_t launch_temporal(DownsampleScratch& s, const float* d_xyz, int64_t n, int rate, double min_dist, float* d_out,
                             int32_t* d_idx_out, cudaStream_t st, int* launches);
 
@@ -230,6 +240,10 @@ int64_t cloud_bound(int64_t n, int rate);
  * gets kAsyncCloudNaN for a NaN time */
 cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err, cudaStream_t st,
                                  int* launches);
+/* Processor::fill's header stamp (PointCloudProcessor.cpp:125-133): *d_stamp_us = max over the *d_n (clamped to [0, n_max]) times of
+ * round(t * 1e6) as uint64 (Conversions::sec2Microsec, Utils.cpp:14-16), 0 for no point.  One launch */
+cudaError_t launch_cloud_stamp(const double* d_time, const int64_t* d_n, int64_t n_max, uint64_t* d_stamp_us, uint32_t* err, cudaStream_t st,
+                               int* launches);
 
 /* lv_deskew.cu: Compensator::compensate over d_n ? *d_n : n_max points.  d_bad (one int) is set when a timestamp is out of
  * range / out of order; err (may be NULL) gets kAsyncDeskewPath then too */
@@ -248,20 +262,26 @@ struct LidarWords {
 struct LidarRing {
     float* xyz = nullptr;      /* cap x 3 */
     double* time = nullptr;    /* cap     */
+    float* intensity = nullptr;   /* cap, or NULL: a ring without attribute lanes (lv_lidar_reserve_full adds them) */
+    float* range = nullptr;       /* cap, with intensity */
     int64_t cap = 0;           /* 0: not reserved yet */
     LidarWords* words = nullptr;
     LidarWords* h_words = nullptr;   /* pinned */
 };
-/* push *d_n (clamped to [0, n_max]) points; kAsyncLidarFull and nothing appended when they do not fit */
+/* push *d_n (clamped to [0, n_max]) points; kAsyncLidarFull and nothing appended when they do not fit.  On a ring with lanes the
+ * points' intensity and range go with them (NULL: 0) */
 cudaError_t launch_lidar_push(const LidarRing& r, const float* xyz, const double* time, const int64_t* d_n, int64_t n_max, uint32_t* err,
-                              cudaStream_t st, int* launches);
+                              cudaStream_t st, int* launches, const float* intensity = nullptr, const float* range = nullptr);
 /* Accumulator::get(BUFFER_L, t1, t2) into xyz / time; the count goes to words->count and to *d_n_out (may be NULL); a window
- * above n_max writes count 0 and raises kAsyncLidarWindow (err may be NULL) */
+ * above n_max writes count 0 and raises kAsyncLidarWindow (err may be NULL).  intensity / range non-NULL (a ring with lanes
+ * only): the window's lanes too */
 cudaError_t launch_lidar_get(const LidarRing& r, double t1, double t2, float* xyz, double* time, int64_t n_max, int64_t* d_n_out, uint32_t* err,
-                             cudaStream_t st, int* launches);
+                             cudaStream_t st, int* launches, float* intensity = nullptr, float* range = nullptr);
 cudaError_t launch_lidar_clear(const LidarRing& r, double t, cudaStream_t st, int* launches);
-/* copy the `live` live points of `from` into the arrays of a ring of capacity cap (the counters stay as they are) */
-cudaError_t launch_lidar_move(const LidarRing& from, int64_t live, float* xyz, double* time, int64_t cap, cudaStream_t st, int* launches);
+/* copy the `live` live points of `from` into the arrays of a ring of capacity cap (the counters stay as they are); intensity /
+ * range non-NULL: into those lanes too (0 where `from` has none) */
+cudaError_t launch_lidar_move(const LidarRing& from, int64_t live, float* xyz, double* time, int64_t cap, cudaStream_t st, int* launches,
+                              float* intensity = nullptr, float* range = nullptr);
 
 }  // namespace lv
 #endif

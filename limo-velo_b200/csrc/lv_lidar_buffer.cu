@@ -12,6 +12,9 @@
  *   clear  one block walks up from head chunk by chunk until a point fails `t >= time` (the lowest such position, a
  *          min-reduction); head moves there, or to tail.
  * Each is one launch; the counters never leave the device.
+ * A ring reserved with lv_lidar_reserve_full carries two more float lanes per slot, intensity and range.  Push, get and move are
+ * templates on `Lanes`: the <false> instantiations are the xyz + time kernels as they always were, and the <true> ones copy the
+ * lanes in the same loop, slot for slot (lidar_copy_lanes).  Clear reads times only and has one form.
  */
 #include <cub/block/block_scan.cuh>
 
@@ -22,10 +25,19 @@ namespace lv {
 
 enum { kLidarPushThreads = 256, kLidarBlock = 1024 };
 
+/* the lanes of one launch (Lanes = true): intensity and range of the source and of the destination; a NULL source stores 0 */
+struct LaneCopy {
+    const float* from_i;
+    const float* from_r;
+    float* to_i;
+    float* to_r;
+};
+
+template <bool Lanes>
 __global__ void __launch_bounds__(kLidarPushThreads) lv_lidar_push_kernel(float* __restrict__ ring_xyz, double* __restrict__ ring_time, int64_t cap,
                                                                           LidarWords* w, const float* __restrict__ xyz,
                                                                           const double* __restrict__ time, const int64_t* __restrict__ d_n,
-                                                                          int64_t n_max, uint32_t* err) {
+                                                                          int64_t n_max, uint32_t* err, LaneCopy lanes) {
     const int64_t head = w->head, tail = w->tail;
     const int64_t n = device_count(d_n, n_max, err);
     const bool fits = lidar_fits(head, tail, n, cap);
@@ -36,6 +48,7 @@ __global__ void __launch_bounds__(kLidarPushThreads) lv_lidar_push_kernel(float*
             ring_xyz[3 * s + 1] = xyz[3 * i + 1];
             ring_xyz[3 * s + 2] = xyz[3 * i + 2];
             ring_time[s] = time[i];
+            if (Lanes) lidar_copy_lanes(lanes.from_i, lanes.from_r, i, lanes.to_i, lanes.to_r, s);
         }
     }
     /* every thread has read the counters before its block takes a ticket: the last block may move tail */
@@ -50,9 +63,11 @@ __global__ void __launch_bounds__(kLidarPushThreads) lv_lidar_push_kernel(float*
     }
 }
 
+template <bool Lanes>
 __global__ void __launch_bounds__(kLidarBlock) lv_lidar_get_kernel(const float* __restrict__ ring_xyz, const double* __restrict__ ring_time,
                                                                    int64_t cap, LidarWords* w, double t1, double t2, float* __restrict__ xyz,
-                                                                   double* __restrict__ time, int64_t n_max, int64_t* d_n_out, uint32_t* err) {
+                                                                   double* __restrict__ time, int64_t n_max, int64_t* d_n_out, uint32_t* err,
+                                                                   LaneCopy lanes) {
     typedef cub::BlockScan<int, kLidarBlock> Scan;
     __shared__ typename Scan::TempStorage scan;
     __shared__ long long s_top, s_break;
@@ -102,6 +117,7 @@ __global__ void __launch_bounds__(kLidarBlock) lv_lidar_get_kernel(const float* 
             xyz[3 * o + 1] = ring_xyz[3 * s + 1];
             xyz[3 * o + 2] = ring_xyz[3 * s + 2];
             time[o] = tp;
+            if (Lanes) lidar_copy_lanes(lanes.from_i, lanes.from_r, s, lanes.to_i, lanes.to_r, o);
         }
         base += total;
         __syncthreads();                                         /* the scan's storage is reused */
@@ -128,8 +144,10 @@ __global__ void __launch_bounds__(kLidarBlock) lv_lidar_clear_kernel(const doubl
 }
 
 /* lv_lidar_reserve: the live positions into a ring of another capacity, each to slot p % new_cap (the counters stay) */
+template <bool Lanes>
 __global__ void __launch_bounds__(256) lv_lidar_move_kernel(const float* __restrict__ from_xyz, const double* __restrict__ from_time, int64_t from_cap,
-                                                            const LidarWords* w, float* __restrict__ xyz, double* __restrict__ time, int64_t cap) {
+                                                            const LidarWords* w, float* __restrict__ xyz, double* __restrict__ time, int64_t cap,
+                                                            LaneCopy lanes) {
     const int64_t head = w->head, tail = w->tail;
     for (int64_t p = head + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < tail; p += (int64_t)gridDim.x * blockDim.x) {
         const int64_t a = lidar_slot(p, from_cap), b = lidar_slot(p, cap);
@@ -137,6 +155,7 @@ __global__ void __launch_bounds__(256) lv_lidar_move_kernel(const float* __restr
         xyz[3 * b + 1] = from_xyz[3 * a + 1];
         xyz[3 * b + 2] = from_xyz[3 * a + 2];
         time[b] = from_time[a];
+        if (Lanes) lidar_copy_lanes(lanes.from_i, lanes.from_r, a, lanes.to_i, lanes.to_r, b);
     }
 }
 
@@ -146,15 +165,23 @@ static unsigned lidar_grid(int64_t n) {
 }
 
 cudaError_t launch_lidar_push(const LidarRing& r, const float* xyz, const double* time, const int64_t* d_n, int64_t n_max, uint32_t* err,
-                              cudaStream_t st, int* launches) {
-    lv_lidar_push_kernel<<<lidar_grid(n_max), kLidarPushThreads, 0, st>>>(r.xyz, r.time, r.cap, r.words, xyz, time, d_n, n_max, err);
+                              cudaStream_t st, int* launches, const float* intensity, const float* range) {
+    const LaneCopy lanes{intensity, range, r.intensity, r.range};
+    if (r.intensity)
+        lv_lidar_push_kernel<true><<<lidar_grid(n_max), kLidarPushThreads, 0, st>>>(r.xyz, r.time, r.cap, r.words, xyz, time, d_n, n_max, err, lanes);
+    else
+        lv_lidar_push_kernel<false><<<lidar_grid(n_max), kLidarPushThreads, 0, st>>>(r.xyz, r.time, r.cap, r.words, xyz, time, d_n, n_max, err, lanes);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }
 
 cudaError_t launch_lidar_get(const LidarRing& r, double t1, double t2, float* xyz, double* time, int64_t n_max, int64_t* d_n_out, uint32_t* err,
-                             cudaStream_t st, int* launches) {
-    lv_lidar_get_kernel<<<1, kLidarBlock, 0, st>>>(r.xyz, r.time, r.cap, r.words, t1, t2, xyz, time, n_max, d_n_out, err);
+                             cudaStream_t st, int* launches, float* intensity, float* range) {
+    const LaneCopy lanes{r.intensity, r.range, intensity, range};
+    if (intensity)
+        lv_lidar_get_kernel<true><<<1, kLidarBlock, 0, st>>>(r.xyz, r.time, r.cap, r.words, t1, t2, xyz, time, n_max, d_n_out, err, lanes);
+    else
+        lv_lidar_get_kernel<false><<<1, kLidarBlock, 0, st>>>(r.xyz, r.time, r.cap, r.words, t1, t2, xyz, time, n_max, d_n_out, err, lanes);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }
@@ -165,9 +192,14 @@ cudaError_t launch_lidar_clear(const LidarRing& r, double t, cudaStream_t st, in
     return cudaGetLastError();
 }
 
-cudaError_t launch_lidar_move(const LidarRing& from, int64_t live, float* xyz, double* time, int64_t cap, cudaStream_t st, int* launches) {
+cudaError_t launch_lidar_move(const LidarRing& from, int64_t live, float* xyz, double* time, int64_t cap, cudaStream_t st, int* launches,
+                              float* intensity, float* range) {
     if (live == 0) return cudaSuccess;
-    lv_lidar_move_kernel<<<lidar_grid(live), 256, 0, st>>>(from.xyz, from.time, from.cap, from.words, xyz, time, cap);
+    const LaneCopy lanes{from.intensity, from.range, intensity, range};
+    if (intensity)
+        lv_lidar_move_kernel<true><<<lidar_grid(live), 256, 0, st>>>(from.xyz, from.time, from.cap, from.words, xyz, time, cap, lanes);
+    else
+        lv_lidar_move_kernel<false><<<lidar_grid(live), 256, 0, st>>>(from.xyz, from.time, from.cap, from.words, xyz, time, cap, lanes);
     if (launches) *launches += 1;
     return cudaGetLastError();
 }

@@ -58,5 +58,14 @@ LV_HD bool lidar_keeps(double time, double t2) { return t2 >= time; }
  * this fails (a NaN time stops it, as it stops the loop) */
 LV_HD bool lidar_pops(double time, double t) { return t >= time; }
 
+/* The attribute lanes of a ring reserved with lv_lidar_reserve_full: the reference's BUFFER_L holds whole Points, and push / get
+ * copy their intensity and range with xyz and time (Accumulator.hpp:61-74, Point.cpp:21-35).  One lane copy of element a of a
+ * source into element b of a destination; a source without lanes (NULL) gives 0: a plain push onto a ring with lanes, or
+ * lv_lidar_reserve_full over points that arrived before the ring had lanes. */
+LV_HD void lidar_copy_lanes(const float* from_i, const float* from_r, int64_t a, float* to_i, float* to_r, int64_t b) {
+    to_i[b] = from_i ? from_i[a] : 0.f;
+    to_r[b] = from_r ? from_r[a] : 0.f;
+}
+
 }  // namespace lv
 #endif

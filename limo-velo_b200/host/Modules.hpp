@@ -8,7 +8,7 @@
  * (use-ikfom.cpp:18-19 reaches Localizator::getInstance() / Mapper::getInstance()).
  *
  *   reference                                      here
- *   Points = std::deque<Point> (Common.hpp:231)    lv::Points = std::vector<lv::Point> (xyz + time)
+ *   Points = std::deque<Point> (Common.hpp:231)    lv::Points = std::vector<lv::Point> (xyz, time, intensity, range)
  *   State (Objects.hpp:97-137, fp32)               lv::State  = flat state_ikfom layout (26 doubles) + time
  *   Mapper::add(Points&, t, downsample)            Mapper::add(...)          -> lv_map_build / lv_map_add
  *   Mapper::exists() / size()                      same                      -> lv_map_exists / lv_map_size
@@ -30,7 +30,8 @@
 
 namespace lv {
 
-struct Point { float x, y, z; double time; };
+/* Point (Objects.hpp): xyz, time and the attributes the publishers send (Point::toPCL, Point.cpp:113-122) */
+struct Point { float x, y, z; double time; float intensity, range; };
 typedef std::vector<Point> Points;
 struct IMU { double a[3]; double w[3]; double time; };
 typedef std::deque<IMU> IMUs;
@@ -198,16 +199,24 @@ class Compensator {
         return res;
     }
     Points compensate(const Points& sweep) { return sweep; }                   /* a sweep that arrives deskewed (synthetic reader) */
-    /* Compensator::downsample -> voxelgrid_downsample (Compensator.cpp:115-118,148-163): centroids carry xyz only */
+    /* Compensator::downsample -> voxelgrid_downsample (Compensator.cpp:115-118,148-163) of full points: per leaf the centroid, time 0,
+     * the mean intensity and range = |centroid| (Point(const full_info::Point&), Point.cpp:21-25) — lv_voxelgrid_downsample_full.
+     * When PCL passes the input through (cell-index overflow) the points keep xyz, time and intensity, and range becomes |p| */
     Points downsample(const Points& sweep, float downsample_prec) {
         if (sweep.empty()) return Points();
-        std::vector<float> xyz(3 * sweep.size()), out(3 * sweep.size());
-        for (size_t i = 0; i < sweep.size(); ++i) { xyz[3 * i] = sweep[i].x; xyz[3 * i + 1] = sweep[i].y; xyz[3 * i + 2] = sweep[i].z; }
+        const size_t n = sweep.size();
+        std::vector<float> xyz(3 * n), out(3 * n), in_i(n), out_i(n), out_r(n);
+        std::vector<double> t(n), out_t(n);
+        for (size_t i = 0; i < n; ++i) {
+            xyz[3 * i] = sweep[i].x; xyz[3 * i + 1] = sweep[i].y; xyz[3 * i + 2] = sweep[i].z;
+            t[i] = sweep[i].time; in_i[i] = sweep[i].intensity;
+        }
         int64_t m = 0;
-        if (lv_voxelgrid_downsample(ctx.h, xyz.data(), (int64_t)sweep.size(), downsample_prec, out.data(), &m) != LV_OK)
-            return sweep;                                                      /* PCL returns the input when it refuses */
+        check(lv_voxelgrid_downsample_full(ctx.h, xyz.data(), t.data(), in_i.data(), (int64_t)n, downsample_prec, out.data(), out_t.data(),
+                                           out_i.data(), out_r.data(), &m),
+              "Compensator::downsample");                                      /* the overflow pass-through is LV_OK, done on the device */
         Points res((size_t)m);
-        for (int64_t i = 0; i < m; ++i) res[(size_t)i] = Point{out[3 * i], out[3 * i + 1], out[3 * i + 2], 0.0};
+        for (int64_t i = 0; i < m; ++i) res[(size_t)i] = Point{out[3 * i], out[3 * i + 1], out[3 * i + 2], out_t[i], out_i[i], out_r[i]};
         return res;
     }
     Points downsample(const Points& sweep) { return sweep; }                   /* a sweep that arrives downsampled */
@@ -228,7 +237,10 @@ class Compensator {
 class Accumulator {
    public:
     Accumulator() = default;
-    explicit Accumulator(Context& c, int64_t lidar_capacity) : ctx(&c) { check(lv_lidar_reserve(c.h, lidar_capacity), "Accumulator"); }
+    /* full: BUFFER_L keeps each point's intensity and range too (lv_lidar_reserve_full), for the *_full forms below */
+    explicit Accumulator(Context& c, int64_t lidar_capacity, bool full = false) : ctx(&c) {
+        check(full ? lv_lidar_reserve_full(c.h, lidar_capacity) : lv_lidar_reserve(c.h, lidar_capacity), "Accumulator");
+    }
     void receive_lidar(const Points& sweep) { points = sweep; }                /* Accumulator.cpp:39-48 */
     /* Accumulator::receive_lidar on the message's bytes in device memory: Accumulator::process (lv_process_cloud_device_async into
      * the caller's scratch d_xyz / d_time / d_n, room for msg_n points) -> every point pushed onto BUFFER_L; no host wait */
@@ -243,9 +255,25 @@ class Accumulator {
               "Accumulator::receive_lidar_device");
         if (m.n > 0) check(lv_lidar_push_device_async(ctx->h, d_xyz, d_time, d_n, m.n), "Accumulator::receive_lidar_device");
     }
+    /* the same with whole Points: the message's intensity and range (Point.cpp:164-173) go into the caller's d_intensity / d_range
+     * and onto a BUFFER_L made with `full` */
+    void receive_lidar_device_full(const DeviceMessage& m, float* d_xyz, double* d_time, float* d_intensity, float* d_range, int64_t* d_n) {
+        check(lv_process_cloud_device_async(ctx->h, m.type, m.layout, m.d_data, m.data_bytes, m.n, m.stamp_us, m.stamp_beginning,
+                                            m.offset_beginning, m.full_rotation_time, m.downsample_rate, m.min_dist, d_xyz, d_time,
+                                            d_intensity, d_range, nullptr, d_n),
+              "Accumulator::receive_lidar_device_full");
+        if (m.n > 0)
+            check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.n), "Accumulator::receive_lidar_device_full");
+    }
     /* Accumulator::get_points(t1, t2) (Accumulator.hpp:61-74) into device buffers of n_max points; the count goes to *d_n_out */
     void get_points_device(double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* d_n_out) {
         check(lv_lidar_get_points_device_async(ctx->h, t1, t2, d_xyz, d_time, n_max, d_n_out), "Accumulator::get_points_device");
+    }
+    /* the same window with its intensity and range */
+    void get_points_device_full(double t1, double t2, float* d_xyz, double* d_time, float* d_intensity, float* d_range, int64_t n_max,
+                                int64_t* d_n_out) {
+        check(lv_lidar_get_points_full_device_async(ctx->h, t1, t2, d_xyz, d_time, d_intensity, d_range, n_max, d_n_out),
+              "Accumulator::get_points_device_full");
     }
     void clear_lidar(double t) { check(lv_lidar_clear_async(ctx->h, t), "Accumulator::clear_lidar"); }   /* Accumulator.cpp:68-70 */
     void receive_imu(const IMU& imu) { imus.push_back(imu); }

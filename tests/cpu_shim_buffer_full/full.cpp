@@ -1,0 +1,103 @@
+/*
+ * tests/cpu_shim_buffer_full/full.cpp — TEST-ONLY host build of the device LiDAR buffer with attribute lanes (lv_lidar_buffer.h).
+ *
+ * A ring of `cap` slots with xyz, time and, once it has them, the intensity / range lanes of lv_lidar_reserve_full, driven serially
+ * through the header's functions as lv_lidar_buffer.cu's push / get / move kernels use them: the same slot mapping, the same binary
+ * search, the same predicates, and lidar_copy_lanes for every lane copy (a source without lanes stores 0).  Not part of the product.
+ */
+#include <vector>
+
+#include "../../limo-velo_b200/csrc/lv_lidar_buffer.h"
+
+using namespace lv;
+
+struct ShimRing {
+    int64_t cap, head = 0, tail = 0;
+    bool lanes = false;
+    std::vector<float> xyz, intensity, range;
+    std::vector<double> time;
+};
+
+extern "C" {
+
+ShimRing* shim_full_create(int64_t cap, int lanes) {
+    ShimRing* r = new ShimRing();
+    r->cap = cap;
+    r->lanes = lanes != 0;
+    r->xyz.assign(3 * (size_t)cap, 0.f);
+    r->time.assign((size_t)cap, 0.0);
+    if (r->lanes) { r->intensity.assign((size_t)cap, -1.f); r->range.assign((size_t)cap, -1.f); }
+    return r;
+}
+void shim_full_destroy(ShimRing* r) { delete r; }
+int64_t shim_full_size(const ShimRing* r) { return r->tail - r->head; }
+
+/* lv_lidar_reserve (lanes = 0: keep the ring's) / lv_lidar_reserve_full (lanes = 1): the live positions into new arrays, slot
+ * p % new_cap; 0 when more points are live than fit */
+int shim_full_reserve(ShimRing* r, int64_t cap, int lanes) {
+    if (r->tail - r->head > cap) return 0;
+    ShimRing n;
+    n.cap = cap;
+    n.lanes = lanes || r->lanes;
+    n.xyz.assign(3 * (size_t)cap, 0.f);
+    n.time.assign((size_t)cap, 0.0);
+    if (n.lanes) { n.intensity.assign((size_t)cap, -1.f); n.range.assign((size_t)cap, -1.f); }
+    for (int64_t p = r->head; p < r->tail; ++p) {
+        const int64_t a = lidar_slot(p, r->cap), b = lidar_slot(p, cap);
+        for (int c = 0; c < 3; ++c) n.xyz[3 * b + c] = r->xyz[3 * a + c];
+        n.time[b] = r->time[a];
+        if (n.lanes)
+            lidar_copy_lanes(r->lanes ? r->intensity.data() : nullptr, r->lanes ? r->range.data() : nullptr, a, n.intensity.data(),
+                             n.range.data(), b);
+    }
+    r->cap = cap;
+    r->lanes = n.lanes;
+    r->xyz.swap(n.xyz);
+    r->time.swap(n.time);
+    r->intensity.swap(n.intensity);
+    r->range.swap(n.range);
+    return 1;
+}
+
+/* 1: appended; 0: they do not fit.  intensity / range NULL: the plain push (lanes, if any, get 0) */
+int shim_full_push(ShimRing* r, const float* xyz, const double* time, const float* intensity, const float* range, int64_t n) {
+    if (!lidar_fits(r->head, r->tail, n, r->cap)) return 0;
+    for (int64_t i = 0; i < n; ++i) {
+        const int64_t s = lidar_slot(r->tail + i, r->cap);
+        for (int c = 0; c < 3; ++c) r->xyz[3 * s + c] = xyz[3 * i + c];
+        r->time[s] = time[i];
+        if (r->lanes) lidar_copy_lanes(intensity, range, i, r->intensity.data(), r->range.data(), s);
+    }
+    r->tail += n;
+    return 1;
+}
+
+/* the window's size; its points and lanes are written (ascending position) only when it fits n_max */
+int64_t shim_full_get(const ShimRing* r, double t1, double t2, float* xyz, double* time, float* intensity, float* range, int64_t n_max) {
+    const int64_t top = lidar_window_top(r->time.data(), r->cap, r->head, r->tail, t2);
+    int64_t brk = r->head - 1;
+    for (int64_t p = top; p >= r->head; --p)
+        if (lidar_breaks(r->time[lidar_slot(p, r->cap)], t1)) { brk = p; break; }
+    int64_t count = 0;
+    for (int64_t p = brk + 1; p <= top; ++p) count += lidar_keeps(r->time[lidar_slot(p, r->cap)], t2) ? 1 : 0;
+    if (count > n_max) return count;
+    int64_t o = 0;
+    for (int64_t p = brk + 1; p <= top; ++p) {
+        const int64_t s = lidar_slot(p, r->cap);
+        if (!lidar_keeps(r->time[s], t2)) continue;
+        for (int c = 0; c < 3; ++c) xyz[3 * o + c] = r->xyz[3 * s + c];
+        time[o] = r->time[s];
+        lidar_copy_lanes(r->intensity.data(), r->range.data(), s, intensity, range, o);
+        ++o;
+    }
+    return count;
+}
+
+void shim_full_clear(ShimRing* r, double t) {
+    int64_t stop = r->tail;
+    for (int64_t p = r->head; p < r->tail; ++p)
+        if (!lidar_pops(r->time[lidar_slot(p, r->cap)], t)) { stop = p; break; }
+    r->head = stop;
+}
+
+}  // extern "C"

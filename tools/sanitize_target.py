@@ -76,3 +76,33 @@ assert loc.async_status() == (lv.OK, "")
 dev.close()
 loc.close()
 print("sanitize target: lidar buffer ok", flush=True)
+
+# full points: the buffer's lane kernels, the full voxel grid (and its pass-through) and the stamp, against the restatement
+import full_points_ref as P
+from test_gpu_full_points import FullBuffer, same_window as same_full_window
+loc = lv.Localizer(lv.default_params(max_points=1 << 13, max_map_points=1 << 13))
+dev, ref = FullBuffer(loc, 2000, n_max=4096), P.LidarBufferFull()
+for j in range(8):
+    xyz, t = velodyne_message(rng, 1.0 + 0.01 * j - (0.03 if j == 5 else 0.0), 8)
+    inten, rg = (None, None) if j == 2 else (rng.uniform(0, 255, len(t)).astype(np.float32), rng.uniform(0, 90, len(t)).astype(np.float32))
+    if ref.size() + len(t) > 2000:
+        ref.clear(1.0 + 0.01 * j - 0.02)
+        loc.lidar_clear_async(1.0 + 0.01 * j - 0.02)
+    dev.push(xyz, t, inten, rg)
+    ref.push_message(xyz, t, inten, rg)
+    same_full_window(dev, ref, float(t[0]), float(t[-1]), j)
+loc.lidar_reserve(2500)
+same_full_window(dev, ref, -np.inf, np.inf, "reserve")
+for pts, leaf in ((sweep[:3000], 0.5), (np.array([[0, 0, 0], [8388607, 255, 0], [8388608, 0, 0]], np.float32), 1.0)):
+    n = len(pts)
+    t, inten, rg = rng.uniform(0, 20, n), rng.uniform(0, 255, n).astype(np.float32), rng.uniform(0, 90, n).astype(np.float32)
+    got, want = loc.voxelgrid_downsample_full(pts, t, inten, leaf), P.voxelgrid_full(pts, t, inten, leaf)
+    assert all(np.array_equal(a, b) for a, b in zip(got, want))
+d_t, d_n, d_s = loc.upload(np.sort(rng.uniform(1.7e9, 1.7e9 + 0.1, 3000))), loc.upload(np.array([3000], np.int64)), loc.device_alloc(8)
+loc.cloud_stamp_async(d_t, d_n, 3000, d_s)
+assert loc.async_status() == (lv.OK, "")
+dev.close()
+for d in (d_t, d_n, d_s):
+    loc.device_free(d)
+loc.close()
+print("sanitize target: full points ok", flush=True)
