@@ -470,7 +470,16 @@ LV_HD_NOINLINE void map_merge_run(const VoxelMapRW& m, const uint32_t* skeys, co
                     if (cached) ocell[wr] = ocell[t];
                     own[wr++] = q;
                 }
-                if (cached) ocell[wr] = gcell;
+                if (cached) {
+                    /* the winner is an old point for the later groups: filed under its box cell like every other own point
+                     * (a new point on a face inside the voxel can lie in the box of the next cell, a later group) */
+                    if (best_new >= 0) {
+                        const int lx = cell_coord_old(w.x, ds) - vx0, ly = cell_coord_old(w.y, ds) - vy0, lz = cell_coord_old(w.z, ds) - vz0;
+                        ocell[wr] = (lx < 0 || ly < 0 || lz < 0 || lx >= k || ly >= k || lz >= k) ? (uint8_t)255 : (uint8_t)(lx + k * (ly + k * lz));
+                    } else {
+                        ocell[wr] = gcell;                        /* an old winner was filed under this group's cell */
+                    }
+                }
                 own[wr++] = w;
                 cnt = wr;
                 changed = true;

@@ -146,6 +146,23 @@ int shim_map_check(const ShimMap* sm) {
     }
     return 0;
 }
+/* sizes of the layout: dims = {voxel slots, block slots, arena_top, list capacity}; counters = the kMapCounters words */
+void shim_map_dims(const ShimMap* sm, uint32_t* dims, uint32_t* counters) {
+    dims[0] = sm->rw.mask + 1u;
+    dims[1] = sm->rw.bmask + 1u;
+    dims[2] = sm->counters[kCtrArenaTop];
+    dims[3] = sm->rw.list_cap;
+    memcpy(counters, sm->counters.data(), sizeof(uint32_t) * kMapCounters);
+}
+/* the whole layout as it stands (tests/map_ref.py checks it): both tables, arena[0, arena_top), the touched and dirty lists
+ * of the last add (as many entries as their counters say, at most the list capacity) */
+void shim_map_dump(const ShimMap* sm, uint32_t* table, uint32_t* btable, float* arena, uint32_t* touched, uint32_t* dirty) {
+    memcpy(table, sm->table.data(), sizeof(uint4) * sm->table.size());
+    memcpy(btable, sm->btable.data(), sizeof(uint4) * sm->btable.size());
+    memcpy(arena, sm->arena.data(), sizeof(float4) * (size_t)sm->counters[kCtrArenaTop]);
+    memcpy(touched, sm->touched.data(), sizeof(uint32_t) * std::min(sm->counters[kCtrTouched], sm->rw.list_cap));
+    memcpy(dirty, sm->dirty.data(), sizeof(uint32_t) * std::min(sm->counters[kCtrDirty], sm->rw.list_cap));
+}
 void shim_map_destroy(ShimMap* m) { delete m; }
 
 static void search_setup(const ShimParams* p, float cell, float* max_d2, double* gate, int* max_ring) {

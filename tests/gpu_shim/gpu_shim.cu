@@ -129,4 +129,105 @@ out:
     return rc;
 }
 
+/* ---- the map update (lv_map.cu) through the library's own map_alloc / map_add / map_grow / map_clear / map_free, one stream ---- */
+struct GsMap {
+    MapBuffers b;
+    cudaStream_t st = nullptr;
+    float* d_xyz = nullptr;      /* the points of one add (add_cap x 3) */
+    int64_t* d_n = nullptr;      /* the device count of a MapAddCount add */
+};
+
+void* gs_map_create(int64_t max_map_points, int64_t max_points, float voxel_size, float ds) {
+    GsMap* g = new GsMap();
+    if (cudaStreamCreateWithFlags(&g->st, cudaStreamNonBlocking) != cudaSuccess ||
+        map_alloc(g->b, max_map_points, max_points, voxel_size, ds, g->st) != cudaSuccess ||
+        cudaMalloc(&g->d_xyz, sizeof(float) * 3 * (size_t)g->b.add_cap) != cudaSuccess || cudaMalloc(&g->d_n, sizeof(int64_t)) != cudaSuccess ||
+        map_clear(g->b, g->st, nullptr) != cudaSuccess || cudaStreamSynchronize(g->st) != cudaSuccess) {
+        map_free(g->b);
+        cudaFree(g->d_xyz);
+        cudaFree(g->d_n);
+        if (g->st) cudaStreamDestroy(g->st);
+        delete g;
+        return nullptr;
+    }
+    return g;
+}
+/* n points of xyz (host).  dev_count >= 0: the add takes its count from device memory (MapAddCount: clamped to n, none below
+ * max(min_points, 1), build_if_empty); dev_count < 0: n on the host, as lv_map_add after its argument checks */
+int gs_map_add(void* h, const float* xyz, int64_t n, int downsample, int64_t dev_count, int64_t min_points, int build_if_empty) {
+    GsMap* g = static_cast<GsMap*>(h);
+    int rc = 0;
+    MapAddCount cnt;
+    if (n > g->b.add_cap) return (int)cudaErrorInvalidValue;
+    if (n > 0) GS_CUDA(cudaMemcpyAsync(g->d_xyz, xyz, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, g->st));
+    if (dev_count >= 0) {
+        GS_CUDA(cudaMemcpyAsync(g->d_n, &dev_count, sizeof(int64_t), cudaMemcpyHostToDevice, g->st));
+        cnt.n = g->d_n;
+        cnt.min_points = min_points;
+        cnt.build_if_empty = build_if_empty;
+    }
+    GS_CUDA(map_add(g->b, g->d_xyz, n, downsample, g->st, nullptr, cnt));
+    GS_CUDA(cudaStreamSynchronize(g->st));
+out:
+    return rc;
+}
+int gs_map_grow(void* h, int64_t cap) {
+    GsMap* g = static_cast<GsMap*>(h);
+    int rc = 0;
+    GS_CUDA(map_grow(g->b, cap, g->st, nullptr));
+    if (g->b.add_cap > 0) {                       /* the add scratch grew with the map */
+        cudaFree(g->d_xyz);
+        g->d_xyz = nullptr;
+        GS_CUDA(cudaMalloc(&g->d_xyz, sizeof(float) * 3 * (size_t)g->b.add_cap));
+    }
+    GS_CUDA(cudaStreamSynchronize(g->st));
+out:
+    return rc;
+}
+int gs_map_clear(void* h) {
+    GsMap* g = static_cast<GsMap*>(h);
+    int rc = 0;
+    GS_CUDA(map_clear(g->b, g->st, nullptr));
+    GS_CUDA(cudaStreamSynchronize(g->st));
+out:
+    return rc;
+}
+/* dims = {voxel slots, block slots, arena capacity, list capacity, add capacity}; counters = the kMapCounters device words */
+int gs_map_dims(void* h, int64_t* dims, uint32_t* counters) {
+    GsMap* g = static_cast<GsMap*>(h);
+    int rc = 0;
+    dims[0] = g->b.slots;
+    dims[1] = g->b.bslots;
+    dims[2] = g->b.arena_cap;
+    dims[3] = g->b.list_cap;
+    dims[4] = g->b.add_cap;
+    GS_CUDA(cudaMemcpy(counters, g->b.counters, sizeof(uint32_t) * kMapCounters, cudaMemcpyDeviceToHost));
+out:
+    return rc;
+}
+/* both tables, arena[0, arena_top) and the first n_touched / n_dirty entries of the lists (the caller takes them from the counters) */
+int gs_map_dump(void* h, uint32_t* table, uint32_t* btable, float* arena, uint32_t arena_top, uint32_t* touched, uint32_t n_touched,
+                uint32_t* dirty, uint32_t n_dirty) {
+    GsMap* g = static_cast<GsMap*>(h);
+    int rc = 0;
+    GS_CUDA(cudaMemcpy(table, g->b.table, sizeof(uint4) * 2 * (size_t)g->b.slots, cudaMemcpyDeviceToHost));
+    GS_CUDA(cudaMemcpy(btable, g->b.btable, sizeof(uint4) * (size_t)g->b.bslots, cudaMemcpyDeviceToHost));
+    if (arena_top > g->b.arena_cap) return (int)cudaErrorInvalidValue;
+    GS_CUDA(cudaMemcpy(arena, g->b.arena, sizeof(float4) * (size_t)arena_top, cudaMemcpyDeviceToHost));
+    if (n_touched > g->b.list_cap || n_dirty > g->b.list_cap) return (int)cudaErrorInvalidValue;
+    GS_CUDA(cudaMemcpy(touched, g->b.touched, sizeof(uint32_t) * (size_t)n_touched, cudaMemcpyDeviceToHost));
+    GS_CUDA(cudaMemcpy(dirty, g->b.dirty, sizeof(uint32_t) * (size_t)n_dirty, cudaMemcpyDeviceToHost));
+out:
+    return rc;
+}
+void gs_map_free(void* h) {
+    GsMap* g = static_cast<GsMap*>(h);
+    if (!g) return;
+    map_free(g->b);
+    cudaFree(g->d_xyz);
+    cudaFree(g->d_n);
+    cudaStreamDestroy(g->st);
+    delete g;
+}
+
 }  // extern "C"

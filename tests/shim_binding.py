@@ -42,6 +42,8 @@ def lib():
         L.shim_map_points.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_int64]
         L.shim_map_points.restype = C.c_int64
         L.shim_map_check.argtypes = [C.c_void_p]
+        L.shim_map_dims.argtypes = [C.c_void_p] * 3
+        L.shim_map_dump.argtypes = [C.c_void_p] * 6
         assert L.shim_sizeof_iterlog() == C.sizeof(IterLog)
         _lib = L
     return _lib
@@ -75,6 +77,7 @@ class ShimMap:
         """capacity: map points to size the tables for (default: the build); isolated points need 27 table slots each"""
         self.L = lib()
         xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+        self.k = min(3, max(1, int(np.floor(float(np.float32(cell)) / float(np.float32(0.2)) + 0.5))))   # map_alloc's k
         self.h = self.L.shim_map_create_cap(_f(xyz), xyz.shape[0], int(capacity), C.c_float(cell))
 
     def __del__(self):
@@ -104,6 +107,20 @@ class ShimMap:
     def check(self):
         """0 when every halo bucket equals the concatenation of its 27 own extents, flags are clear, blocks are marked"""
         return int(self.L.shim_map_check(C.c_void_p(self.h)))
+
+    def dump(self):
+        """the layout as it stands: map_ref.Dump of both tables, arena[0, arena_top), counters and the last add's lists"""
+        import map_ref
+        dims, ctr = np.zeros(4, np.uint32), np.zeros(16, np.uint32)
+        self.L.shim_map_dims(C.c_void_p(self.h), dims.ctypes.data_as(C.c_void_p), ctr.ctypes.data_as(C.c_void_p))
+        slots, bslots, top, list_cap = (int(v) for v in dims)
+        table, btable = np.zeros((slots, 8), np.uint32), np.zeros((bslots, 4), np.uint32)
+        arena = np.zeros((max(top, 1), 4), np.uint32)
+        touched = np.zeros(max(1, min(int(ctr[map_ref.CTR_TOUCHED]), list_cap)), np.uint32)
+        dirty = np.zeros(max(1, min(int(ctr[map_ref.CTR_DIRTY]), list_cap)), np.uint32)
+        self.L.shim_map_dump(C.c_void_p(self.h), *(a.ctypes.data_as(C.c_void_p) for a in (table, btable, arena, touched, dirty)))
+        return map_ref.Dump(table, btable, arena[:top], ctr, touched[:min(int(ctr[map_ref.CTR_TOUCHED]), list_cap)],
+                            dirty[:min(int(ctr[map_ref.CTR_DIRTY]), list_cap)], self.k)
 
     def match_all(self, x, prm, xyz, rows=False):
         xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
