@@ -257,6 +257,61 @@ lv_status lv_last_logs(lv_handle h, lv_iter_log* logs, int32_t* n_evals);
 /* Localizator::last_time_updated; synchronises when an lv_correct_device_async is still to be resolved */
 double lv_last_time_updated(lv_handle h);
 
+/* ---- starting a sequence in a saved map (no counterpart in the reference: its README lists prelocalization in a saved map as
+ * work in progress).  The update converges from errors well inside MAX_DIST_PLANE only; lv_prelocalize searches a window of
+ * positions and headings about the gravity axis around the filter's state and moves the state to the best candidate.
+ *
+ * Semantics of lv_prelocalize:
+ *   base state   the filter's current state on the device, the one lv_get_state would return after preceding
+ *                lv_propagate_device / update work.  The call synchronises.
+ *   axes         rotation axis g = grav / |grav| (the state's S2 field), right-hand rule.  Position axes
+ *                u = normalize(e - (e.g) g) and v = g x u, with e the world x axis, or the y axis when |g_x| > 0.9.
+ *   grid         I = floor(radius / step + 1e-9), K = floor(yaw_range / yaw_step + 1e-9) (in double);
+ *                a_i = i step, b_j = j step for i, j in [-I, I]; theta_k = k yaw_step for k in [-K, K].
+ *                Linear index ((k + K)(2I + 1) + (i + I))(2I + 1) + (j + I).  More than 2^24 candidates are refused.
+ *   candidate    rot' = q(g, theta_k) (x) rot and pos' = pos + (a_i u + b_j v), both in fp64 (a_i u + b_j v: the products,
+ *                then the sum); vel' = R(g, theta_k) vel; every other field unchanged.  theta_k = 0 keeps rot and vel as
+ *                they are.
+ *   score        the number of the S scored points whose world point lands in a voxel that holds map points (its
+ *                block-mask bit is set).  The world point is fp32: F_k = make_frame(x with rot').lidar_to_world, once per
+ *                heading; o_ij = (float)(a_i u + b_j v); t = fadd(F_k.t, o_ij); w = fadd(dot3f(F_k.R row, p), t) (rt_apply);
+ *                the voxel of each axis as the map computes it (cell floor(w / map_downsample_size), voxel_size cells).
+ *                A point with a coordinate not below 1e9 m in magnitude, or NaN, never scores (the map holds no such point).
+ *                For k = i = j = 0 the world points are, by construction, bit for bit lv_match_all's g_world at the base.
+ *   subset       S = min(n, max_points); point s is d_xyz_lidar[floor(s n / S)] (int64 arithmetic).
+ *   winner       the highest score; ties go to the smaller |k|, then the smaller i^2 + j^2, then the smaller linear index.
+ *                The selection does not depend on launch order (one packed 64-bit key per candidate, atomicMax).
+ *   effect       the filter state becomes out->x, as lv_set_state(out->x, NULL) would set it; P, the map, the time and
+ *                the recorded sweep (lv_map_add_last_sweep) are unchanged.
+ *   empty map    LV_EMPTY_MAP and nothing changes, also after an asynchronous first build that the gate left empty.
+ *   arguments    LV_ERR_ARG before any device work, also with a null handle, lv_last_error naming the problem: null params,
+ *                result or points, n outside [1, 2^31 - 1], a parameter outside its range, more than 2^24 candidates.
+ * scores_out (host, NULL or lv_preloc_count(p) entries) receives every candidate's score at its linear index: a second peak
+ * far from the winner means the window is ambiguous (a corridor, a symmetric hall).  One kernel launch. */
+typedef struct lv_preloc_params {
+    float radius;       /* half-width (m) of the square of positions searched around the current position, >= 0          */
+    float step;         /* grid step of positions (m), > 0; the voxel edge (voxel_size) is the natural choice              */
+    float yaw_range;    /* half-width (rad) of the headings searched about the gravity axis, in [0, pi] (pi: 3.1415927f)   */
+    float yaw_step;     /* rad, > 0                                                                                      */
+    int32_t max_points; /* sweep points scored, 1 .. 4096 (evenly strided subset when the sweep has more)                 */
+    int32_t pad_;
+} lv_preloc_params;
+typedef struct lv_preloc_result {
+    double x[LV_STATE_LEN]; /* the winning candidate's state (written to the filter)                          */
+    int64_t candidates;     /* (2K+1) (2I+1)^2                                                              */
+    int64_t index;          /* linear index of the winner                                                  */
+    int32_t k, i, j;        /* its heading and position indices                                            */
+    int32_t score;          /* scored points that fall in an occupied voxel                                */
+    int32_t points;         /* points scored (S)                                                           */
+    int32_t pad_;
+} lv_preloc_result;
+/* the number of candidates (2K+1)(2I+1)^2 of p, or -1 for invalid params (or a count above 2^61); no GPU needed.  A count
+ * above 2^24 is returned as it is: lv_prelocalize refuses it. */
+int64_t lv_preloc_count(const lv_preloc_params* p);
+/* d_xyz_lidar: DEVICE buffer of n sweep points in the LiDAR frame (e.g. the deskewed, voxel-grid downsampled first sweep) */
+lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p,
+                         lv_preloc_result* out, int32_t* scores_out /* NULL or lv_preloc_count(p) entries */);
+
 /* ---- utilities --------------------------------------------------------------------------- */
 void* lv_host_alloc(int64_t bytes);                           /* pinned host memory            */
 void lv_host_free(void* p);
@@ -545,6 +600,21 @@ typedef struct lv_imu_sample {
     double linear_acceleration[3];
 } lv_imu_sample;
 lv_status lv_bag_parse_imu(const uint8_t* msg, int64_t size, lv_imu_sample* out);
+
+/* ---- PCD map files (the map format of PCL, pcl::io::savePCDFileBinary, and of most LiDAR SLAM tools).  Host code.
+ * Saving the device map: lv_map_points -> lv_pcd_write.  Loading it: lv_pcd_read -> lv_map_build (KD_TREE::Build: file order
+ * becomes insertion order and point ids).  INTEGRATION.md B7. */
+/* PCD v0.7, DATA binary, FIELDS x y z, SIZE 4 4 4, TYPE F F F, COUNT 1 1 1, WIDTH n, HEIGHT 1, VIEWPOINT 0 0 0 1 0 0 0,
+ * POINTS n; the floats as they are (bit for bit).  LV_ERR_IO for a failed open, a short write or a failed close;
+ * LV_ERR_ARG for a null path, null xyz with n > 0, or n < 0. */
+lv_status lv_pcd_write(const char* path, const float* xyz, int64_t n);
+/* DATA ascii or binary (VERSION 0.7 or .7, '#' comment lines; no COUNT line means counts of 1).  x, y and z must each be
+ * TYPE F, SIZE 4, COUNT 1; every other field (SIZE 1, 2, 4 or 8, any COUNT, '_' padding) is skipped by its bytes.  Points
+ * with a non-finite coordinate are dropped, file order is kept; *n = points kept.  xyz == NULL: only *n is set.
+ * LV_ERR_CAPACITY when cap < *n (nothing is written).  LV_ERR_IO, lv_last_error naming it, for an unreadable file,
+ * DATA binary_compressed (convert it with pcl_convert_pcd_ascii_binary), a missing or ill-typed coordinate field,
+ * POINTS != WIDTH x HEIGHT, a data section shorter than POINTS records, or another malformed header. */
+lv_status lv_pcd_read(const char* path, float* xyz, int64_t cap, int64_t* n);
 
 #ifdef __cplusplus
 }

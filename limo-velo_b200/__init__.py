@@ -67,6 +67,38 @@ class LidarInfo(C.Structure):
     _fields_ = [("points", C.c_int64), ("capacity", C.c_int64), ("oldest_time", C.c_double), ("newest_time", C.c_double)]
 
 
+class PrelocParams(C.Structure):
+    """lv_preloc_params: the window lv_prelocalize searches"""
+    _fields_ = [("radius", C.c_float), ("step", C.c_float), ("yaw_range", C.c_float), ("yaw_step", C.c_float),
+                ("max_points", C.c_int32), ("pad_", C.c_int32)]
+
+
+class PrelocResult(C.Structure):
+    """lv_preloc_result: the winning candidate"""
+    _fields_ = [("x", C.c_double * STATE_LEN), ("candidates", C.c_int64), ("index", C.c_int64), ("k", C.c_int32),
+                ("i", C.c_int32), ("j", C.c_int32), ("score", C.c_int32), ("points", C.c_int32), ("pad_", C.c_int32)]
+
+
+def preloc_count(radius, step, yaw_range, yaw_step, max_points=2048):
+    """the number of candidates of a window, -1 for invalid parameters (no GPU needed)"""
+    return int(lib().lv_preloc_count(C.byref(PrelocParams(radius, step, yaw_range, yaw_step, max_points, 0))))
+
+
+def pcd_write(path, xyz):
+    """the points (m x 3, float32) as a binary PCD v0.7 file with fields x y z"""
+    xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+    _check(lib().lv_pcd_write(str(path).encode(), _f(xyz), xyz.shape[0]))
+
+
+def pcd_read(path):
+    """the finite x y z points of an ascii or binary PCD file, in file order (m x 3, float32)"""
+    L, n = lib(), C.c_int64(0)
+    _check(L.lv_pcd_read(str(path).encode(), None, 0, C.byref(n)))
+    out = np.zeros((max(n.value, 1), 3), np.float32)
+    _check(L.lv_pcd_read(str(path).encode(), _f(out), n.value, C.byref(n)))
+    return out[:n.value]
+
+
 def build(verbose=False):
     """Compile liblimovelo_b200.so in-tree with nvcc for sm_90a (works without a GPU)."""
     cmd = ["make", "-C", _HERE, "-j8"]
@@ -165,6 +197,12 @@ def lib():
         L.lv_voxelgrid_downsample_full.argtypes = [vp, vp, vp, vp, i64, C.c_float, vp, vp, vp, vp, C.POINTER(i64)]
         L.lv_voxelgrid_downsample_full_device_async.argtypes = [vp, vp, vp, vp, vp, i64, C.c_float, vp, vp, vp, vp, vp]
         L.lv_cloud_stamp_device_async.argtypes = [vp, vp, vp, i64, vp]
+    if hasattr(L, "lv_prelocalize"):   # start pose search and PCD files; absent from older builds
+        L.lv_preloc_count.argtypes = [C.POINTER(PrelocParams)]
+        L.lv_preloc_count.restype = i64
+        L.lv_prelocalize.argtypes = [vp, vp, i64, C.POINTER(PrelocParams), C.POINTER(PrelocResult), i32p]
+        L.lv_pcd_write.argtypes = [C.c_char_p, fp, i64]
+        L.lv_pcd_read.argtypes = [C.c_char_p, fp, i64, C.POINTER(i64)]
     L.lv_synchronize.argtypes = [vp]
     L.lv_profile_enable.argtypes = [vp, C.c_int]
     L.lv_profile_get.argtypes = [vp, C.POINTER(Profile), C.c_int]
@@ -476,6 +514,23 @@ class Localizer:
         out = np.zeros((n, 5), np.int32)
         _check(self.L.lv_last_neighbours(self.h, C.c_int64(n), out.ctypes.data_as(C.POINTER(C.c_int32))), allow=(EMPTY_MAP,))
         return out
+
+    def prelocalize(self, d_xyz, n, radius, step, yaw_range, yaw_step, max_points, scores=False):
+        """lv_prelocalize: search the window of positions and headings around the filter's state for the pose at which most of
+        the n sweep points (device buffer, LiDAR frame) land in occupied map voxels, and move the state there.  Returns
+        (status, result dict); with scores=True the dict holds every candidate's score as scores[k + K, i + I, j + I]."""
+        prm = PrelocParams(radius, step, yaw_range, yaw_step, max_points, 0)
+        res = PrelocResult()
+        cnt = self.L.lv_preloc_count(C.byref(prm))
+        buf = np.zeros(max(cnt, 1) if scores else 1, np.int32)
+        st = _check(self.L.lv_prelocalize(self.h, C.c_void_p(d_xyz), int(n), C.byref(prm), C.byref(res),
+                                          buf.ctypes.data_as(C.POINTER(C.c_int32)) if scores else None), allow=(EMPTY_MAP,))
+        out = {k: getattr(res, k) for k, _ in PrelocResult._fields_ if k not in ("x", "pad_")}
+        out["x"] = np.array(res.x[:])
+        if scores and st == OK:
+            I = int(np.floor(float(np.float32(radius)) / float(np.float32(step)) + 1e-9))
+            out["scores"] = buf.reshape(-1, 2 * I + 1, 2 * I + 1)
+        return st, out
 
     # Localizator
     def set_state(self, x, P):

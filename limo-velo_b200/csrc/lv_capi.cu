@@ -19,6 +19,7 @@
 #include "lv_host.h"
 #include "lv_internal.h"
 #include "lv_lidar_buffer.h"
+#include "lv_preloc.h"
 #include "lv_predict.h"
 #include "lv_wire.h"
 
@@ -30,6 +31,7 @@ static_assert(LV_STATE_LEN == kStateLen && LV_DOF == kDof, "state layout");
 
 static thread_local std::string g_last_error;
 static void set_error(const std::string& s) { g_last_error = s; }
+void lvh_set_error(const char* msg) { set_error(msg); }
 
 #define LV_CUDA(call)                                                                            \
     do {                                                                                         \
@@ -105,6 +107,9 @@ struct lv_context {
     /* per-point debug outputs (lazily allocated, max_points) */
     uint8_t* d_valid = nullptr; int32_t* d_nn_idx = nullptr; float* d_nn_sqd = nullptr;
     float* d_plane = nullptr; float* d_dist = nullptr; float* d_gworld = nullptr; double* d_rows = nullptr;
+    /* lv_prelocalize: winner key, heading frames, position offsets, scores (lazily allocated, grows) */
+    void* d_preloc = nullptr;
+    size_t preloc_bytes = 0;
     /* host mirror of the filter (get_x / get_P) */
     double x[LV_STATE_LEN];
     double P[LV_DOF * LV_DOF];
@@ -366,6 +371,7 @@ void lv_destroy(lv_handle h) {
     cudaFree(h->d_reduced); cudaFreeHost(h->h_reduced); cudaFreeHost(h->h_nevals); cudaFree(h->d_flush);
     cudaFree(h->d_valid); cudaFree(h->d_nn_idx); cudaFree(h->d_nn_sqd); cudaFree(h->d_plane);
     cudaFree(h->d_dist); cudaFree(h->d_gworld); cudaFree(h->d_rows);
+    cudaFree(h->d_preloc);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
@@ -1099,6 +1105,119 @@ lv_status lv_last_neighbours(lv_handle h, int64_t n, int32_t* nn_idx) {
     LV_CUDA(cudaGetLastError());
     LV_CUDA(cudaMemcpyAsync(nn_idx, h->d_nn_idx, sizeof(int32_t) * 5 * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(cudaStreamSynchronize(h->stream));
+    return LV_OK;
+}
+
+/* ---- start pose in a saved map (lv_prelocalize) ---------------------------------------------- */
+/* NULL when p is valid (I, K and the candidate count filled in), else what is wrong with it */
+static const char* preloc_params_error(const lv_preloc_params* p, int64_t* I, int64_t* K, int64_t* count) {
+    if (!(p->radius >= 0.f && p->radius <= 3.402823466e38f)) return "radius outside [0, inf)";
+    if (!(p->step > 0.f && p->step <= 3.402823466e38f)) return "step not a positive finite number";
+    if (!(p->yaw_range >= 0.f && p->yaw_range <= 3.14159274f)) return "yaw_range outside [0, pi]";
+    if (!(p->yaw_step > 0.f && p->yaw_step <= 3.402823466e38f)) return "yaw_step not a positive finite number";
+    if (p->max_points < 1 || p->max_points > kPrelocMaxPoints) return "max_points outside [1, 4096]";
+    const double hi = preloc_half(p->radius, p->step), hk = preloc_half(p->yaw_range, p->yaw_step);
+    if ((2.0 * hk + 1.0) * (2.0 * hi + 1.0) * (2.0 * hi + 1.0) > 2305843009213693952.0) return "more than 2^61 candidates";
+    *I = (int64_t)hi;
+    *K = (int64_t)hk;
+    *count = (2 * *K + 1) * (2 * *I + 1) * (2 * *I + 1);
+    return nullptr;
+}
+int64_t lv_preloc_count(const lv_preloc_params* p) {
+    int64_t I, K, c;
+    if (!p || preloc_params_error(p, &I, &K, &c)) return -1;
+    return c;
+}
+lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p, lv_preloc_result* out,
+                         int32_t* scores_out) {
+    if (!p || !out || !d_xyz_lidar) { set_error("prelocalize: null params, result or points"); return LV_ERR_ARG; }
+    if (n < 1 || n > 0x7fffffff) { set_error("prelocalize: n outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    int64_t I = 0, K = 0, count = 0;
+    if (const char* e = preloc_params_error(p, &I, &K, &count)) { set_error(std::string("prelocalize: ") + e); return LV_ERR_ARG; }
+    if (count > LV_PRELOC_MAX_CANDIDATES) {
+        set_error("prelocalize: " + std::to_string((long long)count) + " candidates, more than 2^24");
+        return LV_ERR_ARG;
+    }
+    if (!h) { set_error("prelocalize: null handle"); return LV_ERR_ARG; }
+    if (h->map.empty) { set_error("prelocalize: the map is empty"); return LV_EMPTY_MAP; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    sync_mirror(h);                                               /* the base: what lv_get_state returns */
+    if (h->map_unknown) {                                         /* an async first build the gate may have left without points */
+        LV_CUDA(map_fetch_counters(h->map, h->stream));
+        LV_CUDA(cudaStreamSynchronize(h->stream));
+        if ((int32_t)h->map.h_counters[kCtrPoints] == 0) h->map.empty = true;
+        h->map_unknown = false;
+    }
+    if (h->map.empty) { set_error("prelocalize: the map is empty"); return LV_EMPTY_MAP; }
+
+    const int64_t H = 2 * K + 1, W = 2 * I + 1, P = W * W;
+    const int32_t S = (int32_t)(n < p->max_points ? n : p->max_points);
+    double x0[LV_STATE_LEN];
+    memcpy(x0, h->x, sizeof(x0));
+    const PrelocAxes ax = preloc_axes(x0);
+    std::vector<float> frames((size_t)H * 12);
+    for (int64_t k = -K; k <= K; ++k) {
+        const Rt32 F = preloc_heading_frame(x0, ax, (double)k * (double)p->yaw_step);
+        memcpy(&frames[(size_t)(k + K) * 12], F.R, sizeof(float) * 9);
+        memcpy(&frames[(size_t)(k + K) * 12 + 9], F.t, sizeof(float) * 3);
+    }
+    std::vector<float4> offsets((size_t)P);
+    for (int64_t i = -I; i <= I; ++i)
+        for (int64_t j = -I; j <= I; ++j) {
+            float o[3];
+            preloc_offset(ax, (double)i * (double)p->step, (double)j * (double)p->step, o);
+            offsets[(size_t)((i + I) * W + (j + I))] = make_float4(o[0], o[1], o[2], 0.f);
+        }
+    /* scratch: key (256 B slot), frames, offsets, scores */
+    const size_t off_frames = 256, off_offsets = (off_frames + sizeof(float) * frames.size() + 255) & ~(size_t)255;
+    const size_t off_scores = (off_offsets + sizeof(float4) * offsets.size() + 255) & ~(size_t)255;
+    const size_t bytes = off_scores + (scores_out ? sizeof(int32_t) * (size_t)count : 0);
+    if (bytes > h->preloc_bytes) {
+        cudaFree(h->d_preloc);
+        h->d_preloc = nullptr;
+        h->preloc_bytes = 0;
+        LV_CUDA(cudaMalloc(&h->d_preloc, bytes));
+        h->preloc_bytes = bytes;
+    }
+    uint8_t* base = static_cast<uint8_t*>(h->d_preloc);
+    PrelocArgs a;
+    a.xyz = d_xyz_lidar;
+    a.n = n;
+    a.S = S;
+    a.I = I;
+    a.K = K;
+    a.headings = H;
+    a.positions = P;
+    a.frames = reinterpret_cast<const float*>(base + off_frames);
+    a.offsets = reinterpret_cast<const float4*>(base + off_offsets);
+    a.map = map_view(h->map);
+    a.scores = scores_out ? reinterpret_cast<int32_t*>(base + off_scores) : nullptr;
+    a.best = reinterpret_cast<unsigned long long*>(base);
+    LV_CUDA(cudaMemcpyAsync(base + off_frames, frames.data(), sizeof(float) * frames.size(), cudaMemcpyHostToDevice, h->stream));
+    LV_CUDA(cudaMemcpyAsync(base + off_offsets, offsets.data(), sizeof(float4) * offsets.size(), cudaMemcpyHostToDevice, h->stream));
+    LV_CUDA(cudaMemsetAsync(base, 0, sizeof(unsigned long long), h->stream));
+    int launches = 0;
+    LV_CUDA(launch_preloc(a, h->stream, &launches));
+    h->prof.total_launches += launches;
+    unsigned long long key = 0;
+    LV_CUDA(cudaMemcpyAsync(&key, base, sizeof(key), cudaMemcpyDeviceToHost, h->stream));
+    if (scores_out) LV_CUDA(cudaMemcpyAsync(scores_out, a.scores, sizeof(int32_t) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+
+    const int64_t idx = preloc_key_index(key);
+    const int64_t hk = idx / P, q = idx % P;
+    memset(out, 0, sizeof(*out));
+    out->candidates = count;
+    out->index = idx;
+    out->k = (int32_t)(hk - K);
+    out->i = (int32_t)(q / W - I);
+    out->j = (int32_t)(q % W - I);
+    out->score = preloc_key_score(key);
+    out->points = S;
+    preloc_candidate(x0, ax, (double)out->k * (double)p->yaw_step, (double)out->i * (double)p->step, (double)out->j * (double)p->step,
+                     out->x);
+    memcpy(h->x, out->x, sizeof(h->x));                           /* lv_set_state(out->x, NULL) */
+    h->state_dirty = true;
     return LV_OK;
 }
 

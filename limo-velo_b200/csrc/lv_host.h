@@ -15,5 +15,7 @@
 void lvh_init_state(const lv_params& prm, const float q_imu[4], double* x, double* P);
 /* Localizator::propagate -> esekf::predict (Localizator.cpp:159-173, esekfom.hpp:279-384) */
 void lvh_predict(const lv_params& prm, const double acc[3], const double gyro[3], double dt, double* x, double* P);
+/* the text lv_last_error() returns (this thread) */
+void lvh_set_error(const char* msg);
 
 #endif

@@ -283,5 +283,22 @@ cudaError_t launch_lidar_clear(const LidarRing& r, double t, cudaStream_t st, in
 cudaError_t launch_lidar_move(const LidarRing& from, int64_t live, float* xyz, double* time, int64_t cap, cudaStream_t st, int* launches,
                               float* intensity = nullptr, float* range = nullptr);
 
+/* lv_preloc.cu: the scoring kernel of lv_prelocalize (arithmetic: lv_preloc.h) */
+enum { kPrelocThreads = 256, kPrelocPosPerCta = 64 };
+struct PrelocArgs {
+    const float* xyz;          /* the sweep, n x 3, LiDAR frame (device)                                  */
+    int64_t n;
+    int32_t S;                 /* scored points: xyz[floor(s n / S)], s < S <= kPrelocMaxPoints             */
+    int64_t I, K;              /* half-widths of the position and heading grids                           */
+    int64_t headings;          /* 2K + 1                                                                  */
+    int64_t positions;         /* (2I + 1)^2                                                              */
+    const float* frames;       /* headings x 12: lidar_to_world R (row-major) and t of each heading       */
+    const float4* offsets;     /* positions: the fp32 offset (x, y, z, 0) of each position                */
+    VoxelMapView map;
+    int32_t* scores;           /* headings x positions, or NULL                                           */
+    unsigned long long* best;  /* the largest selection key (preloc_key); 0 before the launch             */
+};
+cudaError_t launch_preloc(const PrelocArgs& a, cudaStream_t st, int* launches);
+
 }  // namespace lv
 #endif
