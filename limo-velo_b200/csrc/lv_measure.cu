@@ -390,7 +390,7 @@ __global__ void __launch_bounds__(kMeasureThreads, 4) lv_fit_kernel(const Measur
                 orig[3] = __float_as_int(q3.w); orig[4] = __float_as_int(q4.w);
                 for (int k = 0; k < 5; ++k) dsq[k] = sq_dist(g[0], g[1], g[2], q[k][0], q[k][1], q[k][2]);
                 LV_FK(58);
-                canonical_neighbour_order(q, dsq, orig);             /* equidistant neighbours: the reference's (distance, x) order */
+                canonical_neighbour_order(q, dsq, orig);             /* equidistant neighbours: (distance, x, y, z, id) */
                 /* Plane.cpp:36-43: 5 neighbours and the farthest closer than MAX_DIST_PLANE */
                 if ((double)d4 < a.gate_d2) {
                     chosen = plane_fit(q, a.planes_threshold, abcd);               /* Plane.cpp:45-55 */

@@ -596,15 +596,33 @@ __device__ __forceinline__ void knn5_rings_warp(const VoxelMapView& m, float gx,
  * search meets first depends on how it walks the map (lanes, buckets, rings); that must not leak into the plane fit,
  * whose rounding depends on the order of its five points.  Called on the five neighbours (ascending distances) before
  * the fit.  (Seen on the bench data: one query of 65 536 in sweep 1 has its 3rd and 4th neighbour at equal distance.)
+ * Points the comparator leaves unordered (equal x: mirror images about the query, duplicates) are put in (y, z, map point id)
+ * order: the reference pops them in whatever order its tree walk left, so any fixed order is as faithful, and without one
+ * the lane count of the search (4 or 8 per query, 32 in the ring search) would decide the plane's last bits.  `id` is the
+ * map point id (insertion order), not a position in the arena.
  */
+LV_HD bool neighbour_before(const float* a, int ia, const float* b, int ib) {
+    if (a[0] != b[0]) return a[0] < b[0];
+    if (a[1] != b[1]) return a[1] < b[1];
+    if (a[2] != b[2]) return a[2] < b[2];
+    return ia < ib;
+}
 LV_HD void canonical_neighbour_order(float (*q)[3], float* d, int* id) {
     /* ascending distances: a tie anywhere shows in one of the four adjacent gaps (a float test first: the fp64 compare of the
      * reference's comparator costs more than the rest of the function and one query in 10^5 has a tie at all) */
     const float gap = fminf(fminf(d[1] - d[0], d[2] - d[1]), fminf(d[3] - d[2], d[4] - d[3]));
     if (!(gap < 2e-10f)) return;
+    /* exactly equal distances first: the search hands them over in lane order, so put them in key order before the 1e-10
+     * relation (not transitive: a chain of near-ties can exceed 1e-10) is applied, and the result depends only on the set */
     for (int pass = 0; pass < 4; ++pass)
         for (int k = 0; k < 4; ++k)
-            if (fabs((double)(d[k + 1] - d[k])) < 1e-10 && q[k + 1][0] < q[k][0]) {
+            if (d[k + 1] == d[k] && neighbour_before(q[k + 1], id[k + 1], q[k], id[k])) {
+                for (int a = 0; a < 3; ++a) { const float t = q[k][a]; q[k][a] = q[k + 1][a]; q[k + 1][a] = t; }
+                const int ti = id[k]; id[k] = id[k + 1]; id[k + 1] = ti;
+            }
+    for (int pass = 0; pass < 4; ++pass)
+        for (int k = 0; k < 4; ++k)
+            if (fabs((double)(d[k + 1] - d[k])) < 1e-10 && neighbour_before(q[k + 1], id[k + 1], q[k], id[k])) {
                 for (int a = 0; a < 3; ++a) { const float t = q[k][a]; q[k][a] = q[k + 1][a]; q[k + 1][a] = t; }
                 const float td = d[k]; d[k] = d[k + 1]; d[k + 1] = td;
                 const int ti = id[k]; id[k] = id[k + 1]; id[k + 1] = ti;

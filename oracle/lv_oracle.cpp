@@ -731,6 +731,29 @@ void map_prepare(const lvo_map* m) {
     m->dirty = false;
 }
 
+// Neighbours PointType_CMP leaves unordered (distances within 1e-10 and equal x) come off the heap in whatever order the
+// walk left them.  They are put in (y, z, point id) order, the product's fixed choice, so that the plane fit sees one row
+// order; the (distance, x) order of the comparator is kept.
+void tie_order(int found, int32_t* idx, float* sqd, float* nn) {
+    auto before = [&](int a, int b) {
+        for (int c = 0; c < 3; ++c)
+            if (nn[3 * a + c] != nn[3 * b + c]) return nn[3 * a + c] < nn[3 * b + c];
+        return idx[a] < idx[b];
+    };
+    auto swap_next = [&](int i) {
+        std::swap(idx[i], idx[i + 1]);
+        std::swap(sqd[i], sqd[i + 1]);
+        for (int c = 0; c < 3; ++c) std::swap(nn[3 * i + c], nn[3 * (i + 1) + c]);
+    };
+    // exact ties first, so that the non-transitive 1e-10 pass below starts from an order that depends only on the set
+    for (int pass = 0; pass + 1 < found; ++pass)
+        for (int i = 0; i + 1 < found; ++i)
+            if (sqd[i + 1] == sqd[i] && before(i + 1, i)) swap_next(i);
+    for (int pass = 0; pass + 1 < found; ++pass)
+        for (int i = 0; i + 1 < found; ++i)
+            if (std::fabs(sqd[i + 1] - sqd[i]) < 1e-10 && before(i + 1, i)) swap_next(i);
+}
+
 int map_knn(const lvo_map* m, const float* g, int k, int32_t* idx, float* sqd, float* nn) {
     if (k > 16) k = 16;
     if (m->backend == LVO_KNN_REF_IKDTREE) {
@@ -741,6 +764,7 @@ int map_knn(const lvo_map* m, const float* g, int k, int32_t* idx, float* sqd, f
             if (sqd) sqd[i] = d[i];
             if (nn) { nn[3 * i] = pts[3 * i]; nn[3 * i + 1] = pts[3 * i + 1]; nn[3 * i + 2] = pts[3 * i + 2]; }
         }
+        if (idx && sqd && nn) tie_order(found, idx, sqd, nn);
         return found;
     }
     map_prepare(m);
@@ -759,6 +783,7 @@ int map_knn(const lvo_map* m, const float* g, int k, int32_t* idx, float* sqd, f
         if (sqd) sqd[i] = it.d;
         if (nn) { nn[3 * i] = m->pts[3 * it.idx]; nn[3 * i + 1] = m->pts[3 * it.idx + 1]; nn[3 * i + 2] = m->pts[3 * it.idx + 2]; }
     }
+    if (idx && sqd && nn) tie_order(found, idx, sqd, nn);
     return found;
 }
 

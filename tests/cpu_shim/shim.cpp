@@ -200,8 +200,11 @@ void shim_match_all(const ShimMap* sm, const double* x, const ShimParams* p, con
         int ids[5] = {t.i0, t.i1, t.i2, t.i3, t.i4};
         float ds[5] = {t.d0, t.d1, t.d2, t.d3, t.d4};
         float q[5][3];
-        if (t.i4 >= 0) {
-            for (int k = 0; k < 5; ++k) { q[k][0] = src[ids[k]].x; q[k][1] = src[ids[k]].y; q[k][2] = src[ids[k]].z; }
+        if (t.i4 >= 0) {                                     /* map point ids, as the fit kernel orders them */
+            for (int k = 0; k < 5; ++k) {
+                q[k][0] = src[ids[k]].x; q[k][1] = src[ids[k]].y; q[k][2] = src[ids[k]].z;
+                memcpy(&ids[k], &src[ids[k]].w, 4);
+            }
             canonical_neighbour_order(q, ds, ids);
         }
         if (t.i4 >= 0 && (double)t.d4 < gate) {
@@ -216,9 +219,7 @@ void shim_match_all(const ShimMap* sm, const double* x, const ShimParams* p, con
         if (valid) valid[i] = chosen;
         if (g_world) memcpy(g_world + 3 * i, g, sizeof(g));
         for (int k = 0; k < 5; ++k) {
-            int32_t orig = -1;
-            if (t.i4 >= 0) memcpy(&orig, &src[ids[k]].w, 4);
-            if (nn_idx) nn_idx[5 * i + k] = orig;
+            if (nn_idx) nn_idx[5 * i + k] = t.i4 >= 0 ? ids[k] : -1;
             if (nn_sqd) nn_sqd[5 * i + k] = t.i4 >= 0 ? ds[k] : INFINITY;
         }
         if (plane) memcpy(plane + 4 * i, abcd, sizeof(abcd));
@@ -319,6 +320,32 @@ void shim_plane_fit(const float* pts5, float thr, float* abcd, int* ok) {
     float q[5][3];
     memcpy(q, pts5, sizeof(q));
     *ok = plane_fit(q, thr, abcd) ? 1 : 0;
+}
+/* tests/gpu_shim's gs_fit_sets on the host: per set, distances from g, the tie order, fit, distance and row */
+void shim_fit_sets(const float* q_in, const float* g_in, const int* id_in, const double* x, float thr, int est, int n, int* id_out,
+                   float* abcd_out, int* ok_out, float* dist_out, double* row_out) {
+    Frame fr;
+    make_frame(x, &fr);
+    for (int i = 0; i < n; ++i) {
+        float q[5][3], d[5], abcd[4];
+        int id[5];
+        const float g[3] = {g_in[3 * i], g_in[3 * i + 1], g_in[3 * i + 2]};
+        for (int k = 0; k < 5; ++k) {
+            for (int a = 0; a < 3; ++a) q[k][a] = q_in[15 * i + 3 * k + a];
+            d[k] = sq_dist(g[0], g[1], g[2], q[k][0], q[k][1], q[k][2]);
+            id[k] = id_in[5 * i + k];
+        }
+        canonical_neighbour_order(q, d, id);
+        ok_out[i] = plane_fit(q, thr, abcd) ? 1 : 0;
+        const float dist = plane_dist(abcd, g);
+        double row[12], h;
+        jacobian_row(fr, g, abcd, dist, est != 0, row, &h);
+        memcpy(id_out + 5 * i, id, sizeof(id));
+        memcpy(abcd_out + 4 * i, abcd, sizeof(abcd));
+        dist_out[i] = dist;
+        memcpy(row_out + 13 * (size_t)i, row, sizeof(row));
+        row_out[13 * (size_t)i + 12] = h;
+    }
 }
 int shim_sizeof_iterlog() { return (int)sizeof(IterLog); }
 unsigned long long shim_block_cube_mask(int cbx, int cby, int cbz, int r) { return block_cube_mask(cbx, cby, cbz, r); }

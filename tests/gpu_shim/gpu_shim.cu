@@ -22,6 +22,34 @@ __global__ void __launch_bounds__(128) gs_prepare_kernel(UpdateCtrl* c) {
     ieskf_prepare(ex, c, &w);
 }
 
+/* the match stage's per-set arithmetic as lv_fit_kernel runs it, one thread per given set: distances from g, the tie order,
+ * the fit, the distance and the row (frame from state x).  q: 15 floats, id: 5 ints per set; out: the reordered ids, abcd,
+ * is_plane, dist and 13 doubles (row, then h) whatever is_plane says */
+__global__ void gs_fit_sets_kernel(const float* q_in, const float* g_in, const int* id_in, const Frame* fr, float thr, int est, int n,
+                                   int* id_out, float* abcd_out, int* ok_out, float* dist_out, double* row_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float q[5][3], d[5], abcd[4];
+    int id[5];
+    const float g[3] = {g_in[3 * i], g_in[3 * i + 1], g_in[3 * i + 2]};
+    for (int k = 0; k < 5; ++k) {
+        for (int a = 0; a < 3; ++a) q[k][a] = q_in[15 * i + 3 * k + a];
+        d[k] = sq_dist(g[0], g[1], g[2], q[k][0], q[k][1], q[k][2]);
+        id[k] = id_in[5 * i + k];
+    }
+    canonical_neighbour_order(q, d, id);
+    const bool ok = plane_fit(q, thr, abcd);
+    const float dist = plane_dist(abcd, g);
+    double row[12], h;
+    jacobian_row(*fr, g, abcd, dist, est != 0, row, &h);
+    for (int k = 0; k < 5; ++k) id_out[5 * i + k] = id[k];
+    for (int k = 0; k < 4; ++k) abcd_out[4 * i + k] = abcd[k];
+    ok_out[i] = ok ? 1 : 0;
+    dist_out[i] = dist;
+    for (int k = 0; k < 12; ++k) row_out[13 * (size_t)i + k] = row[k];
+    row_out[13 * (size_t)i + 12] = h;
+}
+
 #define GS_CUDA(call)                             \
     do {                                          \
         cudaError_t e__ = (call);                 \
@@ -228,6 +256,42 @@ void gs_map_free(void* h) {
     cudaFree(g->d_n);
     cudaStreamDestroy(g->st);
     delete g;
+}
+
+/* gs_fit_sets_kernel on n sets (host arrays in and out; shapes there); returns a cudaError_t */
+int gs_fit_sets(const float* q, const float* g, const int* id, const double* x, float thr, int est, int n, int* id_out, float* abcd,
+                int* ok, float* dist, double* rows) {
+    int rc = 0;
+    Frame fr;
+    make_frame(x, &fr);
+    float *dq = nullptr, *dg = nullptr, *dabcd = nullptr, *ddist = nullptr;
+    int *did = nullptr, *dido = nullptr, *dok = nullptr;
+    double* drows = nullptr;
+    Frame* dfr = nullptr;
+    GS_CUDA(cudaMalloc(&dq, sizeof(float) * 15 * (size_t)n));
+    GS_CUDA(cudaMalloc(&dg, sizeof(float) * 3 * (size_t)n));
+    GS_CUDA(cudaMalloc(&did, sizeof(int) * 5 * (size_t)n));
+    GS_CUDA(cudaMalloc(&dido, sizeof(int) * 5 * (size_t)n));
+    GS_CUDA(cudaMalloc(&dabcd, sizeof(float) * 4 * (size_t)n));
+    GS_CUDA(cudaMalloc(&dok, sizeof(int) * (size_t)n));
+    GS_CUDA(cudaMalloc(&ddist, sizeof(float) * (size_t)n));
+    GS_CUDA(cudaMalloc(&drows, sizeof(double) * 13 * (size_t)n));
+    GS_CUDA(cudaMalloc(&dfr, sizeof(Frame)));
+    GS_CUDA(cudaMemcpy(dq, q, sizeof(float) * 15 * (size_t)n, cudaMemcpyHostToDevice));
+    GS_CUDA(cudaMemcpy(dg, g, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice));
+    GS_CUDA(cudaMemcpy(did, id, sizeof(int) * 5 * (size_t)n, cudaMemcpyHostToDevice));
+    GS_CUDA(cudaMemcpy(dfr, &fr, sizeof(Frame), cudaMemcpyHostToDevice));
+    gs_fit_sets_kernel<<<(unsigned)((n + 127) / 128), 128>>>(dq, dg, did, dfr, thr, est, n, dido, dabcd, dok, ddist, drows);
+    GS_CUDA(cudaGetLastError());
+    GS_CUDA(cudaMemcpy(id_out, dido, sizeof(int) * 5 * (size_t)n, cudaMemcpyDeviceToHost));
+    GS_CUDA(cudaMemcpy(abcd, dabcd, sizeof(float) * 4 * (size_t)n, cudaMemcpyDeviceToHost));
+    GS_CUDA(cudaMemcpy(ok, dok, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost));
+    GS_CUDA(cudaMemcpy(dist, ddist, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost));
+    GS_CUDA(cudaMemcpy(rows, drows, sizeof(double) * 13 * (size_t)n, cudaMemcpyDeviceToHost));
+out:
+    cudaFree(dq); cudaFree(dg); cudaFree(did); cudaFree(dido); cudaFree(dabcd); cudaFree(dok); cudaFree(ddist); cudaFree(drows);
+    cudaFree(dfr);
+    return rc;
 }
 
 }  // extern "C"

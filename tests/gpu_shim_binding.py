@@ -25,6 +25,7 @@ def lib():
         L.gs_map_dims.argtypes = [vp, vp, vp]
         L.gs_map_dump.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32]
         L.gs_map_free.argtypes = [vp]
+        L.gs_fit_sets.argtypes = [vp, vp, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp, vp, vp]
         _lib = L
     return _lib
 

@@ -197,3 +197,20 @@ def plane_fit(pts5, thr):
     ok = C.c_int(0)
     lib().shim_plane_fit(_f(pts5), C.c_float(thr), _f(abcd), C.byref(ok))
     return abcd, bool(ok.value)
+
+
+def fit_sets(q, g, ids, x, thr, est=True, L=None):
+    """the per-set arithmetic of the fit kernel on n given sets (q: n x 5 x 3, g: n x 3, ids: n x 5): the tie order, the fit,
+    the distance and the row.  L: this module's library (host build) or gpu_shim_binding's (the device)."""
+    q = np.ascontiguousarray(q, np.float32).reshape(-1, 15)
+    n = q.shape[0]
+    g = np.ascontiguousarray(g, np.float32).reshape(n, 3)
+    ids = np.ascontiguousarray(ids, np.int32).reshape(n, 5)
+    out = dict(ids=np.zeros((n, 5), np.int32), plane=np.zeros((n, 4), np.float32), ok=np.zeros(n, np.int32),
+               dist=np.zeros(n, np.float32), rows=np.zeros((n, 13)))
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)
+    fn = lib().shim_fit_sets if L is None else L.gs_fit_sets
+    rc = fn(vp(q), vp(g), vp(ids), vp(np.ascontiguousarray(x, np.float64)), C.c_float(thr), int(est), int(n), vp(out["ids"]),
+            vp(out["plane"]), vp(out["ok"]), vp(out["dist"]), vp(out["rows"]))
+    assert L is None or rc == 0, "CUDA error %d" % rc
+    return out

@@ -10,6 +10,10 @@ import bench
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1500, method="thread")]
 
 
+def om_points(mp):
+    return np.ascontiguousarray(mp, np.float32).reshape(-1, 3)
+
+
 def _setup(lv, O, cfg, n_sweeps):
     prm = bench.config_params(lv, cfg)
     world, mp, sweeps, x_props, truths = bench.make_scene(lv, 0, n_sweeps=n_sweeps, prm=prm, cfg=cfg)
@@ -20,7 +24,7 @@ def _setup(lv, O, cfg, n_sweeps):
     om = O.Map(O.KNN_REF_IKDTREE if O.ref_available() else O.KNN_KDTREE)
     om.build(mp)
     x0, P0 = lv.init_state_host(prm)
-    return prm, loc, om, sweeps, x_props, truths, P0, bench.oracle_params(O, prm)
+    return prm, loc, om, sweeps, x_props, truths, P0, bench.oracle_params(O, prm), mp
 
 
 def _check_update(loc, om, oprm, x_prop, P0, sweep, O, min_matches):
@@ -48,9 +52,25 @@ def _check_update(loc, om, oprm, x_prop, P0, sweep, O, min_matches):
     return x, logs
 
 
-def _check_points(loc, om, oprm, x_prop, sweep, max_ties=4):
+def _in_tie_order(points, ids, sqd):
+    """per query: the five (map point ids into `points`, squared distances) are in the product's order, ascending distance
+    and (x, y, z, id) among neighbours less than 1e-10 apart"""
+    p = points[ids]
+    ok = np.ones(len(ids), bool)
+    for k in range(4):
+        near = np.abs(sqd[:, k + 1] - sqd[:, k]) < 1e-10
+        a, b = p[:, k], p[:, k + 1]
+        key_le = ((a[:, 0] < b[:, 0]) | ((a[:, 0] == b[:, 0]) & ((a[:, 1] < b[:, 1]) | ((a[:, 1] == b[:, 1]) & (
+            (a[:, 2] < b[:, 2]) | ((a[:, 2] == b[:, 2]) & (ids[:, k] < ids[:, k + 1])))))))
+        ok &= np.where(near, key_le, sqd[:, k] < sqd[:, k + 1])
+    return ok
+
+
+def _check_points(loc, om, oprm, x_prop, sweep, max_ties=4, points=None, oracle_ids=True):
     """max_ties: at most this many tied queries (None: any number, each of them a tie — maps with repeated points);
-    got["ties"] counts them"""
+    got["ties"] counts them.  points: the map's input in submission order (a map point's id indexes it); with it the
+    neighbour ids are checked to come in the product's order, and (oracle_ids: the oracle's map was built from the same
+    input, so its ids are the same ids) equal to the oracle's kd-tree ids"""
     got = loc.match_all(x_prop, sweep)
     ref = om.match_all(x_prop, oprm, sweep)
     inside = np.isfinite(got["nn_sqd"][:, 4])
@@ -63,25 +83,31 @@ def _check_points(loc, om, oprm, x_prop, sweep, max_ties=4):
         from test_gpu_fullsize import boundary_ties
         assert max_ties is None or len(differ) <= max_ties, differ
         assert len(boundary_ties(om, ref["g"][differ])) == len(differ), differ
+    if points is not None:
+        rest = inside.copy()
+        rest[differ] = False
+        assert _in_tie_order(points, got["nn_idx"][rest], got["nn_sqd"][rest]).all()
+        same_ids = rest & (ref["nn_idx"][:, 0] >= 0) & oracle_ids
+        assert (got["nn_idx"][same_ids] == ref["nn_idx"][same_ids]).all()
     got["ties"] = len(differ)
     return got
 
 
 def test_cfg0_planar_map_single_evaluation(lv, O):
-    prm, loc, om, sweeps, x_props, truths, P0, oprm = _setup(lv, O, "cfg0", 2)
+    prm, loc, om, sweeps, x_props, truths, P0, oprm, mp = _setup(lv, O, "cfg0", 2)
     assert prm.MAX_NUM_ITERS == 0
     for k in range(2):
         x, logs = _check_update(loc, om, oprm, x_props[k], P0, sweeps[k], O, 40000)
         assert len(logs) == 1                                       # I forced to 1 (esekfom.hpp:1634 with max_iter = 0)
         err = np.abs(O.boxminus(x, truths[k]))
         assert err[2] < 5e-3 and err[3:5].max() < 2e-3              # a plane observes z, roll, pitch only
-    got = _check_points(loc, om, oprm, x_props[0], sweeps[0])
+    got = _check_points(loc, om, oprm, x_props[0], sweeps[0], points=om_points(mp))
     assert got["valid"].mean() > 0.8
     loc.close()
 
 
 def test_cfg2_kitti_subsweeps_5m_map(lv, O):
-    prm, loc, om, sweeps, x_props, truths, P0, oprm = _setup(lv, O, "cfg2", 1)
+    prm, loc, om, sweeps, x_props, truths, P0, oprm, mp = _setup(lv, O, "cfg2", 1)
     assert prm.estimate_extrinsics == 0 and abs(prm.MAX_DIST_PLANE - 2.23) < 1e-12
     assert len(sweeps) == 10 and all(len(s) == 13107 for s in sweeps)
     for k in range(10):
@@ -89,16 +115,16 @@ def test_cfg2_kitti_subsweeps_5m_map(lv, O):
         for a in logs:                                              # extrinsics not estimated: columns 6..11 of every row are zero
             assert (a["HTH"][6:, :] == 0).all() and (a["HTH"][:, 6:] == 0).all()
     for k in (0, 9):
-        _check_points(loc, om, oprm, x_props[k], sweeps[k])
+        _check_points(loc, om, oprm, x_props[k], sweeps[k], points=om_points(mp))
     loc.close()
 
 
 def test_cfg3_ouster_10m_map(lv, O):
-    prm, loc, om, sweeps, x_props, truths, P0, oprm = _setup(lv, O, "cfg3", 1)
+    prm, loc, om, sweeps, x_props, truths, P0, oprm, mp = _setup(lv, O, "cfg3", 1)
     x, logs = _check_update(loc, om, oprm, x_props[0], P0, sweeps[0], O, 200000)
     err = np.abs(O.boxminus(x, truths[0]))
     assert err[:3].max() < 5e-3 and err[3:6].max() < 5e-4
-    _check_points(loc, om, oprm, x_props[0], sweeps[0])
+    _check_points(loc, om, oprm, x_props[0], sweeps[0], points=om_points(mp))
     # Mapper::add at this size: the sweep, in world coordinates, goes into the 10 M map on the device
     g = bench.world_points(sweeps[0], x)
     loc.map_add(g, downsample=True)

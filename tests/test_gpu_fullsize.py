@@ -21,8 +21,10 @@ def full(lv, O):
 
 
 def boundary_ties(om, g):
-    """The queries (world points g, n x 3) whose 5th and 6th nearest map points are EXACTLY equidistant (fp32 squared
-    distance, the search's arithmetic).  WHICH of the two joins the five is then decided by the order a search meets them:
+    """The queries (world points g, n x 3) whose 5th and 6th nearest map points are equidistant under the reference's
+    comparator: fp32 squared distances (the search's arithmetic) less than 1e-10 apart (PointType_CMP, ikd_Tree.h:109-115;
+    below ~1.6e-3 m^2 that window holds distinct fp32 values, and the reference's heap, whose top() is the comparator's
+    maximum, can then keep the 6th and drop the 5th: test_match_cases.test_near_ties_inside_the_comparators_window).  WHICH of the two joins the five is then decided by the order a search meets them:
     the reference's max-heap keeps the first one its tree walk visits (ikd_Tree.cpp:1087-1093, strict <), the voxel
     search has other walks, and inside an update a query may keep the five an earlier evaluation found.  About one query
     in 10^6 is such a tie, i.e. one update in ten has one.  Found with the oracle's own 6-NN.  Two copies of one point are
@@ -30,7 +32,7 @@ def boundary_ties(om, g):
     out = []
     for i in range(len(g)):
         found, idx, sqd, nn = om.knn(g[i], 6)
-        if found == 6 and sqd[4] == sqd[5] and (nn[4] != nn[5]).any():
+        if found == 6 and abs(sqd[5] - sqd[4]) < 1e-10 and (nn[4] != nn[5]).any():
             out.append(i)
     return np.array(out, dtype=np.int64)
 

@@ -61,7 +61,8 @@ def test_every_search_shape_matches_the_oracle(lv, O, scenes, monkeypatch, name,
             monkeypatch.delenv("LV_SEARCH_GROUP", raising=False)
         else:
             monkeypatch.setenv("LV_SEARCH_GROUP", str(group))
-        got = _check_points(loc, om, oprm, sc.x, sc.queries, max_ties=None if name == "cluster" else 4)
+        got = _check_points(loc, om, oprm, sc.x, sc.queries, max_ties=None if name == "cluster" else 4,
+                            points=np.concatenate([sc.build] + sc.adds), oracle_ids=not sc.adds)
         st, HTH, HTh, nm = loc.measure_reduced(sc.x, sc.queries)
         assert st == st_o
         if got["ties"] == 0:
