@@ -312,6 +312,48 @@ int64_t lv_preloc_count(const lv_preloc_params* p);
 lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p,
                          lv_preloc_result* out, int32_t* scores_out /* NULL or lv_preloc_count(p) entries */);
 
+/* ---- the start pose anywhere in a saved map: an exact branch-and-bound form of the same search, for windows that cover a
+ * whole map.
+ *
+ * Semantics of lv_prelocalize_global: base state, axes, grid, candidate, score, subset, winner, effect, empty map and
+ * arguments as lv_prelocalize above, except:
+ *   cap          up to 2^40 candidates and 2^20 headings (yaw_step >= about 6e-6 rad over every heading); more are refused
+ *                (LV_ERR_ARG, "more than 2^40" / "more than 2^20").  There is no scores array: only a fraction of the
+ *                candidates is ever scored.
+ *   result       out holds exactly what lv_prelocalize would return for the same state, map, points and params: index,
+ *                k, i, j, score, points, candidates, and x bit for bit; the filter state is set the same way.  P, the
+ *                time, the map and the recorded sweep are untouched.
+ *   how          a cell is one heading with an aligned block of 2^l x 2^l positions (clipped at the window's edge).
+ *                Every step from (i, j) to a point's voxel is monotone per axis, so over a cell each voxel coordinate of
+ *                a scored point lies between its values at the cell's four corners; the cell's upper bound counts the
+ *                points whose voxel box may hold an occupied voxel.  A cell is pruned only when its bound is strictly
+ *                below a score some candidate reaches, so every candidate that could win or tie is scored exactly with
+ *                lv_prelocalize's arithmetic.  The cells are bounded at 32 x 32 positions (more for very large windows),
+ *                taken in order of bound, and refined level by level; level-1 survivors are scored exactly.
+ *   stats        NULL or filled.  Every count depends on the inputs only (not on launch order or timing).  Each candidate
+ *                counts once in candidates_scored.  launches counts the search's launches; the map's occupancy summary
+ *                (extent and bitmaps, two launches) is built once per map state and kept until an add, build or growth
+ *                changes the map (those launches appear in the profile's total_launches, not in stats).
+ *   environment  LV_PRELOC_NO_PRUNE=1 (read at each call) scores every candidate through the same exact kernel and
+ *                selection, bounding nothing: the exhaustive reference for windows above lv_prelocalize's cap.
+ * Covering every position inside the map's extent: lv_map_extent, then radius = the largest |(c - pos).u|, |(c - pos).v|
+ * over the box's corners c (INTEGRATION.md B7).  Synchronises; several launches (stats->launches). */
+typedef struct lv_preloc_stats {
+    int64_t candidates;        /* (2K+1)(2I+1)^2 of the window                                              */
+    int64_t cells_bounded;     /* cells (blocks of positions x one heading) whose upper bound was computed  */
+    int64_t candidates_scored; /* candidates scored exactly (level 0)                                       */
+    int64_t probes;            /* occupancy probes, all levels: S per bounded cell and per scored candidate */
+    int32_t launches, pad_;    /* kernel launches of the search                                             */
+} lv_preloc_stats;
+lv_status lv_prelocalize_global(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p,
+                                lv_preloc_result* out, lv_preloc_stats* stats /* NULL or filled */);
+/* axis-aligned box (world frame, metres) of the occupied voxels' extent: lo = the low face of the lowest occupied voxel,
+ * hi = the high face of the highest (voxel_low of the next voxel), per axis.  A window built from it as above covers every
+ * position inside the map's extent.  A sweep reaches beyond the vehicle, so a pose just outside the box can still see the
+ * map: pad the radius by the sweep's range to include those.  Synchronises; LV_EMPTY_MAP on an empty map; LV_ERR_ARG for a
+ * null handle, lo or hi. */
+lv_status lv_map_extent(lv_handle h, double lo[3], double hi[3]);
+
 /* ---- utilities --------------------------------------------------------------------------- */
 void* lv_host_alloc(int64_t bytes);                           /* pinned host memory            */
 void lv_host_free(void* p);

@@ -79,6 +79,12 @@ class PrelocResult(C.Structure):
                 ("i", C.c_int32), ("j", C.c_int32), ("score", C.c_int32), ("points", C.c_int32), ("pad_", C.c_int32)]
 
 
+class PrelocStats(C.Structure):
+    """lv_preloc_stats: the work of one lv_prelocalize_global call"""
+    _fields_ = [("candidates", C.c_int64), ("cells_bounded", C.c_int64), ("candidates_scored", C.c_int64), ("probes", C.c_int64),
+                ("launches", C.c_int32), ("pad_", C.c_int32)]
+
+
 def preloc_count(radius, step, yaw_range, yaw_step, max_points=2048):
     """the number of candidates of a window, -1 for invalid parameters (no GPU needed)"""
     return int(lib().lv_preloc_count(C.byref(PrelocParams(radius, step, yaw_range, yaw_step, max_points, 0))))
@@ -203,6 +209,9 @@ def lib():
         L.lv_prelocalize.argtypes = [vp, vp, i64, C.POINTER(PrelocParams), C.POINTER(PrelocResult), i32p]
         L.lv_pcd_write.argtypes = [C.c_char_p, fp, i64]
         L.lv_pcd_read.argtypes = [C.c_char_p, fp, i64, C.POINTER(i64)]
+    if hasattr(L, "lv_prelocalize_global"):   # the whole-map start pose search; absent from older builds
+        L.lv_prelocalize_global.argtypes = [vp, vp, i64, C.POINTER(PrelocParams), C.POINTER(PrelocResult), C.POINTER(PrelocStats)]
+        L.lv_map_extent.argtypes = [vp, dp, dp]
     L.lv_synchronize.argtypes = [vp]
     L.lv_profile_enable.argtypes = [vp, C.c_int]
     L.lv_profile_get.argtypes = [vp, C.POINTER(Profile), C.c_int]
@@ -531,6 +540,23 @@ class Localizer:
             I = int(np.floor(float(np.float32(radius)) / float(np.float32(step)) + 1e-9))
             out["scores"] = buf.reshape(-1, 2 * I + 1, 2 * I + 1)
         return st, out
+
+    def prelocalize_global(self, d_xyz, n, radius, step, yaw_range, yaw_step, max_points):
+        """lv_prelocalize_global: the same search, winner and effect as prelocalize, pruned by an exact upper bound, for windows
+        of up to 2^40 candidates (a whole map).  Returns (status, result dict, stats dict)."""
+        prm = PrelocParams(radius, step, yaw_range, yaw_step, max_points, 0)
+        res, stats = PrelocResult(), PrelocStats()
+        st = _check(self.L.lv_prelocalize_global(self.h, C.c_void_p(d_xyz), int(n), C.byref(prm), C.byref(res), C.byref(stats)),
+                    allow=(EMPTY_MAP,))
+        out = {k: getattr(res, k) for k, _ in PrelocResult._fields_ if k not in ("x", "pad_")}
+        out["x"] = np.array(res.x[:])
+        return st, out, {k: getattr(stats, k) for k, _ in PrelocStats._fields_ if k != "pad_"}
+
+    def map_extent(self):
+        """(lo, hi): the world-frame box of the occupied voxels' faces (m); raises on an empty map"""
+        lo, hi = np.zeros(3), np.zeros(3)
+        _check(self.L.lv_map_extent(self.h, _d(lo), _d(hi)))
+        return lo, hi
 
     # Localizator
     def set_state(self, x, P):

@@ -20,6 +20,7 @@
 #include "lv_internal.h"
 #include "lv_lidar_buffer.h"
 #include "lv_preloc.h"
+#include "lv_preloc_bound.h"
 #include "lv_predict.h"
 #include "lv_wire.h"
 
@@ -110,6 +111,15 @@ struct lv_context {
     /* lv_prelocalize: winner key, heading frames, position offsets, scores (lazily allocated, grows) */
     void* d_preloc = nullptr;
     size_t preloc_bytes = 0;
+    /* lv_prelocalize_global / lv_map_extent: extent, heading frames, cell lists and results, occupancy bitmaps (grows) */
+    void* d_pglob = nullptr;
+    size_t pglob_bytes = 0;
+    /* the occupancy summary (extent, bitmap pyramid) of the map as of map_gen occ_gen; rebuilt when the map changed since */
+    uint64_t map_gen = 0;              /* bumped by every add, build and growth (map_enqueue, map_grow_to) */
+    uint64_t occ_gen = ~0ull;
+    PrelocOcc occ;
+    uint32_t* d_occ = nullptr;         /* extent (8 words), then the bitmaps */
+    size_t occ_bytes = 0;
     /* host mirror of the filter (get_x / get_P) */
     double x[LV_STATE_LEN];
     double P[LV_DOF * LV_DOF];
@@ -372,6 +382,8 @@ void lv_destroy(lv_handle h) {
     cudaFree(h->d_valid); cudaFree(h->d_nn_idx); cudaFree(h->d_nn_sqd); cudaFree(h->d_plane);
     cudaFree(h->d_dist); cudaFree(h->d_gworld); cudaFree(h->d_rows);
     cudaFree(h->d_preloc);
+    cudaFree(h->d_pglob);
+    cudaFree(h->d_occ);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
@@ -411,6 +423,7 @@ static lv_status map_grow_to(lv_context* h, int64_t cap) {
     const bool pr = prof_begin(h, kProfMap, &ep);
     const int64_t old_cap = h->map.cap;
     int launches = 0;
+    h->map_gen++;                                                  /* new tables: the occupancy summary is rebuilt */
     const cudaError_t e = map_grow(h->map, cap, h->stream, &launches);
     if (pr) prof_end(h, &ep);
     if (e != cudaSuccess) {
@@ -591,6 +604,7 @@ static lv_status map_enqueue(lv_context* h, const float* xyz, bool on_host, int6
         xyz = h->map.stage_xyz;
     }
     if (cnt.n && empty) h->map_unknown = true;                   /* a device count of 0 leaves the map without a point */
+    h->map_gen++;                                                  /* the occupancy summary of lv_prelocalize_global is stale */
     EventPair ep;
     const bool pr = prof_begin(h, kProfMap, &ep);
     int launches = 0;
@@ -1216,6 +1230,224 @@ lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const
     out->points = S;
     preloc_candidate(x0, ax, (double)out->k * (double)p->yaw_step, (double)out->i * (double)p->step, (double)out->j * (double)p->step,
                      out->x);
+    memcpy(h->x, out->x, sizeof(h->x));                           /* lv_set_state(out->x, NULL) */
+    h->state_dirty = true;
+    return LV_OK;
+}
+
+/* ---- start pose anywhere in a saved map (lv_prelocalize_global, lv_map_extent) ---------------- */
+/* LV_EMPTY_MAP when the map holds no point (also after an asynchronous first build that the gate left empty) */
+static lv_status pglob_map_empty(lv_context* h, const char* what) {
+    if (h->map_unknown) {
+        LV_CUDA(map_fetch_counters(h->map, h->stream));
+        LV_CUDA(cudaStreamSynchronize(h->stream));
+        if ((int32_t)h->map.h_counters[kCtrPoints] == 0) h->map.empty = true;
+        h->map_unknown = false;
+    }
+    if (h->map.empty) { set_error(std::string(what) + ": the map is empty"); return LV_EMPTY_MAP; }
+    return LV_OK;
+}
+static lv_status pglob_reserve(lv_context* h, size_t bytes) {
+    if (bytes <= h->pglob_bytes) return LV_OK;
+    cudaFree(h->d_pglob);
+    h->d_pglob = nullptr;
+    h->pglob_bytes = 0;
+    LV_CUDA(cudaMalloc(&h->d_pglob, bytes));
+    h->pglob_bytes = bytes;
+    return LV_OK;
+}
+static size_t pglob_align(size_t b) { return (b + 255) & ~(size_t)255; }
+/* the occupancy summary of the map (h->occ: extent, bitmap pyramid in h->d_occ), rebuilt only when the map changed since it
+ * was built (map_gen); LV_EMPTY_MAP when no block holds an occupied voxel */
+static lv_status pglob_occupancy(lv_context* h, const char* what, int* launches) {
+    if (h->occ_gen != h->map_gen) {
+        if (h->occ_bytes < 256) {
+            cudaFree(h->d_occ);
+            h->d_occ = nullptr;
+            h->occ_bytes = 0;
+            LV_CUDA(cudaMalloc(&h->d_occ, 256));
+            h->occ_bytes = 256;
+        }
+        uint32_t ext[6];
+        LV_CUDA(cudaMemsetAsync(h->d_occ, 0xFF, 3 * sizeof(uint32_t), h->stream));
+        LV_CUDA(cudaMemsetAsync(h->d_occ + 3, 0, 3 * sizeof(uint32_t), h->stream));
+        LV_CUDA(launch_occ_extent(map_view(h->map), h->map.bslots, h->d_occ, h->stream, launches));
+        LV_CUDA(cudaMemcpyAsync(ext, h->d_occ, 6 * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+        LV_CUDA(cudaStreamSynchronize(h->stream));
+        PrelocOcc& o = h->occ;
+        memset(&o, 0, sizeof(o));
+        for (int a = 0; a < 3; ++a) { o.lo[a] = ext[a]; o.hi[a] = ext[3 + a]; }
+        if (ext[0] <= ext[3]) {
+            const size_t words = (size_t)occ_layout(o);
+            const size_t bytes = 256 + sizeof(uint32_t) * words;
+            if (bytes > h->occ_bytes) {                            /* the extent stays in the first words: copied out above */
+                cudaFree(h->d_occ);
+                h->d_occ = nullptr;
+                h->occ_bytes = 0;
+                LV_CUDA(cudaMalloc(&h->d_occ, bytes));
+                h->occ_bytes = bytes;
+            }
+            uint32_t* bits = h->d_occ + 64;
+            o.map = map_view(h->map);
+            o.bits = bits;
+            LV_CUDA(cudaMemsetAsync(bits, 0, sizeof(uint32_t) * words, h->stream));
+            LV_CUDA(launch_occ_bits(o, h->map.bslots, bits, h->stream, launches));
+        }
+        h->occ_gen = h->map_gen;
+    }
+    if (h->occ.lo[0] > h->occ.hi[0]) { set_error(std::string(what) + ": the map is empty"); return LV_EMPTY_MAP; }
+    h->occ.map = map_view(h->map);
+    return LV_OK;
+}
+
+lv_status lv_map_extent(lv_handle h, double lo[3], double hi[3]) {
+    if (!h) { set_error("map_extent: null handle"); return LV_ERR_ARG; }
+    if (!lo || !hi) { set_error("map_extent: null lo or hi"); return LV_ERR_ARG; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    if (lv_status s = pglob_map_empty(h, "map_extent")) return s;
+    int launches = 0;
+    const lv_status s = pglob_occupancy(h, "map_extent", &launches);
+    h->prof.total_launches += launches;
+    if (s != LV_OK) return s;
+    for (int a = 0; a < 3; ++a) {
+        lo[a] = (double)voxel_low(h->map.grid, h->occ.lo[a]);
+        hi[a] = (double)voxel_low(h->map.grid, h->occ.hi[a] + 1);
+    }
+    return LV_OK;
+}
+
+namespace {
+/* PrelocSearch's evaluator on the device: one launch per call, the results read back (the schedule decides on the host) */
+struct DevicePrelocEval {
+    cudaStream_t st;
+    PrelocGlobalArgs a;
+    PrelocCell* d_cells;
+    int32_t* d_bounds;
+    PrelocBest* d_best;
+    cudaError_t err;
+    int launches;
+    void bounds(const PrelocCell* c, int64_t n, int32_t* out) {
+        if (err == cudaSuccess) err = cudaMemcpyAsync(d_cells, c, sizeof(PrelocCell) * (size_t)n, cudaMemcpyHostToDevice, st);
+        a.cells = d_cells;
+        a.count = n;
+        if (err == cudaSuccess) err = launch_preloc_bounds(a, st, &launches);
+        if (err == cudaSuccess) err = cudaMemcpyAsync(out, d_bounds, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, st);
+        if (err == cudaSuccess) err = cudaStreamSynchronize(st);
+        if (err != cudaSuccess) std::fill(out, out + n, -2);        /* below any score: the search winds down */
+    }
+    void exact(const PrelocCell* c, int64_t n, PrelocBest* out) {
+        if (err == cudaSuccess) err = cudaMemcpyAsync(d_cells, c, sizeof(PrelocCell) * (size_t)n, cudaMemcpyHostToDevice, st);
+        a.cells = d_cells;
+        a.count = n;
+        if (err == cudaSuccess) err = launch_preloc_exact(a, st, &launches);
+        if (err == cudaSuccess) err = cudaMemcpyAsync(out, d_best, sizeof(PrelocBest) * (size_t)n, cudaMemcpyDeviceToHost, st);
+        if (err == cudaSuccess) err = cudaStreamSynchronize(st);
+        if (err != cudaSuccess)
+            for (int64_t t = 0; t < n; ++t) { out[t].score = -1; out[t].pad_ = 0; out[t].tie = 0; out[t].idx = 0; }
+    }
+};
+}  // namespace
+
+lv_status lv_prelocalize_global(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p, lv_preloc_result* out,
+                                lv_preloc_stats* stats) {
+    if (!p || !out || !d_xyz_lidar) { set_error("prelocalize_global: null params, result or points"); return LV_ERR_ARG; }
+    if (n < 1 || n > 0x7fffffff) { set_error("prelocalize_global: n outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    int64_t I = 0, K = 0, count = 0;
+    if (const char* e = preloc_params_error(p, &I, &K, &count)) {
+        set_error(std::string("prelocalize_global: ") + e);
+        return LV_ERR_ARG;
+    }
+    if (count > LV_PRELOC_GLOBAL_MAX_CANDIDATES) {
+        set_error("prelocalize_global: " + std::to_string((long long)count) + " candidates, more than 2^40");
+        return LV_ERR_ARG;
+    }
+    if (2 * K + 1 > kPrelocMaxTopCells) {
+        set_error("prelocalize_global: " + std::to_string((long long)(2 * K + 1)) + " headings, more than 2^20");
+        return LV_ERR_ARG;
+    }
+    if (!h) { set_error("prelocalize_global: null handle"); return LV_ERR_ARG; }
+    if (h->map.empty) { set_error("prelocalize_global: the map is empty"); return LV_EMPTY_MAP; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    sync_mirror(h);                                               /* the base: what lv_get_state returns */
+    if (lv_status s = pglob_map_empty(h, "prelocalize_global")) return s;
+
+    int launches = 0;
+    {
+        const lv_status s = pglob_occupancy(h, "prelocalize_global", &launches);
+        h->prof.total_launches += launches;
+        if (s != LV_OK) return s;
+    }
+    const PrelocOcc occ = h->occ;
+    const int64_t H = 2 * K + 1;
+    const int32_t S = (int32_t)(n < p->max_points ? n : p->max_points);
+    double x0[LV_STATE_LEN];
+    memcpy(x0, h->x, sizeof(x0));
+    const PrelocAxes ax = preloc_axes(x0);
+    std::vector<float> frames((size_t)H * 12);
+    for (int64_t k = -K; k <= K; ++k) {
+        const Rt32 F = preloc_heading_frame(x0, ax, (double)k * (double)p->yaw_step);
+        memcpy(&frames[(size_t)(k + K) * 12], F.R, sizeof(float) * 9);
+        memcpy(&frames[(size_t)(k + K) * 12 + 9], F.t, sizeof(float) * 3);
+    }
+    /* scratch: frames, cells, bounds, best */
+    const size_t off_frames = 0, off_cells = pglob_align(off_frames + sizeof(float) * frames.size());
+    const size_t off_bounds = pglob_align(off_cells + sizeof(PrelocCell) * kPrelocChunk);
+    const size_t off_best = pglob_align(off_bounds + sizeof(int32_t) * kPrelocChunk);
+    if (lv_status s = pglob_reserve(h, off_best + sizeof(PrelocBest) * kPrelocChunk)) return s;
+    uint8_t* base = static_cast<uint8_t*>(h->d_pglob);
+    LV_CUDA(cudaMemcpyAsync(base + off_frames, frames.data(), sizeof(float) * frames.size(), cudaMemcpyHostToDevice, h->stream));
+
+    DevicePrelocEval ev;
+    ev.st = h->stream;
+    memset(&ev.a, 0, sizeof(ev.a));
+    ev.a.xyz = d_xyz_lidar;
+    ev.a.n = n;
+    ev.a.S = S;
+    ev.a.step = p->step;
+    ev.a.I = I;
+    ev.a.K = K;
+    ev.a.ax = ax;
+    ev.a.frames = reinterpret_cast<const float*>(base + off_frames);
+    ev.a.occ = occ;
+    ev.a.bounds = reinterpret_cast<int32_t*>(base + off_bounds);
+    ev.a.best = reinterpret_cast<PrelocBest*>(base + off_best);
+    ev.d_cells = reinterpret_cast<PrelocCell*>(base + off_cells);
+    ev.d_bounds = ev.a.bounds;
+    ev.d_best = ev.a.best;
+    ev.err = cudaSuccess;
+    ev.launches = 0;
+    const char* np = getenv("LV_PRELOC_NO_PRUNE");
+    PrelocSearch<DevicePrelocEval> search(ev, I, K, S, !(np && np[0] == '1'));
+    try {
+        search.run();
+    } catch (const std::bad_alloc&) {                             /* the cell lists are host vectors */
+        h->prof.total_launches += ev.launches;
+        set_error("prelocalize_global: out of host memory for the cell lists");
+        return LV_ERR_CAPACITY;
+    }
+    h->prof.total_launches += ev.launches;
+    LV_CUDA(ev.err);
+
+    const int64_t W = 2 * I + 1, P = W * W, idx = search.best.idx;
+    const int64_t hk = idx / P, q = idx % P;
+    memset(out, 0, sizeof(*out));
+    out->candidates = count;
+    out->index = idx;
+    out->k = (int32_t)(hk - K);
+    out->i = (int32_t)(q / W - I);
+    out->j = (int32_t)(q % W - I);
+    out->score = search.best.score;
+    out->points = S;
+    preloc_candidate(x0, ax, (double)out->k * (double)p->yaw_step, (double)out->i * (double)p->step, (double)out->j * (double)p->step,
+                     out->x);
+    if (stats) {
+        memset(stats, 0, sizeof(*stats));
+        stats->candidates = search.st.candidates;
+        stats->cells_bounded = search.st.cells_bounded;
+        stats->candidates_scored = search.st.candidates_scored;
+        stats->probes = search.st.probes;
+        stats->launches = search.st.launches;
+    }
     memcpy(h->x, out->x, sizeof(h->x));                           /* lv_set_state(out->x, NULL) */
     h->state_dirty = true;
     return LV_OK;

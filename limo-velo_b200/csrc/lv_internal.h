@@ -9,6 +9,7 @@
 
 #include "../../include/limovelo_b200.h"
 #include "lv_ieskf.h"
+#include "lv_preloc_bound.h"
 #include "lv_voxel_search.h"
 
 namespace lv {
@@ -299,6 +300,30 @@ struct PrelocArgs {
     unsigned long long* best;  /* the largest selection key (preloc_key); 0 before the launch             */
 };
 cudaError_t launch_preloc(const PrelocArgs& a, cudaStream_t st, int* launches);
+
+/* lv_preloc_global.cu: the occupancy summary, the cell bounds and the exact cell scores of lv_prelocalize_global
+ * (arithmetic and schedule: lv_preloc_bound.h) */
+enum { kPrelocGlobalThreads = 256 };
+struct PrelocGlobalArgs {
+    const float* xyz;          /* the sweep, n x 3, LiDAR frame (device)                                  */
+    int64_t n;
+    int32_t S;                 /* scored points: xyz[floor(s n / S)]                                       */
+    float step;                /* position grid step (m)                                                   */
+    int64_t I, K;              /* half-widths of the position and heading grids                           */
+    PrelocAxes ax;             /* u, v: the position offsets are computed in the kernel (preloc_offset)  */
+    const float* frames;       /* (2K + 1) x 12: lidar_to_world R (row-major) and t of each heading       */
+    PrelocOcc occ;
+    const PrelocCell* cells;   /* the cells of one launch                                                 */
+    int64_t count;
+    int32_t* bounds;           /* bound launch: the bound of each cell                                    */
+    PrelocBest* best;          /* exact launch: the best candidate of each cell                           */
+};
+/* ext: 6 words, lo (x, y, z) then hi; set to 0xFFFFFFFF / 0 before the launch */
+cudaError_t launch_occ_extent(const VoxelMapView& m, uint32_t bslots, uint32_t* ext, cudaStream_t st, int* launches);
+/* o.bits zeroed before the launch; o.lo / o.hi, the levels and offsets from occ_layout */
+cudaError_t launch_occ_bits(const PrelocOcc& o, uint32_t bslots, uint32_t* bits, cudaStream_t st, int* launches);
+cudaError_t launch_preloc_bounds(const PrelocGlobalArgs& a, cudaStream_t st, int* launches);
+cudaError_t launch_preloc_exact(const PrelocGlobalArgs& a, cudaStream_t st, int* launches);
 
 }  // namespace lv
 #endif
