@@ -7,8 +7,11 @@
  * the very code the kernels run against the oracle, in a container without a GPU.
  *
  * It is NOT part of the product, is not linked into liblimovelo_b200.so and is not reachable from
- * the C ABI; the product has no CPU path.  The map is built and updated by the product's own per-item functions
+ * the C ABI; the product has no CPU path.  The map is built, updated and grown by the product's own per-item functions
  * (lv_voxel_map.h), called from plain host loops in the order lv_map.cu launches its kernels.
+ *
+ * liblv_cpushim.so is this file, lidar_ring.cpp (the LiDAR buffer) and preloc.cpp (the start-pose searches); tests/shim_binding.py
+ * loads it.
  */
 #include <stdint.h>
 #include <string.h>
@@ -66,21 +69,27 @@ static void shim_add_impl(ShimMap* sm, const float* xyz, int64_t n, int downsamp
     sm->n_inserted += (uint32_t)n;
 }
 
-/* cap: map points the tables are sized for (at least m): 8 table slots and 64 arena entries per point */
+/* empty tables and a zeroed arena for `cap` map points: 8 table slots and 64 arena entries per point; returns the slots */
+static uint32_t alloc_tables(int64_t cap, std::vector<uint4>& table, std::vector<uint4>& btable, std::vector<float4>& arena) {
+    uint32_t slots = 1u << 14;
+    while (slots < 8 * (uint64_t)(cap + 65536)) slots <<= 1;
+    uint4 empty; empty.x = empty.y = 0xFFFFFFFFu; empty.z = empty.w = 0;
+    uint4 zero; zero.x = zero.y = zero.z = zero.w = 0;
+    table.assign(2 * (size_t)slots, zero);
+    for (uint32_t s = 0; s < slots; ++s) table[2 * (size_t)s] = empty;
+    btable.assign(slots / 4, empty);
+    arena.assign((size_t)64 * (size_t)(cap + 65536) + (1u << 20), float4{});
+    return slots;
+}
+
+/* cap: map points the tables are sized for (at least m) */
 ShimMap* shim_map_create_cap(const float* xyz, int64_t m, int64_t cap, float cell) {
     ShimMap* sm = new ShimMap();
     const float ds = 0.2f;
     int k = (int)floor((double)cell / (double)ds + 0.5);
     k = k < 1 ? 1 : (k > kMaxCellsPerVoxel ? kMaxCellsPerVoxel : k);
     if (cap < m) cap = m;
-    uint32_t slots = 1u << 14;
-    while (slots < 8 * (uint64_t)(cap + 65536)) slots <<= 1;
-    uint4 empty; empty.x = empty.y = 0xFFFFFFFFu; empty.z = empty.w = 0;
-    uint4 zero; zero.x = zero.y = zero.z = zero.w = 0;
-    sm->table.assign(2 * (size_t)slots, zero);
-    for (uint32_t s = 0; s < slots; ++s) sm->table[2 * (size_t)s] = empty;
-    sm->btable.assign(slots / 4, empty);
-    sm->arena.resize((size_t)64 * (size_t)(cap + 65536) + (1u << 20));
+    const uint32_t slots = alloc_tables(cap, sm->table, sm->btable, sm->arena);
     sm->counters.assign(kMapCounters, 0u);
     sm->counters[kCtrArenaTop] = 16u;
     sm->touched.resize(slots);
@@ -163,6 +172,33 @@ void shim_map_dump(const ShimMap* sm, uint32_t* table, uint32_t* btable, float* 
     memcpy(touched, sm->touched.data(), sizeof(uint32_t) * std::min(sm->counters[kCtrTouched], sm->rw.list_cap));
     memcpy(dirty, sm->dirty.data(), sizeof(uint32_t) * std::min(sm->counters[kCtrDirty], sm->rw.list_cap));
 }
+/* lv_map.cu's map_grow: fresh tables for `cap` points, every old slot re-inserted by the product's voxel_rehash_item /
+ * block_rehash_item (the functions the rehash kernel runs), the used prefix of the arena copied with its indices unchanged */
+void shim_map_grow(ShimMap* sm, int64_t cap) {
+    std::vector<uint4> table, btable;
+    std::vector<float4> arena;
+    const uint32_t slots = alloc_tables(cap, table, btable, arena);
+    if (arena.size() < sm->arena.size()) arena.resize(sm->arena.size());
+    const uint32_t top = std::min<uint32_t>(sm->counters[kCtrArenaTop], (uint32_t)sm->arena.size());
+    std::copy(sm->arena.begin(), sm->arena.begin() + top, arena.begin());
+    VoxelMapRW r = sm->rw;
+    r.table = table.data(); r.mask = slots - 1; r.btable = btable.data(); r.bmask = slots / 4 - 1;
+    r.arena = arena.data(); r.arena_cap = (uint32_t)arena.size();
+    sm->counters[kCtrSlotsUsed] = 0;
+    sm->counters[kCtrBlocksUsed] = 0;
+    for (uint32_t s = 0; s <= sm->rw.mask; ++s) voxel_rehash_item(r, sm->table.data(), s);
+    for (uint32_t s = 0; s <= sm->rw.bmask; ++s) block_rehash_item(r, sm->btable.data(), s);
+    sm->table.swap(table);              /* the buffers move with the swap: r's pointers stay valid */
+    sm->btable.swap(btable);
+    sm->arena.swap(arena);
+    sm->touched.assign(slots, 0u);
+    sm->dirty.assign(slots, 0u);
+    r.touched = sm->touched.data(); r.dirty = sm->dirty.data(); r.list_cap = slots;
+    sm->rw = r;
+    sm->view = map_view_of(r);
+}
+/* one device counter of the map (lv_voxel_map.h kCtr*) */
+uint32_t shim_map_counter(const ShimMap* sm, int k) { return sm->counters[k]; }
 void shim_map_destroy(ShimMap* m) { delete m; }
 
 static void search_setup(const ShimParams* p, float cell, float* max_d2, double* gate, int* max_ring) {

@@ -8,7 +8,7 @@
 
 Nothing is fixed.  Of m points whose time equals t2 exactly only min(m, 2) are returned, and on unsorted content the result
 depends on the binary search's exact probe sequence.  This is the oracle of the device buffer (lv_lidar_*), of its host build
-(tests/cpu_shim_buffer) and of the windowed tick tests.  Points are (time, x, y, z) tuples; x, y, z are float32 values.
+(tests/cpu_shim/lidar_ring.cpp) and of the windowed tick tests.  Points are (time, x, y, z) tuples; x, y, z are float32 values.
 """
 import collections
 

@@ -1,4 +1,4 @@
-"""lv_prelocalize_global's cell bound restated in numpy, and the binding of its host build (tests/cpu_shim_preloc_global).
+"""lv_prelocalize_global's cell bound restated in numpy, and calls into its host build (tests/cpu_shim/preloc.cpp).
 
 The restatement takes the voxel code of tests/preloc_ref.py: for each cell it forms every scored point's world point at the
 cell's four corner candidates (the offsets a u + b v in fp64, rounded to fp32, fadd(F.t, o), fadd(row, t)), takes the
@@ -6,12 +6,11 @@ per-axis minimum and maximum of their voxel coordinates as the point's voxel box
 occupied voxel, exactly (a summed-volume table over the occupied voxels).  It does not use the header's route (the corner
 offsets' range first, then one fadd per end), so equal results also say that the route is monotone as DESIGN.md §5e argues."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 import preloc_ref as R
+import shim_binding
 
 f32 = np.float32
 
@@ -95,24 +94,6 @@ class Scene:
 
 
 # ---- the host build of csrc/lv_preloc_bound.h -------------------------------------------------------------------------------
-_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "cpu_shim_preloc_global")
-_slib = None
-
-
-def shim():
-    global _slib
-    if _slib is None:
-        subprocess.check_call(["make", "-s", "-C", _DIR])
-        L = C.CDLL(os.path.join(_DIR, "liblv_cpushim_preloc_global.so"))
-        dp, fp, i64, f, i32p = C.POINTER(C.c_double), C.POINTER(C.c_float), C.c_int64, C.c_float, C.POINTER(C.c_int32)
-        L.shim_pg_bounds.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, i64, i64, i64, i32p, i64, i32p]
-        L.shim_pg_search.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, f, f, C.c_int32, C.c_int, C.POINTER(i64), C.POINTER(i64)]
-        L.shim_pg_extent.argtypes = [fp, i64, f, f, C.POINTER(C.c_uint32), i32p]
-        L.shim_pg_top_level.argtypes = [i64, i64]
-        _slib = L
-    return _slib
-
-
 def _fp(a):
     return a.ctypes.data_as(C.POINTER(C.c_float))
 
@@ -123,9 +104,10 @@ def host_bounds(x, xyz, map_xyz, ds, voxel_size, step, yaw_step, I, K, S, cells)
     mp = np.ascontiguousarray(map_xyz, np.float32)
     cells = np.ascontiguousarray(cells, np.int32).reshape(-1, 4)
     out = np.zeros(len(cells), np.int32)
-    st = shim().shim_pg_bounds(x.ctypes.data_as(C.POINTER(C.c_double)), _fp(xyz), len(xyz), _fp(mp), len(mp), ds, voxel_size, step,
-                               yaw_step, I, K, S, cells.ctypes.data_as(C.POINTER(C.c_int32)), len(cells),
-                               out.ctypes.data_as(C.POINTER(C.c_int32)))
+    L = shim_binding.lib()
+    st = L.shim_pg_bounds(x.ctypes.data_as(C.POINTER(C.c_double)), _fp(xyz), len(xyz), _fp(mp), len(mp), ds, voxel_size, step,
+                          yaw_step, I, K, S, cells.ctypes.data_as(C.POINTER(C.c_int32)), len(cells),
+                          out.ctypes.data_as(C.POINTER(C.c_int32)))
     assert st == 0
     return out
 
@@ -140,9 +122,10 @@ def host_search(x, xyz, map_xyz, ds, voxel_size, radius, step, yaw_range, yaw_st
     mp = np.ascontiguousarray(map_xyz, np.float32)
     best = np.zeros(3, np.int64)
     stats = np.zeros(5, np.int64)
-    st = shim().shim_pg_search(x.ctypes.data_as(C.POINTER(C.c_double)), _fp(xyz), len(xyz), _fp(mp), len(mp), ds, voxel_size, radius,
-                               step, yaw_range, yaw_step, max_points, int(prune), best.ctypes.data_as(C.POINTER(C.c_int64)),
-                               stats.ctypes.data_as(C.POINTER(C.c_int64)))
+    L = shim_binding.lib()
+    st = L.shim_pg_search(x.ctypes.data_as(C.POINTER(C.c_double)), _fp(xyz), len(xyz), _fp(mp), len(mp), ds, voxel_size, radius,
+                          step, yaw_range, yaw_step, max_points, int(prune), best.ctypes.data_as(C.POINTER(C.c_int64)),
+                          stats.ctypes.data_as(C.POINTER(C.c_int64)))
     assert st == 0
     return int(best[2]), int(best[0]), dict(zip(STATS, (int(s) for s in stats)))
 
@@ -152,6 +135,7 @@ def host_extent(map_xyz, ds, voxel_size):
     mp = np.ascontiguousarray(map_xyz, np.float32)
     ext = np.zeros(6, np.uint32)
     lev = np.zeros(2, np.int32)
-    assert shim().shim_pg_extent(_fp(mp), len(mp), ds, voxel_size, ext.ctypes.data_as(C.POINTER(C.c_uint32)),
-                                 lev.ctypes.data_as(C.POINTER(C.c_int32))) == 0
+    L = shim_binding.lib()
+    assert L.shim_pg_extent(_fp(mp), len(mp), ds, voxel_size, ext.ctypes.data_as(C.POINTER(C.c_uint32)),
+                            lev.ctypes.data_as(C.POINTER(C.c_int32))) == 0
     return ext[:3].astype(np.int64), ext[3:].astype(np.int64), (int(lev[0]), int(lev[1]))

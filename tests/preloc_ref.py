@@ -1,4 +1,4 @@
-"""lv_prelocalize restated in numpy, and the binding of its host build (tests/cpu_shim_preloc).
+"""lv_prelocalize restated in numpy, and calls into its host build (tests/cpu_shim/preloc.cpp).
 
 The restatement follows the definition in include/limovelo_b200.h, not the header's code: the rotation matrices from the
 quaternions in fp64 (Python floats, the products and sums in Eigen's toRotationMatrix order), cast to fp32 and composed in fp32
@@ -6,10 +6,10 @@ like State / RotTransl (make_frame's lidar_to_world), the world point w = fadd(d
 floor(floor(w / ds) / k) per axis, and occupancy as the set of voxels that hold a stored map point."""
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
+
+import shim_binding
 
 f32 = np.float32
 BIAS = 1 << 20
@@ -178,26 +178,6 @@ def at_face(w, ds):
 
 
 # ---- the host build of csrc/lv_preloc.h -------------------------------------------------------------------------------------
-_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "cpu_shim_preloc")
-_slib = None
-
-
-def shim():
-    global _slib
-    if _slib is None:
-        subprocess.check_call(["make", "-s", "-C", _DIR])
-        L = C.CDLL(os.path.join(_DIR, "liblv_cpushim_preloc.so"))
-        dp, fp, i64, f = C.POINTER(C.c_double), C.POINTER(C.c_float), C.c_int64, C.c_float
-        L.shim_preloc_scores.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, f, f, C.c_int32, C.POINTER(C.c_int32), fp, fp]
-        L.shim_preloc_scores.restype = i64
-        L.shim_preloc_candidate.argtypes = [dp, f, f, C.c_int32, C.c_int32, C.c_int32, dp]
-        L.shim_preloc_candidate.restype = None
-        L.shim_preloc_axes.argtypes = [dp, dp]
-        L.shim_preloc_axes.restype = None
-        _slib = L
-    return _slib
-
-
 def host_scores(x, xyz, map_xyz, ds, voxel_size, radius, step, yaw_range, yaw_step, max_points):
     """(scores, winner index, frames, offsets) of the host build"""
     I, K = grid(radius, step, yaw_range, yaw_step)
@@ -209,15 +189,16 @@ def host_scores(x, xyz, map_xyz, ds, voxel_size, radius, step, yaw_range, yaw_st
     frames = np.zeros((2 * K + 1, 12), np.float32)
     offs = np.zeros((W * W, 3), np.float32)
     fpt = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
-    best = shim().shim_preloc_scores(x.ctypes.data_as(C.POINTER(C.c_double)), fpt(xyz), len(xyz), fpt(mp), len(mp), ds, voxel_size,
-                                     radius, step, yaw_range, yaw_step, max_points, scores.ctypes.data_as(C.POINTER(C.c_int32)),
-                                     fpt(frames), fpt(offs))
+    L = shim_binding.lib()
+    best = L.shim_preloc_scores(x.ctypes.data_as(C.POINTER(C.c_double)), fpt(xyz), len(xyz), fpt(mp), len(mp), ds, voxel_size,
+                                radius, step, yaw_range, yaw_step, max_points, scores.ctypes.data_as(C.POINTER(C.c_int32)),
+                                fpt(frames), fpt(offs))
     return scores, int(best), frames, offs
 
 
 def host_candidate(x, step, yaw_step, k, i, j):
     x = np.ascontiguousarray(x, np.float64)
     out = np.zeros(26)
-    shim().shim_preloc_candidate(x.ctypes.data_as(C.POINTER(C.c_double)), step, yaw_step, k, i, j,
-                                 out.ctypes.data_as(C.POINTER(C.c_double)))
+    shim_binding.lib().shim_preloc_candidate(x.ctypes.data_as(C.POINTER(C.c_double)), step, yaw_step, k, i, j,
+                                             out.ctypes.data_as(C.POINTER(C.c_double)))
     return out

@@ -1,4 +1,5 @@
-"""ctypes binding of tests/cpu_shim/liblv_cpushim.so (TEST-ONLY host build of the product headers)."""
+"""ctypes binding of tests/cpu_shim/liblv_cpushim.so (TEST-ONLY host build of the product headers): the map, search and
+filter (shim.cpp), the LiDAR buffer (lidar_ring.cpp) and the start-pose searches (preloc.cpp)."""
 import ctypes as C
 import os
 import subprocess
@@ -44,7 +45,38 @@ def lib():
         L.shim_map_check.argtypes = [C.c_void_p]
         L.shim_map_dims.argtypes = [C.c_void_p] * 3
         L.shim_map_dump.argtypes = [C.c_void_p] * 6
+        L.shim_map_grow.argtypes = [C.c_void_p, C.c_int64]
+        L.shim_map_grow.restype = None
+        L.shim_map_counter.argtypes = [C.c_void_p, C.c_int]
+        L.shim_map_counter.restype = C.c_uint32
         assert L.shim_sizeof_iterlog() == C.sizeof(IterLog)
+
+        vp, i64, f, dp, fp, i32p = C.c_void_p, C.c_int64, C.c_float, C.POINTER(C.c_double), C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        L.shim_lidar_create.restype = vp
+        L.shim_lidar_create.argtypes = [i64, C.c_int]
+        L.shim_lidar_destroy.argtypes = [vp]
+        L.shim_lidar_destroy.restype = None
+        L.shim_lidar_size.argtypes = [vp]
+        L.shim_lidar_size.restype = i64
+        L.shim_lidar_content.argtypes = [vp, dp]
+        L.shim_lidar_content.restype = None
+        L.shim_lidar_reserve.argtypes = [vp, i64, C.c_int]
+        L.shim_lidar_push.argtypes = [vp, fp, dp, fp, fp, i64]
+        L.shim_lidar_get.argtypes = [vp, C.c_double, C.c_double, fp, dp, fp, fp, i64]
+        L.shim_lidar_get.restype = i64
+        L.shim_lidar_clear.argtypes = [vp, C.c_double]
+        L.shim_lidar_clear.restype = None
+
+        L.shim_preloc_scores.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, f, f, C.c_int32, i32p, fp, fp]
+        L.shim_preloc_scores.restype = i64
+        L.shim_preloc_candidate.argtypes = [dp, f, f, C.c_int32, C.c_int32, C.c_int32, dp]
+        L.shim_preloc_candidate.restype = None
+        L.shim_preloc_axes.argtypes = [dp, dp]
+        L.shim_preloc_axes.restype = None
+        L.shim_pg_bounds.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, i64, i64, i64, i32p, i64, i32p]
+        L.shim_pg_search.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, f, f, C.c_int32, C.c_int, C.POINTER(i64), C.POINTER(i64)]
+        L.shim_pg_extent.argtypes = [fp, i64, f, f, C.POINTER(C.c_uint32), i32p]
+        L.shim_pg_top_level.argtypes = [i64, i64]
         _lib = L
     return _lib
 

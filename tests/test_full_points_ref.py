@@ -5,13 +5,11 @@
    the centroid, time 0, PCL's overflow pass-through of every attribute, the buffer's lanes, and the header stamp (rounding at .5 us,
    an empty cloud, a 1.7e9 s epoch).
 2. The host build of the device buffer's index arithmetic with attribute lanes (csrc/lv_lidar_buffer.h through
-   tests/cpu_shim_buffer_full) equals the restatement on seeded random push / get / clear / reserve sequences: full and plain pushes,
+   tests/cpu_shim/lidar_ring.cpp) equals the restatement on seeded random push / get / clear / reserve sequences: full and plain pushes,
    rings that gain lanes with points already live, re-reserves, wraps, ties and windows above n_max.
 """
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,6 +17,7 @@ import pytest
 import frontend_ref as F
 import full_points_ref as P
 import lidar_buffer_ref as R
+import shim_binding as S
 
 f32 = np.float32
 
@@ -125,32 +124,6 @@ def test_buffer_carries_the_lanes_with_the_window():
 
 
 # ---- the host build of csrc/lv_lidar_buffer.h with lanes ---------------------------------------------------------------------------
-_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "cpu_shim_buffer_full")
-_slib = None
-
-
-def shim():
-    global _slib
-    if _slib is None:
-        subprocess.check_call(["make", "-s", "-C", _DIR])
-        L = C.CDLL(os.path.join(_DIR, "liblv_cpushim_buffer_full.so"))
-        vp, i64, dp, fp = C.c_void_p, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_float)
-        L.shim_full_create.restype = vp
-        L.shim_full_create.argtypes = [i64, C.c_int]
-        L.shim_full_destroy.argtypes = [vp]
-        L.shim_full_destroy.restype = None
-        L.shim_full_size.argtypes = [vp]
-        L.shim_full_size.restype = i64
-        L.shim_full_reserve.argtypes = [vp, i64, C.c_int]
-        L.shim_full_push.argtypes = [vp, fp, dp, fp, fp, i64]
-        L.shim_full_get.argtypes = [vp, C.c_double, C.c_double, fp, dp, fp, fp, i64]
-        L.shim_full_get.restype = i64
-        L.shim_full_clear.argtypes = [vp, C.c_double]
-        L.shim_full_clear.restype = None
-        _slib = L
-    return _slib
-
-
 def _fp(a):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_float))
 
@@ -161,13 +134,13 @@ def _dp(a):
 
 def test_host_build_with_lanes_equals_the_restatement():
     from test_lidar_buffer_ref import pick_time, random_message
-    L = shim()
+    L = S.lib()
     rng = np.random.default_rng(20261016)
     seen = dict(gets=0, nonempty=0, plain=0, full=0, gained=0, resized=0, over=0, refused=0, wrapped=0)
     for seq in range(3000):
         cap = int(rng.integers(1, 40))
         lanes = bool(rng.random() < 0.7)
-        ring = L.shim_full_create(cap, int(lanes))
+        ring = L.shim_lidar_create(cap, int(lanes))
         ref = P.LidarBufferFull()
         clock, pushed = 0.0, 0
         for _ in range(int(rng.integers(1, 14))):
@@ -178,7 +151,7 @@ def test_host_build_with_lanes_equals_the_restatement():
                 full = lanes and rng.random() < 0.75
                 inten = rng.uniform(0, 255, n).astype(f32) if full else None
                 rg = rng.uniform(0, 100, n).astype(f32) if full else None
-                ok = L.shim_full_push(ring, _fp(xyz), _dp(t), _fp(inten), _fp(rg), n)
+                ok = L.shim_lidar_push(ring, _fp(xyz), _dp(t), _fp(inten), _fp(rg), n)
                 fits = ref.size() + n <= cap
                 assert ok == int(fits), seq
                 if fits:
@@ -188,7 +161,7 @@ def test_host_build_with_lanes_equals_the_restatement():
             elif op < 0.55:
                 new_cap = int(rng.integers(1, 45))
                 add = bool(rng.random() < 0.5)
-                ok = L.shim_full_reserve(ring, new_cap, int(add))
+                ok = L.shim_lidar_reserve(ring, new_cap, int(add))
                 assert ok == int(ref.size() <= new_cap), seq
                 if ok:
                     seen["gained"] += add and not lanes and ref.size() > 0
@@ -203,7 +176,7 @@ def test_host_build_with_lanes_equals_the_restatement():
                 n_max = int(rng.integers(1, cap + 2))
                 ox, ot = np.full((cap, 3), np.nan, f32), np.full(cap, np.nan)
                 oi, orr = np.full(cap, np.nan, f32), np.full(cap, np.nan, f32)
-                m = L.shim_full_get(ring, t1, t2, _fp(ox), _dp(ot), _fp(oi), _fp(orr), n_max)
+                m = L.shim_lidar_get(ring, t1, t2, _fp(ox), _dp(ot), _fp(oi), _fp(orr), n_max)
                 rx, rt, ri, rr = ref.get(t1, t2)
                 assert m == len(rt), (seq, t1, t2)
                 if m > n_max:
@@ -215,10 +188,10 @@ def test_host_build_with_lanes_equals_the_restatement():
                 seen["nonempty"] += m > 0
             else:
                 t = pick_time(rng, ref, clock)
-                L.shim_full_clear(ring, t)
+                L.shim_lidar_clear(ring, t)
                 ref.clear(t)
-            assert L.shim_full_size(ring) == ref.size(), seq
+            assert L.shim_lidar_size(ring) == ref.size(), seq
         seen["wrapped"] += pushed > cap
-        L.shim_full_destroy(ring)
+        L.shim_lidar_destroy(ring)
     for k, v in seen.items():
         assert v >= 100, seen

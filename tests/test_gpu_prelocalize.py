@@ -1,4 +1,4 @@
-"""lv_prelocalize and PCD maps on the GPU: device scores bit for bit against the host build (tests/cpu_shim_preloc), the winner
+"""lv_prelocalize and PCD maps on the GPU: device scores bit for bit against the host build (tests/cpu_shim/preloc.cpp), the winner
 under the tie rule, the base candidate against lv_match_all, the strided subset, growth, the empty map, the effect on the filter;
 finding the start pose from metres and tens of degrees off; and a sequence saved to PCD and resumed in a second handle."""
 import math

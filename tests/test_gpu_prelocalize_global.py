@@ -1,5 +1,5 @@
 """lv_prelocalize_global on the GPU: the same result as lv_prelocalize wherever that runs (field for field, x bit for bit, P
-untouched), counts equal to the host build's (tests/cpu_shim_preloc_global), the tie rule on a map where most candidates score
+untouched), counts equal to the host build's (tests/cpu_shim/preloc.cpp), the tie rule on a map where most candidates score
 alike, the pruned search equal to the exhaustive one (LV_PRELOC_NO_PRUNE=1) above lv_prelocalize's cap, the empty and the
 grown map, lv_map_extent, and the start pose found anywhere on a 1 M-point map from a whole-map window."""
 import math

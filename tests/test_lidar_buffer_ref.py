@@ -3,19 +3,18 @@
 1. tests/lidar_buffer_ref.py (the literal restatement of Buffer / Accumulator::get) on cases worked by hand from the reference's
    text: include/Headers/Utils.hpp:9-23 (binary_search), include/Headers/Accumulator.hpp:61-74 (get), src/Objects/Buffer.cpp:26-28,
    66-70 (push, clear).  content is written newest first, as the deque holds it.
-2. The host build of the device buffer's index arithmetic (csrc/lv_lidar_buffer.h through tests/cpu_shim_buffer) equals the
-   restatement on 10^4 seeded random push / get / clear sequences: small rings that wrap many times, full rings, late and
-   overlapping messages, ties, NaN point times and windows above n_max.
+2. The host build of the device buffer's index arithmetic (csrc/lv_lidar_buffer.h through tests/cpu_shim/lidar_ring.cpp, a ring
+   without lanes) equals the restatement on 10^4 seeded random push / get / clear sequences: small rings that wrap many times,
+   full rings, late and overlapping messages, ties, NaN point times and windows above n_max.
 """
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import lidar_buffer_ref as R
+import shim_binding as S
 
 
 def buf_with(content):
@@ -125,34 +124,7 @@ def test_clear_stops_at_the_first_newer_point_in_insertion_order():
     assert b.size() == 2 and math.isnan(b.times()[1])
 
 
-# ---- the host build of csrc/lv_lidar_buffer.h -----------------------------------------------------------------------------------
-_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "cpu_shim_buffer")
-_slib = None
-
-
-def shim():
-    global _slib
-    if _slib is None:
-        subprocess.check_call(["make", "-s", "-C", _DIR])
-        L = C.CDLL(os.path.join(_DIR, "liblv_cpushim_buffer.so"))
-        vp, i64, dp = C.c_void_p, C.c_int64, C.POINTER(C.c_double)
-        L.shim_lidar_create.restype = vp
-        L.shim_lidar_create.argtypes = [i64]
-        L.shim_lidar_destroy.argtypes = [vp]
-        L.shim_lidar_destroy.restype = None
-        L.shim_lidar_size.argtypes = [vp]
-        L.shim_lidar_size.restype = i64
-        L.shim_lidar_content.argtypes = [vp, dp]
-        L.shim_lidar_content.restype = None
-        L.shim_lidar_push.argtypes = [vp, C.POINTER(C.c_float), dp, i64]
-        L.shim_lidar_get.argtypes = [vp, C.c_double, C.c_double, C.POINTER(C.c_float), dp, i64]
-        L.shim_lidar_get.restype = i64
-        L.shim_lidar_clear.argtypes = [vp, C.c_double]
-        L.shim_lidar_clear.restype = None
-        _slib = L
-    return _slib
-
-
+# ---- the host build of csrc/lv_lidar_buffer.h: a ring without lanes, pushed and read with NULL lanes ---------------------------
 def _fp(a):
     return a.ctypes.data_as(C.POINTER(C.c_float))
 
@@ -190,19 +162,19 @@ def pick_time(rng, ref, clock):
 
 
 def test_host_build_equals_the_restatement():
-    L = shim()
+    L = S.lib()
     rng = np.random.default_rng(20261015)
     checked = dict(gets=0, nonempty=0, unsorted=0, full=0, over=0, wrapped=0, cleared=0)
     for seq in range(10_000):
         cap = int(rng.integers(1, 40))
-        ring = L.shim_lidar_create(cap)
+        ring = L.shim_lidar_create(cap, 0)
         ref = R.LidarBuffer()
         clock, pushed = 0.0, 0
         for _ in range(int(rng.integers(1, 14))):
             op = rng.random()
             if op < 0.45:
                 xyz, t, clock = random_message(rng, clock)
-                ok = L.shim_lidar_push(ring, _fp(xyz), _dp(t), len(t))
+                ok = L.shim_lidar_push(ring, _fp(xyz), _dp(t), None, None, len(t))
                 fits = ref.size() + len(t) <= cap
                 assert ok == int(fits), seq
                 if fits:
@@ -216,7 +188,7 @@ def test_host_build_equals_the_restatement():
                     t1, t2 = t2, t1
                 n_max = int(rng.integers(1, cap + 2))
                 out_xyz, out_t = np.full((cap, 3), np.nan, np.float32), np.full(cap, np.nan)
-                m = L.shim_lidar_get(ring, t1, t2, _fp(out_xyz), _dp(out_t), n_max)
+                m = L.shim_lidar_get(ring, t1, t2, _fp(out_xyz), _dp(out_t), None, None, n_max)
                 rx, rt = ref.get(t1, t2)
                 assert m == len(rt), (seq, t1, t2)
                 if m > n_max:
@@ -245,17 +217,17 @@ def test_host_build_equals_the_restatement():
 
 @pytest.mark.parametrize("nan_at", [0, 2, 4])
 def test_nan_point_times_follow_the_comparisons(nan_at):
-    L = shim()
+    L = S.lib()
     t = np.array([1.0, 2.0, 3.0, 4.0, 5.0])
     t[nan_at] = np.nan
     xyz = np.arange(15, dtype=np.float32).reshape(5, 3)
-    ring = L.shim_lidar_create(8)
+    ring = L.shim_lidar_create(8, 0)
     ref = R.LidarBuffer()
-    assert L.shim_lidar_push(ring, _fp(xyz), _dp(t), 5) == 1
+    assert L.shim_lidar_push(ring, _fp(xyz), _dp(t), None, None, 5) == 1
     ref.push_message(xyz, t)
     for t1, t2 in [(0.0, 10.0), (2.0, 4.0), (3.0, 3.0), (0.0, 1.0)]:
         ox, ot = np.zeros((5, 3), np.float32), np.zeros(5)
-        m = L.shim_lidar_get(ring, t1, t2, _fp(ox), _dp(ot), 5)
+        m = L.shim_lidar_get(ring, t1, t2, _fp(ox), _dp(ot), None, None, 5)
         rx, rt = ref.get(t1, t2)
         assert m == len(rt) and bits(ox[:m]) == bits(rx) and bits(ot[:m]) == bits(rt), (t1, t2)
     L.shim_lidar_clear(ring, 10.0)

@@ -1,5 +1,4 @@
-"""Map growth on the host build of the product's per-item code — no GPU needed.  tests/cpu_shim_growth is the CPU shim
-(tests/cpu_shim) as it is, plus shim_map_grow.
+"""Map growth on the host build of the product's per-item code (tests/cpu_shim's shim_map_grow) — no GPU needed.
 
 A growth re-hashes every slot of the voxel and block tables into larger ones (voxel_rehash_item / block_rehash_item of
 lv_voxel_map.h, the functions lv_map.cu's rehash kernel runs) and copies the arena's used prefix, so every arena index
@@ -9,8 +8,6 @@ slot and block counts, and the same search, plane fit and Jacobian rows, bit for
 give the map a handle born at the larger capacity builds.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,50 +16,14 @@ import geometry as geo
 import shim_binding as S
 
 K_SLOTS_USED, K_BLOCKS_USED, K_ARENA_TOP = 5, 7, 0    # lv_voxel_map.h kCtr*
-_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "cpu_shim_growth")
-_glib = None
-
-
-def _lib():
-    """tests/cpu_shim_growth: the CPU shim as it is plus shim_map_grow, in a library of its own"""
-    global _glib
-    if _glib is None:
-        subprocess.check_call(["make", "-s", "-C", _DIR])
-        L = C.CDLL(os.path.join(_DIR, "liblv_cpushim_growth.so"))
-        L.shim_map_create_cap.restype = C.c_void_p
-        L.shim_map_create_cap.argtypes = [C.POINTER(C.c_float), C.c_int64, C.c_int64, C.c_float]
-        L.shim_map_destroy.argtypes = [C.c_void_p]
-        L.shim_map_add.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_int64, C.c_int]
-        L.shim_map_size.argtypes = [C.c_void_p]
-        L.shim_map_size.restype = C.c_int64
-        L.shim_map_error.argtypes = [C.c_void_p]
-        L.shim_map_error.restype = C.c_uint32
-        L.shim_map_points.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_int64]
-        L.shim_map_points.restype = C.c_int64
-        L.shim_map_check.argtypes = [C.c_void_p]
-        L.shim_map_grow.argtypes = [C.c_void_p, C.c_int64]
-        L.shim_map_grow.restype = None
-        L.shim_map_counter.argtypes = [C.c_void_p, C.c_int]
-        L.shim_map_counter.restype = C.c_uint32
-        _glib = L
-    return _glib
-
-
-class GrowMap(S.ShimMap):
-    """shim_binding.ShimMap on the growth library (the same shim code; maps of the two libraries never mix)"""
-
-    def __init__(self, xyz, cell=0.5, max_dist=2.0, capacity=0):
-        self.L = _lib()
-        xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
-        self.h = self.L.shim_map_create_cap(S._f(xyz), xyz.shape[0], int(capacity), C.c_float(cell))
 
 
 def grow(sm, cap):
-    _lib().shim_map_grow(C.c_void_p(sm.h), int(cap))
+    S.lib().shim_map_grow(C.c_void_p(sm.h), int(cap))
 
 
 def counter(sm, k):
-    return int(_lib().shim_map_counter(C.c_void_p(sm.h), k))
+    return int(S.lib().shim_map_counter(C.c_void_p(sm.h), k))
 
 
 @pytest.fixture(scope="module")
@@ -97,8 +58,8 @@ def _same_answers(a, b, sc, voxel, O):
 def test_growth_between_adds_keeps_the_map(O, geo_scenes, name):
     sc = geo_scenes[name]
     voxel = 0.4
-    ref = GrowMap(sc.build, voxel, geo.GATE, capacity=sc.capacity)             # never grown
-    sm = GrowMap(sc.build, voxel, geo.GATE, capacity=sc.capacity // 8)
+    ref = S.ShimMap(sc.build, voxel, geo.GATE, capacity=sc.capacity)             # never grown
+    sm = S.ShimMap(sc.build, voxel, geo.GATE, capacity=sc.capacity // 8)
     growths = 0
     # at least three growths: two after the build, one after every add (and a third after the build when there is no add);
     # the capacity rises geometrically from 1/8 of the scene's to the scene's
@@ -118,8 +79,8 @@ def test_growth_between_adds_keeps_the_map(O, geo_scenes, name):
 def test_adds_after_a_growth_equal_a_map_born_big(O, geo_scenes, name):
     sc = geo_scenes[name]
     voxel = 0.4
-    big = GrowMap(sc.build, voxel, geo.GATE, capacity=sc.capacity)
-    sm = GrowMap(sc.build, voxel, geo.GATE, capacity=sc.capacity // 8)
+    big = S.ShimMap(sc.build, voxel, geo.GATE, capacity=sc.capacity)
+    sm = S.ShimMap(sc.build, voxel, geo.GATE, capacity=sc.capacity // 8)
     grow(sm, sc.capacity // 4)
     grow(sm, sc.capacity)
     for a in sc.adds:
@@ -131,13 +92,13 @@ def test_adds_after_a_growth_equal_a_map_born_big(O, geo_scenes, name):
 
 def test_growth_of_an_empty_map_and_a_scattered_cloud(O):
     """an empty map grows to an empty map; a scattered cloud (27 slots per point) keeps every slot through two growths"""
-    sm = GrowMap(np.zeros((0, 3), np.float32), 0.4, geo.GATE, capacity=1000)
+    sm = S.ShimMap(np.zeros((0, 3), np.float32), 0.4, geo.GATE, capacity=1000)
     grow(sm, 4000)
     assert sm.size() == 0 and counter(sm, K_SLOTS_USED) == 0 and sm.error() == 0
     rng = np.random.default_rng(5)
     pts = rng.uniform(-300, 300, (20_000, 3)).astype(np.float32)
-    ref = GrowMap(pts[:10_000], 0.4, geo.GATE, capacity=16 * 20_000)
-    sm = GrowMap(pts[:10_000], 0.4, geo.GATE, capacity=2 * 20_000)
+    ref = S.ShimMap(pts[:10_000], 0.4, geo.GATE, capacity=16 * 20_000)
+    sm = S.ShimMap(pts[:10_000], 0.4, geo.GATE, capacity=2 * 20_000)
     grow(sm, 8 * 20_000)
     ref.add(pts[10_000:], downsample=True)
     sm.add(pts[10_000:], downsample=True)

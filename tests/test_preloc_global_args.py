@@ -71,8 +71,8 @@ def test_prelocalize_global_refusals(lv, L):
 
 def test_top_level_is_bounded():
     """the top level of the cells returns for every window, also with more headings than the top-level cell budget"""
-    import preloc_bound_ref as B
-    S = B.shim()
+    import shim_binding
+    S = shim_binding.lib()
     assert S.shim_pg_top_level(50, 100) == 5
     assert S.shim_pg_top_level(0, 600000) == 1               # 1 200 001 headings: one cell of one position each
     assert S.shim_pg_top_level(0, 0) == 1

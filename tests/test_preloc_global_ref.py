@@ -1,5 +1,5 @@
-"""The host build of lv_prelocalize_global (csrc/lv_preloc_bound.h, tests/cpu_shim_preloc_global) against the numpy
-restatement of tests/preloc_bound_ref.py and the brute force of tests/cpu_shim_preloc: the cell bound is at least every exact
+"""The host build of lv_prelocalize_global (csrc/lv_preloc_bound.h, tests/cpu_shim/preloc.cpp) against the numpy
+restatement of tests/preloc_bound_ref.py and the brute force of lv_prelocalize's host build: the cell bound is at least every exact
 score in the cell and equals it on single candidates, the pruned search returns the brute force's winner under the tie rule,
 and on a whole-map window the bound prunes most of the candidates.  No GPU."""
 import math

@@ -1,4 +1,4 @@
-"""The host build of lv_prelocalize's arithmetic (csrc/lv_preloc.h, tests/cpu_shim_preloc) against the numpy restatement of
+"""The host build of lv_prelocalize's arithmetic (csrc/lv_preloc.h, tests/cpu_shim/preloc.cpp) against the numpy restatement of
 tests/preloc_ref.py: heading frames and offsets bit for bit, every candidate's score, the winner under the tie rule and the
 winner's state.  A score may differ only by points that lie within an ulp of a cell face (listed when any occur).  No GPU."""
 import math
@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import preloc_ref as R
+import shim_binding
 
 FAR = np.array([2e5, -3e5, 50.0])
 
@@ -83,7 +84,7 @@ def test_axes(lv, O):
     x[23:26] = [0.3, -0.2, -9.8]
     g, u, v = R.axes(x)
     out = np.zeros(9)
-    R.shim().shim_preloc_axes(x.ctypes.data_as(R.C.POINTER(R.C.c_double)), out.ctypes.data_as(R.C.POINTER(R.C.c_double)))
+    shim_binding.lib().shim_preloc_axes(x.ctypes.data_as(R.C.POINTER(R.C.c_double)), out.ctypes.data_as(R.C.POINTER(R.C.c_double)))
     assert out.tobytes() == np.array(g + u + v).tobytes()
     assert abs(np.dot(g, u)) < 1e-15 and abs(np.dot(u, v)) < 1e-15 and abs(np.linalg.norm(v) - 1) < 1e-15
     x[23:26] = [-9.8, 0.1, 0.0]                     # |g_x| > 0.9: u starts from the y axis
