@@ -13,6 +13,7 @@
 #include <string.h>
 
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/limovelo_b200.h"
@@ -56,23 +57,24 @@ struct lv_context {
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     MapBuffers map;
-    float* d_sweep = nullptr;          /* max_points x 3 */
-    UpdateCtrl* d_ctrl = nullptr;
-    UpdateCtrl* h_ctrl = nullptr;      /* pinned mirror for the D2H of results */
-    double* d_partials = nullptr;
-    double* d_group_rows = nullptr;    /* partials pre-reduced in groups of kPartialGroup rows (fit kernel) */
-    uint32_t* d_group_tickets = nullptr;
-    int4* d_nn_a = nullptr;            /* max_points: K1 -> K2 hand-over */
-    int2* d_nn_b = nullptr;
-    uint32_t* d_hard_list = nullptr;   /* kHardBuckets segments of hard_segment(max_points) entries, then kCounters counters */
-    float4* d_ref = nullptr;           /* max_points: reuse reference (lv_reuse_kernel) */
-    uint32_t* d_redo = nullptr;        /* max_points */
-    double* d_imu = nullptr;           /* kImuBatch x 7: lv_propagate_device */
-    double* h_imu = nullptr;           /* pinned */
+    /* reserved once, by create_buffers (as are d_job and d_async): the update graphs bake these pointers into their nodes */
+    DeviceBuf<float> d_sweep;          /* max_points x 3 */
+    DeviceBuf<UpdateCtrl> d_ctrl;
+    PinnedBuf<UpdateCtrl> h_ctrl;      /* mirror for the D2H of results */
+    DeviceBuf<double> d_partials;
+    DeviceBuf<double> d_group_rows;    /* partials pre-reduced in groups of kPartialGroup rows (fit kernel) */
+    DeviceBuf<uint32_t> d_group_tickets;
+    DeviceBuf<int4> d_nn_a;            /* max_points: K1 -> K2 hand-over */
+    DeviceBuf<int2> d_nn_b;
+    DeviceBuf<uint32_t> d_hard_list;   /* kHardBuckets segments of hard_segment(max_points) entries, then kCounters counters */
+    DeviceBuf<float4> d_ref;           /* max_points: reuse reference (lv_reuse_kernel) */
+    DeviceBuf<uint32_t> d_redo;        /* max_points */
+    DeviceBuf<double> d_imu;           /* kImuBatch x 7: lv_propagate_device (lazily allocated) */
+    PinnedBuf<double> h_imu;
     /* recorded after the last H2D copy out of h_imu / h_ctrl: the calls return before those copies run (they queue behind
      * the update), so the next refill of the pinned buffer waits for this event, not for the whole stream */
-    cudaEvent_t imu_copied = nullptr;
-    cudaEvent_t ctrl_copied = nullptr;
+    Event imu_copied;
+    Event ctrl_copied;
     /* the sweep of the last update (correct_enqueue), for lv_map_add_last_sweep and lv_sweep_to_world_device_async */
     struct TickSweep {
         const float* xyz = nullptr;    /* device pointer */
@@ -81,45 +83,40 @@ struct lv_context {
         int64_t min_points = 0;        /* ... and its MAX_POINTS2MATCH gate */
     } tick;
     /* the async tick: deferred errors and the time of the last update that ran (lv_correct_device_async) */
-    AsyncWords* d_async = nullptr;
-    AsyncWords* h_async = nullptr;     /* pinned */
+    DeviceBuf<AsyncWords> d_async;
+    PinnedBuf<AsyncWords> h_async;
     bool time_pending = false;         /* last_time_updated waits for the device's decision (next fetch) */
     bool map_unknown = false;          /* an async add may have left the map without points: the device checks it */
-    cudaEvent_t path_copied = nullptr; /* the last H2D copy out of h_path (lv_compensate_device_async returns before it runs) */
+    Event path_copied;                 /* the last H2D copy out of h_path (lv_compensate_device_async returns before it runs) */
     LidarRing lidar;                   /* Accumulator::BUFFER_L (lv_lidar_reserve) */
     bool use_reuse = true;
     bool use_pdl = true;               /* programmatic dependent launch between the kernels of an update */
     /* Compensator (deskew) staging: lazily allocated */
-    lv_state32* d_path = nullptr;      /* deskew_max_states() */
-    lv_state32* h_path = nullptr;      /* pinned */
-    double* d_times = nullptr;         /* max_points */
-    float* d_deskew_in = nullptr;      /* max_points x 3 */
-    int* d_bad = nullptr;
-    int* h_bad = nullptr;              /* pinned */
+    DeviceBuf<lv_state32> d_path;      /* deskew_max_states() */
+    PinnedBuf<lv_state32> h_path;
+    DeviceBuf<double> d_times;         /* max_points */
+    DeviceBuf<float> d_deskew_in;      /* max_points x 3 */
+    DeviceBuf<int> d_bad;
+    PinnedBuf<int> h_bad;
     DownsampleScratch ds;              /* downsamplers: grows with the largest cloud seen */
-    float* d_ds_in = nullptr;          /* staging for the host-buffer variants */
-    float* d_ds_out = nullptr;
-    int64_t ds_stage_cap = 0;
-    uint8_t* d_ds_lanes = nullptr;     /* attribute staging of lv_voxelgrid_downsample_full: 28 B per point (ds_stage_lanes) */
-    int64_t ds_lanes_cap = 0;
-    double* d_reduced = nullptr;       /* 157 doubles */
-    double* h_reduced = nullptr;       /* pinned */
-    void* d_flush = nullptr;
+    DeviceBuf<float> d_ds_in;          /* staging for the host-buffer variants (ds_stage) */
+    DeviceBuf<float> d_ds_out;
+    DeviceBuf<uint8_t> d_ds_lanes;     /* attribute staging of lv_voxelgrid_downsample_full: 28 B per point */
+    DeviceBuf<double> d_reduced;       /* 157 doubles */
+    PinnedBuf<double> h_reduced;
+    DeviceBuf<uint8_t> d_flush;
     /* per-point debug outputs (lazily allocated, max_points) */
-    uint8_t* d_valid = nullptr; int32_t* d_nn_idx = nullptr; float* d_nn_sqd = nullptr;
-    float* d_plane = nullptr; float* d_dist = nullptr; float* d_gworld = nullptr; double* d_rows = nullptr;
+    DeviceBuf<uint8_t> d_valid; DeviceBuf<int32_t> d_nn_idx; DeviceBuf<float> d_nn_sqd;
+    DeviceBuf<float> d_plane; DeviceBuf<float> d_dist; DeviceBuf<float> d_gworld; DeviceBuf<double> d_rows;
     /* lv_prelocalize: winner key, heading frames, position offsets, scores (lazily allocated, grows) */
-    void* d_preloc = nullptr;
-    size_t preloc_bytes = 0;
+    DeviceBuf<uint8_t> d_preloc;
     /* lv_prelocalize_global / lv_map_extent: extent, heading frames, cell lists and results, occupancy bitmaps (grows) */
-    void* d_pglob = nullptr;
-    size_t pglob_bytes = 0;
+    DeviceBuf<uint8_t> d_pglob;
     /* the occupancy summary (extent, bitmap pyramid) of the map as of map_gen occ_gen; rebuilt when the map changed since */
     uint64_t map_gen = 0;              /* bumped by every add, build and growth (map_enqueue, map_grow_to) */
     uint64_t occ_gen = ~0ull;
     PrelocOcc occ;
-    uint32_t* d_occ = nullptr;         /* extent (8 words), then the bitmaps */
-    size_t occ_bytes = 0;
+    DeviceBuf<uint32_t> d_occ;         /* extent (8 words), then the bitmaps */
     /* host mirror of the filter (get_x / get_P) */
     double x[LV_STATE_LEN];
     double P[LV_DOF * LV_DOF];
@@ -134,7 +131,7 @@ struct lv_context {
     std::vector<EventPair> pending;
     std::vector<EventPair> pool;
     lv_profile prof;
-    int32_t* h_nevals = nullptr;       /* pinned ring: n_evals of profiled updates */
+    PinnedBuf<int32_t> h_nevals;       /* ring: n_evals of profiled updates */
     uint32_t update_seq = 0;
     IeskfParams iprm;
     /* one update = begin + (MAX_NUM_ITERS + 1) x (search, search-upper, fit, step): replayed as a CUDA graph
@@ -146,7 +143,7 @@ struct lv_context {
         cudaGraphNode_t begin_node;
     };
     std::vector<UpdateGraph> graphs;
-    MeasureJob* d_job = nullptr;
+    DeviceBuf<MeasureJob> d_job;
     bool use_graph = true;
     /* map growth (lv_map_set_growth): after every add the 64 B of map counters are copied into a pinned ring and an event is
      * recorded; before the next add the host bounds the map from the newest snapshot the device has finished */
@@ -155,14 +152,23 @@ struct lv_context {
     int64_t growths = 0;
     int64_t grow_waits = 0;
     int64_t waited_at_cap = 0;         /* capacity at which the policy last waited for a snapshot */
-    uint32_t* h_snap = nullptr;       /* pinned, kSnapRing x kMapCounters */
-    cudaEvent_t snap_ev[kSnapRing] = {};
+    PinnedBuf<uint32_t> h_snap;        /* kSnapRing x kMapCounters */
+    Event snap_ev[kSnapRing];
     int64_t snap_seq[kSnapRing] = {-1, -1, -1, -1};   /* add sequence number a slot holds (-1: none) */
     int64_t snap_cum[kSnapRing] = {};  /* points enqueued up to and including that add */
     int64_t add_seq = 0;               /* adds enqueued since the last clear */
     int64_t add_cum = 0;               /* points of those adds */
     uint32_t known[kMapCounters] = {}; /* newest finished snapshot (or the cleared map) */
     int64_t known_seq = 0, known_cum = 0;
+    /* the owners above free their buffers and events after this */
+    ~lv_context() {
+        if (stream) cudaStreamSynchronize(stream);
+        for (auto& e : pending) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
+        for (auto& e : pool) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
+        for (auto& u : graphs) { cudaGraphExecDestroy(u.exec); cudaGraphDestroy(u.graph); }
+        map_free(map);
+        if (own_stream && stream) cudaStreamDestroy(stream);
+    }
 };
 
 static lv_status drain_events(lv_context* h) {
@@ -243,12 +249,6 @@ static MeasureArgs make_measure_args(lv_context* h, const float* d_xyz, int64_t 
     return a;
 }
 
-template <class T>
-static cudaError_t ensure(T** p, size_t count) {
-    if (*p) return cudaSuccess;
-    return cudaMalloc(p, sizeof(T) * count);
-}
-
 /* argument checks of the _async forms; `what` names the call in the message */
 static bool n_max_ok(const char* what, int64_t n_max) {
     if (n_max >= 1 && n_max <= 0x7fffffff) return true;
@@ -278,12 +278,12 @@ static lv_status create_buffers(lv_context* h) {
     else { LV_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)); h->own_stream = true; }
     LV_CUDA(map_alloc(h->map, p->max_map_points, p->max_points, p->voxel_size, p->map_downsample_size, h->stream));
     { int l = 0; LV_CUDA(map_clear(h->map, h->stream, &l)); }
-    LV_CUDA(cudaMalloc(&h->d_sweep, sizeof(float) * 3 * p->max_points));
-    LV_CUDA(cudaMalloc(&h->d_nn_a, sizeof(int4) * p->max_points));
-    LV_CUDA(cudaMalloc(&h->d_nn_b, sizeof(int2) * p->max_points));
-    LV_CUDA(cudaMalloc(&h->d_hard_list, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
-    LV_CUDA(cudaMalloc(&h->d_ref, sizeof(float4) * p->max_points));
-    LV_CUDA(cudaMalloc(&h->d_redo, sizeof(uint32_t) * (p->max_points + 64)));   /* + one block of slack: read speculatively */
+    LV_CUDA(h->d_sweep.reserve(3 * (size_t)p->max_points));
+    LV_CUDA(h->d_nn_a.reserve(p->max_points));
+    LV_CUDA(h->d_nn_b.reserve(p->max_points));
+    LV_CUDA(h->d_hard_list.reserve((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters));
+    LV_CUDA(h->d_ref.reserve(p->max_points));
+    LV_CUDA(h->d_redo.reserve(p->max_points + 64));   /* + one block of slack: read speculatively */
     /* hand-over buffers start defined: lv_search_kernel<.., LIST> reads redo_list[] before it knows the list's length, and a
      * first update's reuse kernel must not see stale neighbours (also keeps compute-sanitizer initcheck quiet) */
     LV_CUDA(cudaMemset(h->d_redo, 0, sizeof(uint32_t) * (p->max_points + 64)));
@@ -293,27 +293,27 @@ static lv_status create_buffers(lv_context* h) {
     LV_CUDA(cudaMemset(h->d_hard_list, 0, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
     h->use_reuse = getenv("LV_NO_REUSE") == nullptr;
     h->use_pdl = getenv("LV_NO_PDL") == nullptr;
-    LV_CUDA(cudaMalloc(&h->d_job, sizeof(MeasureJob)));
+    LV_CUDA(h->d_job.reserve(1));
     measure_init();
     h->use_graph = getenv("LV_NO_GRAPH") == nullptr;
-    LV_CUDA(cudaMalloc(&h->d_ctrl, sizeof(UpdateCtrl)));
+    LV_CUDA(h->d_ctrl.reserve(1));
     LV_CUDA(cudaMemset(h->d_ctrl, 0, sizeof(UpdateCtrl)));
-    LV_CUDA(cudaMallocHost(&h->h_ctrl, sizeof(UpdateCtrl)));
-    LV_CUDA(cudaEventCreateWithFlags(&h->imu_copied, cudaEventDisableTiming));
-    LV_CUDA(cudaEventCreateWithFlags(&h->ctrl_copied, cudaEventDisableTiming));
-    LV_CUDA(cudaEventCreateWithFlags(&h->path_copied, cudaEventDisableTiming));
-    LV_CUDA(cudaMalloc(&h->d_async, sizeof(AsyncWords)));
+    LV_CUDA(h->h_ctrl.reserve(1));
+    LV_CUDA(h->imu_copied.create());
+    LV_CUDA(h->ctrl_copied.create());
+    LV_CUDA(h->path_copied.create());
+    LV_CUDA(h->d_async.reserve(1));
     LV_CUDA(cudaMemset(h->d_async, 0, sizeof(AsyncWords)));
-    LV_CUDA(cudaMallocHost(&h->h_async, sizeof(AsyncWords)));
-    LV_CUDA(cudaMalloc(&h->d_partials, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
+    LV_CUDA(h->h_async.reserve(1));
+    LV_CUDA(h->d_partials.reserve((size_t)kPartialStride * (kMeasureGridCap + 8)));
     LV_CUDA(cudaMemset(h->d_partials, 0, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
-    LV_CUDA(cudaMalloc(&h->d_group_rows, sizeof(double) * kPartialStride * 32));
+    LV_CUDA(h->d_group_rows.reserve((size_t)kPartialStride * 32));
     LV_CUDA(cudaMemset(h->d_group_rows, 0, sizeof(double) * kPartialStride * 32));
-    LV_CUDA(cudaMalloc(&h->d_group_tickets, sizeof(uint32_t) * 32));
+    LV_CUDA(h->d_group_tickets.reserve(32));
     LV_CUDA(cudaMemset(h->d_group_tickets, 0, sizeof(uint32_t) * 32));
-    LV_CUDA(cudaMalloc(&h->d_reduced, sizeof(double) * 160));
-    LV_CUDA(cudaMallocHost(&h->h_reduced, sizeof(double) * 160));
-    LV_CUDA(cudaMallocHost(&h->h_nevals, sizeof(int32_t) * kNevalsRing));
+    LV_CUDA(h->d_reduced.reserve(160));
+    LV_CUDA(h->h_reduced.reserve(160));
+    LV_CUDA(h->h_nevals.reserve(kNevalsRing));
     return LV_OK;
 }
 
@@ -361,30 +361,6 @@ lv_status lv_create(const lv_params* p, lv_handle* out) {
 void lv_destroy(lv_handle h) {
     if (!h) return;
     cudaSetDevice(h->prm.device);
-    if (h->stream) cudaStreamSynchronize(h->stream);
-    for (auto& e : h->pending) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
-    for (auto& e : h->pool) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
-    for (auto& u : h->graphs) { cudaGraphExecDestroy(u.exec); cudaGraphDestroy(u.graph); }
-    if (h->imu_copied) cudaEventDestroy(h->imu_copied);
-    if (h->ctrl_copied) cudaEventDestroy(h->ctrl_copied);
-    if (h->path_copied) cudaEventDestroy(h->path_copied);
-    cudaFree(h->d_async); cudaFreeHost(h->h_async);
-    cudaFree(h->lidar.xyz); cudaFree(h->lidar.time); cudaFree(h->lidar.words); cudaFreeHost(h->lidar.h_words);
-    cudaFree(h->lidar.intensity); cudaFree(h->lidar.range);
-    for (cudaEvent_t e : h->snap_ev) if (e) cudaEventDestroy(e);
-    cudaFreeHost(h->h_snap);
-    cudaFree(h->d_job); cudaFree(h->d_ref); cudaFree(h->d_redo); cudaFree(h->d_imu); cudaFreeHost(h->h_imu);
-    cudaFree(h->d_path); cudaFreeHost(h->h_path); cudaFree(h->d_times); cudaFree(h->d_deskew_in); cudaFree(h->d_bad); cudaFreeHost(h->h_bad);
-    ds_free(h->ds); cudaFree(h->d_ds_in); cudaFree(h->d_ds_out); cudaFree(h->d_ds_lanes);
-    map_free(h->map);
-    cudaFree(h->d_sweep); cudaFree(h->d_nn_a); cudaFree(h->d_nn_b); cudaFree(h->d_hard_list); cudaFree(h->d_ctrl); cudaFreeHost(h->h_ctrl); cudaFree(h->d_partials); cudaFree(h->d_group_rows); cudaFree(h->d_group_tickets);
-    cudaFree(h->d_reduced); cudaFreeHost(h->h_reduced); cudaFreeHost(h->h_nevals); cudaFree(h->d_flush);
-    cudaFree(h->d_valid); cudaFree(h->d_nn_idx); cudaFree(h->d_nn_sqd); cudaFree(h->d_plane);
-    cudaFree(h->d_dist); cudaFree(h->d_gworld); cudaFree(h->d_rows);
-    cudaFree(h->d_preloc);
-    cudaFree(h->d_pglob);
-    cudaFree(h->d_occ);
-    if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
 }
 
@@ -532,10 +508,8 @@ lv_status lv_map_set_growth(lv_handle h, int64_t max_points) {
     if (!h || max_points < 0) return LV_ERR_ARG;
     if (max_points == 0) { h->grow_limit = 0; return LV_OK; }
     LV_CUDA(cudaSetDevice(h->prm.device));
-    if (!h->h_snap) {
-        LV_CUDA(cudaMallocHost(&h->h_snap, sizeof(uint32_t) * kMapCounters * lv_context::kSnapRing));
-        for (cudaEvent_t& e : h->snap_ev) LV_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
+    LV_CUDA(h->h_snap.reserve((size_t)kMapCounters * lv_context::kSnapRing));
+    for (Event& e : h->snap_ev) LV_CUDA(e.create());
     if (!h->grow_limit) {                                          /* the counters as of now: the base of the bounds */
         LV_CUDA(map_fetch_counters(h->map, h->stream));
         LV_CUDA(cudaStreamSynchronize(h->stream));
@@ -609,7 +583,7 @@ static lv_status map_enqueue(lv_context* h, const float* xyz, bool on_host, int6
     const bool pr = prof_begin(h, kProfMap, &ep);
     int launches = 0;
     if (clears) LV_CUDA(map_clear(h->map, h->stream, &launches));
-    LV_CUDA(map_add(h->map, xyz, n, (!build && !empty && downsample) ? 1 : 0, h->stream, &launches, cnt, to_world ? h->d_ctrl : nullptr));
+    LV_CUDA(map_add(h->map, xyz, n, (!build && !empty && downsample) ? 1 : 0, h->stream, &launches, cnt, to_world ? h->d_ctrl.get() : nullptr));
     if (pr) prof_end(h, &ep);
     count_map_launches(h, launches);
     if (clears) snap_reset_cleared(h);
@@ -748,10 +722,8 @@ lv_status lv_propagate_device(lv_handle h, const double* acc, const double* gyro
     if (!h || !acc || !gyro || !dt || k < 0) return LV_ERR_ARG;
     if (k == 0) return LV_OK;
     LV_CUDA(cudaSetDevice(h->prm.device));
-    if (!h->d_imu) {
-        LV_CUDA(cudaMalloc(&h->d_imu, sizeof(double) * 7 * kImuBatch));
-        LV_CUDA(cudaMallocHost(&h->h_imu, sizeof(double) * 7 * kImuBatch));
-    }
+    LV_CUDA(h->d_imu.reserve(7 * kImuBatch));
+    LV_CUDA(h->h_imu.reserve(7 * kImuBatch));
     const lv_status s = sync_device_state(h);                     /* the host mirror may be newer (lv_set_state / lv_predict) */
     if (s != LV_OK) return s;
     const PredictNoise noise = {h->prm.covariance_gyroscope, h->prm.covariance_acceleration, h->prm.covariance_bias_gyroscope,
@@ -893,7 +865,7 @@ static lv_status enqueue_update(lv_context* h, const float* d_xyz, int64_t n, Up
 static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64_t n, bool as_job, bool capture, const UpdateGate& gate) {
     const int pdl = (h->use_pdl && !h->profile) ? 1 : 0;
     uint32_t* counters = h->d_hard_list + (size_t)kHardBuckets * hard_segment(h->prm.max_points);
-    LV_CUDA(launch_ieskf_begin(h->d_ctrl, as_job ? h->d_job : nullptr, d_xyz, (int)n, counters, gate, h->stream));
+    LV_CUDA(launch_ieskf_begin(h->d_ctrl, as_job ? h->d_job.get() : nullptr, d_xyz, (int)n, counters, gate, h->stream));
     if (!capture) h->prof.total_launches += 1;
     MeasureArgs a = update_measure_args(h, d_xyz, n, as_job);
     const int grid = measure_grid((int)n);
@@ -1026,10 +998,10 @@ static lv_status run_measure_once(lv_context* h, const double* x, const float* x
     LV_CUDA(launch_set_frame(h->d_ctrl, h->stream));
     MeasureArgs a = make_measure_args(h, h->d_sweep, n);
     const size_t mp = (size_t)h->prm.max_points;
-    if (want_rows) { LV_CUDA(ensure(&h->d_rows, 13 * mp)); LV_CUDA(ensure(&h->d_valid, mp)); a.rows = h->d_rows; a.valid = h->d_valid; }
+    if (want_rows) { LV_CUDA(h->d_rows.reserve(13 * mp)); LV_CUDA(h->d_valid.reserve(mp)); a.rows = h->d_rows; a.valid = h->d_valid; }
     if (want_debug) {
-        LV_CUDA(ensure(&h->d_valid, mp)); LV_CUDA(ensure(&h->d_nn_idx, 5 * mp)); LV_CUDA(ensure(&h->d_nn_sqd, 5 * mp));
-        LV_CUDA(ensure(&h->d_plane, 4 * mp)); LV_CUDA(ensure(&h->d_dist, mp)); LV_CUDA(ensure(&h->d_gworld, 3 * mp));
+        LV_CUDA(h->d_valid.reserve(mp)); LV_CUDA(h->d_nn_idx.reserve(5 * mp)); LV_CUDA(h->d_nn_sqd.reserve(5 * mp));
+        LV_CUDA(h->d_plane.reserve(4 * mp)); LV_CUDA(h->d_dist.reserve(mp)); LV_CUDA(h->d_gworld.reserve(3 * mp));
         a.valid = h->d_valid; a.nn_idx = h->d_nn_idx; a.nn_sqd = h->d_nn_sqd; a.plane = h->d_plane; a.dist = h->d_dist;
         a.g_world = h->d_gworld;
     }
@@ -1114,7 +1086,7 @@ lv_status lv_last_neighbours(lv_handle h, int64_t n, int32_t* nn_idx) {
     if (!h || !nn_idx || n <= 0 || n > h->prm.max_points) return LV_ERR_ARG;
     if (h->map.empty) return LV_EMPTY_MAP;
     LV_CUDA(cudaSetDevice(h->prm.device));
-    LV_CUDA(ensure(&h->d_nn_idx, 5 * (size_t)h->prm.max_points));
+    LV_CUDA(h->d_nn_idx.reserve(5 * (size_t)h->prm.max_points));
     lv_neighbour_ids_kernel<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(h->d_nn_a, h->d_nn_b, h->map.arena, (int)n, h->d_nn_idx);
     LV_CUDA(cudaGetLastError());
     LV_CUDA(cudaMemcpyAsync(nn_idx, h->d_nn_idx, sizeof(int32_t) * 5 * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
@@ -1186,14 +1158,8 @@ lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const
     const size_t off_frames = 256, off_offsets = (off_frames + sizeof(float) * frames.size() + 255) & ~(size_t)255;
     const size_t off_scores = (off_offsets + sizeof(float4) * offsets.size() + 255) & ~(size_t)255;
     const size_t bytes = off_scores + (scores_out ? sizeof(int32_t) * (size_t)count : 0);
-    if (bytes > h->preloc_bytes) {
-        cudaFree(h->d_preloc);
-        h->d_preloc = nullptr;
-        h->preloc_bytes = 0;
-        LV_CUDA(cudaMalloc(&h->d_preloc, bytes));
-        h->preloc_bytes = bytes;
-    }
-    uint8_t* base = static_cast<uint8_t*>(h->d_preloc);
+    LV_CUDA(h->d_preloc.reserve(bytes));
+    uint8_t* base = h->d_preloc;
     PrelocArgs a;
     a.xyz = d_xyz_lidar;
     a.n = n;
@@ -1247,27 +1213,12 @@ static lv_status pglob_map_empty(lv_context* h, const char* what) {
     if (h->map.empty) { set_error(std::string(what) + ": the map is empty"); return LV_EMPTY_MAP; }
     return LV_OK;
 }
-static lv_status pglob_reserve(lv_context* h, size_t bytes) {
-    if (bytes <= h->pglob_bytes) return LV_OK;
-    cudaFree(h->d_pglob);
-    h->d_pglob = nullptr;
-    h->pglob_bytes = 0;
-    LV_CUDA(cudaMalloc(&h->d_pglob, bytes));
-    h->pglob_bytes = bytes;
-    return LV_OK;
-}
 static size_t pglob_align(size_t b) { return (b + 255) & ~(size_t)255; }
 /* the occupancy summary of the map (h->occ: extent, bitmap pyramid in h->d_occ), rebuilt only when the map changed since it
  * was built (map_gen); LV_EMPTY_MAP when no block holds an occupied voxel */
 static lv_status pglob_occupancy(lv_context* h, const char* what, int* launches) {
     if (h->occ_gen != h->map_gen) {
-        if (h->occ_bytes < 256) {
-            cudaFree(h->d_occ);
-            h->d_occ = nullptr;
-            h->occ_bytes = 0;
-            LV_CUDA(cudaMalloc(&h->d_occ, 256));
-            h->occ_bytes = 256;
-        }
+        LV_CUDA(h->d_occ.reserve(64));
         uint32_t ext[6];
         LV_CUDA(cudaMemsetAsync(h->d_occ, 0xFF, 3 * sizeof(uint32_t), h->stream));
         LV_CUDA(cudaMemsetAsync(h->d_occ + 3, 0, 3 * sizeof(uint32_t), h->stream));
@@ -1279,14 +1230,7 @@ static lv_status pglob_occupancy(lv_context* h, const char* what, int* launches)
         for (int a = 0; a < 3; ++a) { o.lo[a] = ext[a]; o.hi[a] = ext[3 + a]; }
         if (ext[0] <= ext[3]) {
             const size_t words = (size_t)occ_layout(o);
-            const size_t bytes = 256 + sizeof(uint32_t) * words;
-            if (bytes > h->occ_bytes) {                            /* the extent stays in the first words: copied out above */
-                cudaFree(h->d_occ);
-                h->d_occ = nullptr;
-                h->occ_bytes = 0;
-                LV_CUDA(cudaMalloc(&h->d_occ, bytes));
-                h->occ_bytes = bytes;
-            }
+            LV_CUDA(h->d_occ.reserve(64 + words));                 /* a growth loses the extent: copied out above */
             uint32_t* bits = h->d_occ + 64;
             o.map = map_view(h->map);
             o.bits = bits;
@@ -1393,8 +1337,8 @@ lv_status lv_prelocalize_global(lv_handle h, const float* d_xyz_lidar, int64_t n
     const size_t off_frames = 0, off_cells = pglob_align(off_frames + sizeof(float) * frames.size());
     const size_t off_bounds = pglob_align(off_cells + sizeof(PrelocCell) * kPrelocChunk);
     const size_t off_best = pglob_align(off_bounds + sizeof(int32_t) * kPrelocChunk);
-    if (lv_status s = pglob_reserve(h, off_best + sizeof(PrelocBest) * kPrelocChunk)) return s;
-    uint8_t* base = static_cast<uint8_t*>(h->d_pglob);
+    LV_CUDA(h->d_pglob.reserve(off_best + sizeof(PrelocBest) * kPrelocChunk));
+    uint8_t* base = h->d_pglob;
     LV_CUDA(cudaMemcpyAsync(base + off_frames, frames.data(), sizeof(float) * frames.size(), cudaMemcpyHostToDevice, h->stream));
 
     DevicePrelocEval ev;
@@ -1486,12 +1430,10 @@ lv_status lv_memcpy_d2h(lv_handle h, void* dst, const void* src, int64_t bytes) 
 /* d_n: NULL (n points, the flag is read back into h_bad) or the device count of the async form (n is its bound) */
 static lv_status deskew_common(lv_context* h, const lv_state32* path, int32_t ns, const lv_state32* Xt2,
                                const float* d_xyz, const double* d_t, const int64_t* d_n, int64_t n, float* d_out) {
-    if (!h->d_path) {
-        LV_CUDA(cudaMalloc(&h->d_path, sizeof(lv_state32) * deskew_max_states()));
-        LV_CUDA(cudaMallocHost(&h->h_path, sizeof(lv_state32) * deskew_max_states()));
-        LV_CUDA(cudaMalloc(&h->d_bad, sizeof(int)));
-        LV_CUDA(cudaMallocHost(&h->h_bad, sizeof(int)));
-    }
+    LV_CUDA(h->d_path.reserve(deskew_max_states()));
+    LV_CUDA(h->h_path.reserve(deskew_max_states()));
+    LV_CUDA(h->d_bad.reserve(1));
+    LV_CUDA(h->h_bad.reserve(1));
     /* the pinned staging buffer is reused: the copy out of it queued by an earlier async call must have run */
     LV_CUDA(cudaEventSynchronize(h->path_copied));
     memcpy(h->h_path, path, sizeof(lv_state32) * (size_t)ns);
@@ -1548,10 +1490,8 @@ lv_status lv_compensate(lv_handle h, const lv_state32* path, int32_t ns, const l
     lv_status s = deskew_args_ok(h, path, ns, Xt2, xyz, t, n, xyz_out);
     if (s != LV_OK) return s;
     LV_CUDA(cudaSetDevice(h->prm.device));
-    if (!h->d_times) {
-        LV_CUDA(cudaMalloc(&h->d_times, sizeof(double) * h->prm.max_points));
-        LV_CUDA(cudaMalloc(&h->d_deskew_in, sizeof(float) * 3 * h->prm.max_points));
-    }
+    LV_CUDA(h->d_times.reserve(h->prm.max_points));
+    LV_CUDA(h->d_deskew_in.reserve(3 * (size_t)h->prm.max_points));
     LV_CUDA(cudaMemcpyAsync(h->d_deskew_in, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
     LV_CUDA(cudaMemcpyAsync(h->d_times, t, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
     s = deskew_common(h, path, ns, Xt2, h->d_deskew_in, h->d_times, nullptr, n, h->d_deskew_in);
@@ -1563,15 +1503,14 @@ lv_status lv_compensate(lv_handle h, const lv_state32* path, int32_t ns, const l
 }
 
 /* ---- downsamplers ------------------------------------------------------------------------------- */
+/* in / out xyz of the host forms, grown with slack; both are freed first, and d_ds_out, reserved last, is empty unless both fit */
 static lv_status ds_stage(lv_context* h, int64_t n) {
-    if (n <= h->ds_stage_cap) return LV_OK;
-    cudaFree(h->d_ds_in); cudaFree(h->d_ds_out);
-    h->d_ds_in = h->d_ds_out = nullptr;
-    h->ds_stage_cap = 0;
-    const int64_t cap = n + n / 4 + 1024;
-    LV_CUDA(cudaMalloc(&h->d_ds_in, sizeof(float) * 3 * cap));
-    LV_CUDA(cudaMalloc(&h->d_ds_out, sizeof(float) * 3 * cap));
-    h->ds_stage_cap = cap;
+    if (3 * (size_t)n <= h->d_ds_out.size()) return LV_OK;
+    const size_t cap = (size_t)(n + n / 4 + 1024);
+    h->d_ds_in.reset();
+    h->d_ds_out.reset();
+    LV_CUDA(h->d_ds_in.reserve(3 * cap));
+    LV_CUDA(h->d_ds_out.reserve(3 * cap));
     return LV_OK;
 }
 /* the synchronous voxel grid of n > 0 device points (lanes: the full form's attributes): the async form's kernels over the
@@ -1661,17 +1600,6 @@ lv_status lv_voxelgrid_downsample(lv_handle h, const float* xyz, int64_t n, floa
     LV_CUDA(cudaStreamSynchronize(h->stream));
     return LV_OK;
 }
-/* device staging of the full host form's attributes: in / out time, then in / out intensity and out range */
-static lv_status ds_stage_lanes(lv_context* h, int64_t n) {
-    if (n <= h->ds_lanes_cap) return LV_OK;
-    cudaFree(h->d_ds_lanes);
-    h->d_ds_lanes = nullptr;
-    h->ds_lanes_cap = 0;
-    const int64_t cap = n + n / 4 + 1024;
-    LV_CUDA(cudaMalloc(&h->d_ds_lanes, 28 * (size_t)cap));
-    h->ds_lanes_cap = cap;
-    return LV_OK;
-}
 lv_status lv_voxelgrid_downsample_full(lv_handle h, const float* xyz, const double* time, const float* intensity, int64_t n, float leaf,
                                        float* xyz_out, double* time_out, float* intensity_out, float* range_out, int64_t* n_out) {
     if (n_out) *n_out = 0;
@@ -1685,11 +1613,12 @@ lv_status lv_voxelgrid_downsample_full(lv_handle h, const float* xyz, const doub
     if (n == 0) return LV_OK;
     LV_CUDA(cudaSetDevice(h->prm.device));
     lv_status s = ds_stage(h, n);
-    if (s == LV_OK) s = ds_stage_lanes(h, n);
     if (s != LV_OK) return s;
-    const int64_t c = h->ds_lanes_cap;
+    /* device staging of the attributes, grown with slack as ds_stage: in / out time, then in / out intensity and out range */
+    if (28 * (size_t)n > h->d_ds_lanes.size()) LV_CUDA(h->d_ds_lanes.reserve(28 * (size_t)(n + n / 4 + 1024)));
+    const int64_t c = (int64_t)(h->d_ds_lanes.size() / 28);
     VoxelLanes lanes;
-    double* t_in = reinterpret_cast<double*>(h->d_ds_lanes);
+    double* t_in = reinterpret_cast<double*>(h->d_ds_lanes.get());
     float* f = reinterpret_cast<float*>(t_in + 2 * c);
     lanes.time = t_in; lanes.time_out = t_in + c;
     lanes.intensity = f; lanes.intensity_out = f + c; lanes.range_out = f + 2 * c;
@@ -1825,12 +1754,9 @@ static lv_status lidar_resize(lv_handle h, int64_t capacity, bool full, const ch
     if (!h) { set_error(std::string(what) + ": null handle"); return LV_ERR_ARG; }
     LV_CUDA(cudaSetDevice(h->prm.device));
     LidarRing& r = h->lidar;
-    if (!r.words) {
-        LidarWords *d = nullptr, *hw = nullptr;
-        LV_CUDA(cudaMalloc(&d, sizeof(LidarWords)));
-        if (cudaMallocHost(&hw, sizeof(LidarWords)) != cudaSuccess) { cudaFree(d); LV_CUDA(cudaGetLastError()); }
-        r.words = d;
-        r.h_words = hw;
+    if (!r.h_words) {                                             /* the first call, or a retry of one that failed */
+        LV_CUDA(r.words.reserve(1));
+        LV_CUDA(r.h_words.reserve(1));
         LV_CUDA(cudaMemsetAsync(r.words, 0, sizeof(LidarWords), h->stream));
     }
     LV_CUDA(cudaMemcpyAsync(r.h_words, r.words, sizeof(LidarWords), cudaMemcpyDeviceToHost, h->stream));
@@ -1844,27 +1770,24 @@ static lv_status lidar_resize(lv_handle h, int64_t capacity, bool full, const ch
         set_error(buf);
         return LV_ERR_CAPACITY;
     }
-    float *xyz = nullptr, *intensity = nullptr, *range = nullptr;
-    double* time = nullptr;
-    cudaError_t e = cudaMalloc(&xyz, sizeof(float) * 3 * (size_t)capacity);
-    if (e == cudaSuccess) e = cudaMalloc(&time, sizeof(double) * (size_t)capacity);
-    if (e == cudaSuccess && lanes) e = cudaMalloc(&intensity, sizeof(float) * (size_t)capacity);
-    if (e == cudaSuccess && lanes) e = cudaMalloc(&range, sizeof(float) * (size_t)capacity);
+    /* the new arrays are allocated while the old ones still hold the live points */
+    DeviceBuf<float> xyz, intensity, range;
+    DeviceBuf<double> time;
+    cudaError_t e = xyz.reserve(3 * (size_t)capacity);
+    if (e == cudaSuccess) e = time.reserve(capacity);
+    if (e == cudaSuccess && lanes) e = intensity.reserve(capacity);
+    if (e == cudaSuccess && lanes) e = range.reserve(capacity);
     int launches = 0;
     if (e == cudaSuccess) e = launch_lidar_move(r, live, xyz, time, capacity, h->stream, &launches, intensity, range);
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
     if (e != cudaSuccess) {                                       /* the buffer stays as it was */
-        cudaFree(xyz); cudaFree(time); cudaFree(intensity); cudaFree(range);
         cudaGetLastError();
         set_error(std::string(what) + ": " + cudaGetErrorString(e));
         return LV_ERR_CAPACITY;
     }
     h->prof.total_launches += launches;
-    cudaFree(r.xyz); cudaFree(r.time); cudaFree(r.intensity); cudaFree(r.range);
-    r.xyz = xyz;
-    r.time = time;
-    r.intensity = intensity;
-    r.range = range;
+    r.xyz = std::move(xyz); r.time = std::move(time);
+    r.intensity = std::move(intensity); r.range = std::move(range);
     r.cap = capacity;
     return LV_OK;
 }
@@ -2023,7 +1946,7 @@ lv_status lv_flush_l2(lv_handle h) {
     if (!h) return LV_ERR_ARG;
     LV_CUDA(cudaSetDevice(h->prm.device));
     const size_t bytes = 256ull << 20;
-    if (!h->d_flush) LV_CUDA(cudaMalloc(&h->d_flush, bytes));
+    LV_CUDA(h->d_flush.reserve(bytes));
     LV_CUDA(launch_l2_flush(h->d_flush, bytes, h->stream));
     h->prof.total_launches += 1;
     return LV_OK;

@@ -92,13 +92,13 @@ cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const
                                  int* launches) {
     const int64_t bound = cloud_bound(a.n, a.rate);
     lv_cloud_flag_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, st>>>(a, s.flags, s.count);
-    size_t tmp = s.tmp_bytes;
-    cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags, s.sel, s.count, (int)a.n, st);
+    size_t tmp = s.tmp.size();
+    cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags.get(), s.sel.get(), s.count.get(), (int)a.n, st);
     if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)((bound + 255) / 256);
     lv_cloud_key_kernel<<<grid, 256, 0, st>>>(a, s.sel, s.count, bound, s.keys64, s.vals, err);
-    tmp = s.tmp_bytes;
-    e = cub::DeviceRadixSort::SortPairs(s.tmp, tmp, s.keys64, s.keys64_sorted, s.vals, s.vals_sorted, (int)bound, 0, 64, st);
+    tmp = s.tmp.size();
+    e = cub::DeviceRadixSort::SortPairs(s.tmp, tmp, s.keys64.get(), s.keys64_sorted.get(), s.vals.get(), s.vals_sorted.get(), (int)bound, 0, 64, st);
     if (e != cudaSuccess) return e;
     lv_cloud_gather_kernel<<<grid, 256, 0, st>>>(a, s.vals_sorted, s.count, o.xyz, o.time, o.intensity, o.range, o.idx, d_n_out);
     if (!d_n_out) cudaMemcpyAsync(s.h_count, s.count, 2 * sizeof(int), cudaMemcpyDeviceToHost, st);   /* the synchronous form reads them */

@@ -168,15 +168,14 @@ __global__ void __launch_bounds__(256) lv_ds_gather_kernel(const float* __restri
 /* ---- scratch + launchers ------------------------------------------------------------------------ */
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n) {
     if (n <= s.cap) return cudaSuccess;
-    cudaFree(s.keys); cudaFree(s.keys_sorted); cudaFree(s.vals); cudaFree(s.vals_sorted); cudaFree(s.flags); cudaFree(s.sel);
-    cudaFree(s.keys64); cudaFree(s.keys64_sorted);
-    cudaFree(s.tmp);
-    if (!s.box) {
-        cudaError_t e = cudaMalloc(&s.box, sizeof(GridBox));
-        if (e != cudaSuccess) return e;
-        if ((e = cudaMalloc(&s.count, 2 * sizeof(int))) != cudaSuccess) return e;
-        if ((e = cudaMallocHost(&s.h_count, 2 * sizeof(int))) != cudaSuccess) return e;
-    }
+    /* every per-point array is freed before any is reallocated, so the peak stays at the new size */
+    s.cap = 0;
+    s.keys.reset(); s.keys_sorted.reset(); s.vals.reset(); s.vals_sorted.reset(); s.flags.reset(); s.sel.reset();
+    s.keys64.reset(); s.keys64_sorted.reset();
+    s.tmp.reset();
+    cudaError_t e;
+    if ((e = s.box.reserve(1)) != cudaSuccess || (e = s.count.reserve(2)) != cudaSuccess || (e = s.h_count.reserve(2)) != cudaSuccess)
+        return e;
     const int64_t cap = n + n / 4 + 1024;
     size_t a = 0, b = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, a, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
@@ -186,44 +185,37 @@ cudaError_t ds_reserve(DownsampleScratch& s, int64_t n) {
     size_t c = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, c, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const uint32_t*)nullptr,
                                     (uint32_t*)nullptr, (int)cap);
-    s.tmp_bytes = (a > b ? a : b);
-    s.tmp_bytes = (s.tmp_bytes > c ? s.tmp_bytes : c) + 256;
-    cudaError_t e;
-    if ((e = cudaMalloc(&s.keys, sizeof(uint32_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.keys_sorted, sizeof(uint32_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.vals, sizeof(uint32_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.vals_sorted, sizeof(uint32_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.flags, sizeof(uint8_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.sel, sizeof(int32_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.keys64, sizeof(uint64_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.keys64_sorted, sizeof(uint64_t) * cap)) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&s.tmp, s.tmp_bytes)) != cudaSuccess) return e;
+    size_t tmp_bytes = (a > b ? a : b);
+    tmp_bytes = (tmp_bytes > c ? tmp_bytes : c) + 256;
+    if ((e = s.keys.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.keys_sorted.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.vals.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.vals_sorted.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.flags.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.sel.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.keys64.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.keys64_sorted.reserve(cap)) != cudaSuccess) return e;
+    if ((e = s.tmp.reserve(tmp_bytes)) != cudaSuccess) return e;
     s.cap = cap;
     return cudaSuccess;
-}
-void ds_free(DownsampleScratch& s) {
-    cudaFree(s.keys); cudaFree(s.keys_sorted); cudaFree(s.vals); cudaFree(s.vals_sorted); cudaFree(s.flags); cudaFree(s.sel);
-    cudaFree(s.keys64); cudaFree(s.keys64_sorted);
-    cudaFree(s.tmp); cudaFree(s.box); cudaFree(s.count); cudaFreeHost(s.h_count);
-    s = DownsampleScratch();
 }
 
 cudaError_t launch_voxelgrid(DownsampleScratch& s, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf, float* d_out,
                              int64_t* d_n_out, uint32_t* err, cudaStream_t st, int* launches, const VoxelLanes* lanes) {
     const unsigned grid = (unsigned)((n_max + 255) / 256);
-    GridBox* box = static_cast<GridBox*>(s.box);
+    GridBox* box = s.box;
     const float inv = fdiv(1.0f, leaf);
     lv_ds_box_init_kernel<<<1, 32, 0, st>>>(box, d_n, n_max, err);
     lv_ds_box_kernel<<<grid < kNumSMs * 4u ? grid : kNumSMs * 4u, 256, 0, st>>>(d_xyz, box);
     lv_ds_keys_kernel<<<grid, 256, 0, st>>>(d_xyz, n_max, inv, box, s.keys, s.vals);
-    size_t tmp = s.tmp_bytes;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(s.tmp, tmp, s.keys, s.keys_sorted, s.vals, s.vals_sorted, (int)n_max, 0, 32, st);
+    size_t tmp = s.tmp.size();
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(s.tmp, tmp, s.keys.get(), s.keys_sorted.get(), s.vals.get(), s.vals_sorted.get(), (int)n_max, 0, 32, st);
     if (e != cudaSuccess) return e;
     lv_ds_heads_kernel<<<grid, 256, 0, st>>>(s.keys_sorted, n_max, box, s.flags);
-    tmp = s.tmp_bytes;
-    e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags, s.sel, s.count, (int)n_max, st);
+    tmp = s.tmp.size();
+    e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags.get(), s.sel.get(), s.count.get(), (int)n_max, st);
     if (e != cudaSuccess) return e;
-    const uint32_t* starts = reinterpret_cast<const uint32_t*>(s.sel);
+    const uint32_t* starts = reinterpret_cast<const uint32_t*>(s.sel.get());
     const unsigned fgrid = (unsigned)((3 * n_max + 255) / 256);
     if (lanes) {
         lv_ds_centroid_kernel<true><<<grid, 256, 0, st>>>(d_xyz, s.vals_sorted, starts, s.count, box, d_out, *lanes);
@@ -244,9 +236,9 @@ cudaError_t launch_temporal(DownsampleScratch& s, const float* d_xyz, int64_t n,
                             int32_t* d_idx_out, cudaStream_t st, int* launches) {
     const unsigned grid = (unsigned)((n + 255) / 256);
     lv_ds_temporal_flag_kernel<<<grid, 256, 0, st>>>(d_xyz, n, rate, min_dist, s.flags);
-    size_t tmp = s.tmp_bytes;
+    size_t tmp = s.tmp.size();
     int32_t* idx = d_idx_out ? d_idx_out : s.sel;
-    cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags, idx, s.count, (int)n, st);
+    cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags.get(), idx, s.count.get(), (int)n, st);
     if (e != cudaSuccess) return e;
     lv_ds_gather_kernel<<<grid, 256, 0, st>>>(d_xyz, idx, s.count, d_out);
     cudaMemcpyAsync(&s.h_count[0], s.count, sizeof(int), cudaMemcpyDeviceToHost, st);

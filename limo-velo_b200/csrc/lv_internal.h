@@ -8,6 +8,7 @@
 #include <stdint.h>
 
 #include "../../include/limovelo_b200.h"
+#include "lv_buffers.h"
 #include "lv_ieskf.h"
 #include "lv_preloc_bound.h"
 #include "lv_voxel_search.h"
@@ -189,20 +190,19 @@ cudaError_t launch_set_frame(UpdateCtrl* c, cudaStream_t st);   /* frame from c-
 cudaError_t launch_l2_flush(void* buf, size_t bytes, cudaStream_t st);
 
 /* lv_downsample.cu: PointCloudProcessor::temporal_downsample and Compensator::voxelgrid_downsample */
+struct GridBox;
 struct DownsampleScratch {
-    int64_t cap = 0;
-    uint32_t *keys = nullptr, *keys_sorted = nullptr, *vals = nullptr, *vals_sorted = nullptr;
-    uint64_t *keys64 = nullptr, *keys64_sorted = nullptr;   /* time keys of lv_cloud.cu */
-    uint8_t* flags = nullptr;
-    int32_t* sel = nullptr;
-    void* tmp = nullptr;
-    size_t tmp_bytes = 0;
-    void* box = nullptr;           /* GridBox */
-    int* count = nullptr;          /* [0] output count, [1] NaN-time flag (lv_cloud.cu) */
-    int* h_count = nullptr;        /* pinned: [0] output count, [1] overflow flag (voxel grid) / NaN-time flag (cloud) */
+    int64_t cap = 0;               /* points every per-point array holds (0 until all of them are allocated) */
+    DeviceBuf<uint32_t> keys, keys_sorted, vals, vals_sorted;
+    DeviceBuf<uint64_t> keys64, keys64_sorted;   /* time keys of lv_cloud.cu */
+    DeviceBuf<uint8_t> flags;
+    DeviceBuf<int32_t> sel;
+    DeviceBuf<uint8_t> tmp;        /* cub's temporary storage: tmp.size() bytes */
+    DeviceBuf<GridBox> box;
+    DeviceBuf<int> count;          /* [0] output count, [1] NaN-time flag (lv_cloud.cu) */
+    PinnedBuf<int> h_count;        /* [0] output count, [1] overflow flag (voxel grid) / NaN-time flag (cloud) */
 };
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n);
-void ds_free(DownsampleScratch& s);
 /* the attribute lanes of a full voxel grid (lv_voxelgrid_downsample_full): the inputs (intensity summed per leaf; time read by
  * the overflow pass-through only; range is never read: every output's range is |output xyz|) and the outputs, any of which may
  * be NULL */
@@ -261,13 +261,13 @@ struct LidarWords {
     uint32_t pad;
 };
 struct LidarRing {
-    float* xyz = nullptr;      /* cap x 3 */
-    double* time = nullptr;    /* cap     */
-    float* intensity = nullptr;   /* cap, or NULL: a ring without attribute lanes (lv_lidar_reserve_full adds them) */
-    float* range = nullptr;       /* cap, with intensity */
+    DeviceBuf<float> xyz;      /* cap x 3 */
+    DeviceBuf<double> time;    /* cap     */
+    DeviceBuf<float> intensity;   /* cap, or empty: a ring without attribute lanes (lv_lidar_reserve_full adds them) */
+    DeviceBuf<float> range;       /* cap, with intensity */
     int64_t cap = 0;           /* 0: not reserved yet */
-    LidarWords* words = nullptr;
-    LidarWords* h_words = nullptr;   /* pinned */
+    DeviceBuf<LidarWords> words;
+    PinnedBuf<LidarWords> h_words;
 };
 /* push *d_n (clamped to [0, n_max]) points; kAsyncLidarFull and nothing appended when they do not fit.  On a ring with lanes the
  * points' intensity and range go with them (NULL: 0) */

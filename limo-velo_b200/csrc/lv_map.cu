@@ -434,32 +434,26 @@ cudaError_t map_points_sorted(MapBuffers& b, float* host_out, int64_t cap, int64
     const int64_t n = (int64_t)(int32_t)b.h_counters[kCtrPoints];
     *n_out = n;
     if (n <= 0 || !host_out || cap <= 0) return cudaSuccess;
-    float4* pts = nullptr;
-    uint32_t *ids = nullptr, *idx = nullptr, *ids2 = nullptr, *idx2 = nullptr;
-    float* xyz = nullptr;
-    void* tmp = nullptr;
+    DeviceBuf<float4> pts;
+    DeviceBuf<uint32_t> ids, idx, ids2, idx2;
+    DeviceBuf<float> xyz;
+    DeviceBuf<uint8_t> tmp;
     size_t tmp_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ids, ids2, idx, idx2, (int)n, 0, 32);
-    e = cudaMalloc(&pts, sizeof(float4) * (size_t)n);
-    if (e == cudaSuccess) e = cudaMalloc(&ids, sizeof(uint32_t) * (size_t)n);
-    if (e == cudaSuccess) e = cudaMalloc(&idx, sizeof(uint32_t) * (size_t)n);
-    if (e == cudaSuccess) e = cudaMalloc(&ids2, sizeof(uint32_t) * (size_t)n);
-    if (e == cudaSuccess) e = cudaMalloc(&idx2, sizeof(uint32_t) * (size_t)n);
-    if (e == cudaSuccess) e = cudaMalloc(&xyz, sizeof(float) * 3 * (size_t)n);
-    if (e == cudaSuccess) e = cudaMalloc(&tmp, tmp_bytes);
-    if (e == cudaSuccess) {
-        const VoxelMapRW m = map_rw(b);
-        const unsigned blocks = (unsigned)((n + 255) / 256);
-        cudaMemsetAsync(b.counters + kCtrGather, 0, sizeof(uint32_t), st);
-        lv_map_gather_kernel<<<kNumSMs * 8, 256, 0, st>>>(m, pts, (uint32_t)n);
-        lv_map_ids_kernel<<<blocks, 256, 0, st>>>(pts, (uint32_t)n, ids, idx);
-        e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, ids, ids2, idx, idx2, (int)n, 0, 32, st);
-        lv_map_unpack_kernel<<<blocks, 256, 0, st>>>(pts, idx2, (uint32_t)n, xyz);
-        const int64_t m_out = n < cap ? n : cap;
-        if (e == cudaSuccess) e = cudaMemcpyAsync(host_out, xyz, sizeof(float) * 3 * (size_t)m_out, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    }
-    cudaFree(pts); cudaFree(ids); cudaFree(idx); cudaFree(ids2); cudaFree(idx2); cudaFree(xyz); cudaFree(tmp);
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, ids.get(), ids2.get(), idx.get(), idx2.get(), (int)n, 0, 32);
+    if ((e = pts.reserve(n)) != cudaSuccess || (e = ids.reserve(n)) != cudaSuccess || (e = idx.reserve(n)) != cudaSuccess ||
+        (e = ids2.reserve(n)) != cudaSuccess || (e = idx2.reserve(n)) != cudaSuccess || (e = xyz.reserve(3 * (size_t)n)) != cudaSuccess ||
+        (e = tmp.reserve(tmp_bytes)) != cudaSuccess)
+        return e;
+    const VoxelMapRW m = map_rw(b);
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    cudaMemsetAsync(b.counters + kCtrGather, 0, sizeof(uint32_t), st);
+    lv_map_gather_kernel<<<kNumSMs * 8, 256, 0, st>>>(m, pts, (uint32_t)n);
+    lv_map_ids_kernel<<<blocks, 256, 0, st>>>(pts, (uint32_t)n, ids, idx);
+    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, ids.get(), ids2.get(), idx.get(), idx2.get(), (int)n, 0, 32, st);
+    lv_map_unpack_kernel<<<blocks, 256, 0, st>>>(pts, idx2, (uint32_t)n, xyz);
+    const int64_t m_out = n < cap ? n : cap;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(host_out, xyz, sizeof(float) * 3 * (size_t)m_out, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     return e;
 }
 

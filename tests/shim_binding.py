@@ -1,5 +1,6 @@
 """ctypes binding of tests/cpu_shim/liblv_cpushim.so (TEST-ONLY host build of the product headers): the map, search and
-filter (shim.cpp), the LiDAR buffer (lidar_ring.cpp) and the start-pose searches (preloc.cpp)."""
+filter (shim.cpp), the LiDAR buffer (lidar_ring.cpp), the start-pose searches (preloc.cpp) and the buffer and event owners over
+a fake CUDA runtime (buffers.cpp)."""
 import ctypes as C
 import os
 import subprocess
@@ -77,6 +78,29 @@ def lib():
         L.shim_pg_search.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, f, f, C.c_int32, C.c_int, C.POINTER(i64), C.POINTER(i64)]
         L.shim_pg_extent.argtypes = [fp, i64, f, f, C.POINTER(C.c_uint32), i32p]
         L.shim_pg_top_level.argtypes = [i64, i64]
+
+        L.shim_buf_fail_at.argtypes = [i64]
+        L.shim_buf_fail_at.restype = None
+        L.shim_buf_counts.argtypes = [C.POINTER(i64)]
+        L.shim_buf_counts.restype = None
+        L.shim_buf_new.argtypes = [C.c_int]
+        L.shim_buf_new.restype = vp
+        L.shim_buf_move_new.argtypes = [vp]
+        L.shim_buf_move_new.restype = vp
+        L.shim_buf_move_assign.argtypes = [vp, vp]
+        L.shim_buf_move_assign.restype = None
+        L.shim_buf_reserve.argtypes = [vp, i64]
+        L.shim_buf_size.argtypes = [vp]
+        L.shim_buf_size.restype = i64
+        L.shim_buf_ptr.argtypes = [vp]
+        L.shim_buf_ptr.restype = C.c_size_t
+        for fn in (L.shim_buf_reset, L.shim_buf_delete, L.shim_event_delete):
+            fn.argtypes = [vp]
+            fn.restype = None
+        L.shim_event_new.restype = vp
+        L.shim_event_create.argtypes = [vp]
+        L.shim_event_handle.argtypes = [vp]
+        L.shim_event_handle.restype = C.c_size_t
         _lib = L
     return _lib
 
