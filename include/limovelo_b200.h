@@ -468,6 +468,34 @@ lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_clou
                                   float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
                                   int64_t* n_out);
 
+/* ---- Livox messages: livox_ros_driver/CustomMsg (livox_ros_driver2/CustomMsg has the same fields) -------------------------------
+ * Not a PointCloud2: one uint64 time base (ns, the first point's time) per message, then packed 19-byte records
+ *     uint32 offset_time (ns after timebase) | float32 x | float32 y | float32 z | uint8 reflectivity | uint8 tag | uint8 line
+ * (little endian, a record at data + 19 i, any alignment; lv_bag_parse_livox finds them in a bag).  Per point:
+ *   time       total = timebase + offset_time (uint64 ns), then (double)(int64)(total / 10^9) + (double)(total % 10^9) * 1e-9, the sum
+ *              and the product unfused (Conversions::nanosec2Sec, Utils.cpp:25-30, with a 64-bit quotient).  Absolute, like the
+ *              Hesai's: stamp_beginning, offset_beginning and full_rotation_time do not apply and the header stamp is not read.  A
+ *              timebase above 2^64 - 2^32 is refused (the sum could wrap).
+ *   tag        the point is dropped when (tag & tag_reject_mask) != 0: 0 keeps every point, 0x20 keeps the first and the single
+ *              returns (tag bits 4-5 are the return number), 0x0F also drops what the sensor marks as noise (bits 0-3)
+ *   outputs    xyz as stored, intensity = (float)reflectivity, range = the fp32 |p| (Point.cpp:166-169), idx = the index in the message
+ *              (the caller reads tag and line through it). */
+/* msg2points on the host: the tag-kept points, in message order, into xyz (n x 3), time, intensity, range and idx (n each; intensity,
+ * range and idx may be NULL); *n_out = their count.  LV_ERR_ARG for null data / xyz / time / n_out, n outside [0, 2^31 - 1], n
+ * records beyond data_bytes or the timebase limit. */
+lv_status lv_livox_to_points(const uint8_t* data, int64_t data_bytes, int64_t n, uint64_t timebase_ns, uint8_t tag_reject_mask,
+                             float* xyz, double* time, float* intensity, float* range, int32_t* idx, int64_t* n_out);
+/* Accumulator::process on the device for a Livox message: the tag filter (msg2points) -> temporal_downsample on the RANK of the point
+ * among the tag-kept points (not its message index; with mask 0 they are the same) -> sort_points (stable in time, equal times in
+ * message order).  d_data: DEVICE copy of the records (data_bytes long, any alignment).  Outputs as lv_process_cloud_device: DEVICE
+ * buffers with room for n points (d_intensity, d_range, d_idx may be NULL), ascending in time.  Bit for bit lv_livox_to_points, then
+ * lv_temporal_downsample on its output, then lv_time_sort_indices on the kept times, then the gathers.  LV_ERR_ARG, before any device
+ * work and also with a null handle, for null d_data / xyz / time / n_out, n outside [0, 2^31 - 1], n records beyond data_bytes, the
+ * timebase limit, or an output range that overlaps [d_data, d_data + data_bytes).  Synchronises (n_out). */
+lv_status lv_process_livox_device(lv_handle h, const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t timebase_ns,
+                                  uint8_t tag_reject_mask, int32_t downsample_rate, double min_dist,
+                                  float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out);
+
 /* ---- the tick without a host wait (main.cpp:76-105) ------------------------------------------------------------------------
  * Stream-ordered forms of the tick's device calls.  Each takes its input count from DEVICE memory (d_n, an int64_t) and writes
  * its output count to device memory (d_n_out), so that one stage hands its count to the next without the host: none of them
@@ -482,6 +510,12 @@ lv_status lv_process_cloud_device_async(lv_handle h, lv_lidar_type type, const l
                                         const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t header_stamp_us,
                                         int stamp_beginning, int offset_beginning, double full_rotation_time,
                                         int32_t downsample_rate, double min_dist,
+                                        float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
+                                        int64_t* d_n_out);
+/* lv_process_livox_device with *d_n_out = points kept; feeds lv_lidar_push_full_device_async (d_intensity, d_range) or
+ * lv_lidar_push_device_async directly.  The output buffers have room for n points. */
+lv_status lv_process_livox_device_async(lv_handle h, const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t timebase_ns,
+                                        uint8_t tag_reject_mask, int32_t downsample_rate, double min_dist,
                                         float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
                                         int64_t* d_n_out);
 /* Compensator::compensate (Compensator.cpp:123-146) as lv_compensate_device over *d_n points.  The path and Xt2 stay host-built
@@ -642,6 +676,19 @@ typedef struct lv_imu_sample {
     double linear_acceleration[3];
 } lv_imu_sample;
 lv_status lv_bag_parse_imu(const uint8_t* msg, int64_t size, lv_imu_sample* out);
+/* livox_ros_driver(2)/CustomMsg -> a view of the 19-byte records, ready for lv_livox_to_points / lv_process_livox_device
+ * (data, data_bytes, n_points, timebase).  LV_ERR_ARG for a null argument, a truncated message, bytes after the records, or a
+ * point_num that differs from the record count (the driver always writes them equal). */
+typedef struct lv_livox_view {
+    uint32_t stamp_sec, stamp_nsec;      /* header.stamp                                          */
+    uint64_t timebase;                   /* ns: the time of the first point                       */
+    uint32_t point_num;
+    uint8_t lidar_id;
+    int64_t n_points;                    /* records in `points`                                   */
+    const uint8_t* data;                 /* the first record (any alignment)                      */
+    int64_t data_bytes;                  /* 19 x n_points                                         */
+} lv_livox_view;
+lv_status lv_bag_parse_livox(const uint8_t* msg, int64_t size, lv_livox_view* out);
 
 /* ---- PCD map files (the map format of PCL, pcl::io::savePCDFileBinary, and of most LiDAR SLAM tools).  Host code.
  * Saving the device map: lv_map_points -> lv_pcd_write.  Loading it: lv_pcd_read -> lv_map_build (KD_TREE::Build: file order

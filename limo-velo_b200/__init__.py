@@ -203,6 +203,12 @@ def lib():
         L.lv_voxelgrid_downsample_full.argtypes = [vp, vp, vp, vp, i64, C.c_float, vp, vp, vp, vp, C.POINTER(i64)]
         L.lv_voxelgrid_downsample_full_device_async.argtypes = [vp, vp, vp, vp, vp, i64, C.c_float, vp, vp, vp, vp, vp]
         L.lv_cloud_stamp_device_async.argtypes = [vp, vp, vp, i64, vp]
+    if hasattr(L, "lv_process_livox_device"):   # the Livox front end; absent from older builds
+        L.lv_livox_to_points.argtypes = [vp, i64, i64, C.c_uint64, C.c_uint8, vp, vp, vp, vp, vp, C.POINTER(i64)]
+        L.lv_process_livox_device.argtypes = [vp, vp, i64, i64, C.c_uint64, C.c_uint8, C.c_int32, C.c_double, vp, vp, vp, vp, vp,
+                                              C.POINTER(i64)]
+        L.lv_process_livox_device_async.argtypes = [vp, vp, i64, i64, C.c_uint64, C.c_uint8, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
+        L.lv_bag_parse_livox.argtypes = [vp, i64, C.POINTER(LivoxView)]
     if hasattr(L, "lv_prelocalize"):   # start pose search and PCD files; absent from older builds
         L.lv_preloc_count.argtypes = [C.POINTER(PrelocParams)]
         L.lv_preloc_count.restype = i64
@@ -393,6 +399,37 @@ def time_sort_indices(t):
     idx = np.zeros(len(t), np.int32)
     _check(lib().lv_time_sort_indices(_d(t), C.c_int64(len(t)), idx.ctypes.data_as(C.POINTER(C.c_int32))))
     return idx
+
+
+# livox_ros_driver(2)/CustomMsg: one 19-byte record per point (include/limovelo_b200.h)
+LIVOX_RECORD = np.dtype({"names": ["offset_time", "x", "y", "z", "reflectivity", "tag", "line"],
+                         "formats": ["<u4", "<f4", "<f4", "<f4", "u1", "u1", "u1"], "offsets": [0, 4, 8, 12, 16, 17, 18], "itemsize": 19})
+
+
+class LivoxView(C.Structure):
+    _fields_ = [("stamp_sec", C.c_uint32), ("stamp_nsec", C.c_uint32), ("timebase", C.c_uint64), ("point_num", C.c_uint32),
+                ("lidar_id", C.c_uint8), ("n_points", C.c_int64), ("data", C.c_void_p), ("data_bytes", C.c_int64)]
+
+
+def bag_parse_livox(msg):
+    """lv_bag_parse_livox on a serialised CustomMsg (bytes): returns (LivoxView, the records as a LIVOX_RECORD array)"""
+    v = LivoxView()
+    buf = C.create_string_buffer(bytes(msg), len(msg))
+    _check(lib().lv_bag_parse_livox(buf, len(msg), C.byref(v)))
+    off = v.data - C.addressof(buf) if v.n_points else 0
+    return v, np.frombuffer(buf.raw[off:off + v.data_bytes], LIVOX_RECORD).copy()
+
+
+def livox_to_points(records, timebase_ns, tag_reject_mask):
+    """msg2points of a Livox message on the host (records: LIVOX_RECORD array, or its raw bytes): returns (xyz, time, intensity,
+    range, index in the message) of the tag-kept points, in message order"""
+    raw = np.ascontiguousarray(np.frombuffer(np.ascontiguousarray(records).tobytes(), np.uint8))
+    n = len(raw) // 19
+    out = (np.empty((n, 3), np.float32), np.empty(n), np.empty(n, np.float32), np.empty(n, np.float32), np.empty(n, np.int32))
+    m = C.c_int64(0)
+    _check(lib().lv_livox_to_points(raw.ctypes.data_as(C.c_void_p), len(raw), n, C.c_uint64(timebase_ns), int(tag_reject_mask),
+                                    *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
+    return tuple(a[:m.value].copy() for a in out)
 
 
 def init_state_host(params, q_imu=(0, 0, 0, 1)):
@@ -671,6 +708,31 @@ class Localizer:
             for d in bufs:
                 self.device_free(d)
 
+    def process_livox_device(self, d_data, data_bytes, n, timebase_ns, tag_reject_mask, downsample_rate, min_dist, d_xyz, d_time,
+                             d_intensity=None, d_range=None, d_idx=None):
+        """Accumulator::process on the records of a Livox message already in device memory (raw pointers); returns the points kept"""
+        m = C.c_int64(0)
+        _check(self.L.lv_process_livox_device(self.h, C.c_void_p(d_data), int(data_bytes), int(n), C.c_uint64(timebase_ns), int(tag_reject_mask),
+                                              int(downsample_rate), float(min_dist), C.c_void_p(d_xyz), C.c_void_p(d_time),
+                                              C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx), C.byref(m)))
+        return m.value
+
+    def process_livox(self, records, timebase_ns, tag_reject_mask, downsample_rate, min_dist):
+        """Accumulator::process on a Livox message's records (LIVOX_RECORD array): uploads them, returns (xyz, time, intensity, range,
+        index in the message) of the kept points in time order"""
+        raw = np.frombuffer(np.ascontiguousarray(records).tobytes(), np.uint8)
+        n = len(raw) // 19
+        out = (np.empty((n, 3), np.float32), np.empty(n, np.float64), np.empty(n, np.float32), np.empty(n, np.float32),
+               np.empty(n, np.int32))
+        bufs = [self.device_alloc(max(raw.nbytes, 1))] + [self.device_alloc(max(a.nbytes, 1)) for a in out]
+        try:
+            _check(self.L.lv_memcpy_h2d(self.h, bufs[0], raw.ctypes.data_as(C.c_void_p), raw.nbytes))
+            m = self.process_livox_device(bufs[0], raw.nbytes, n, timebase_ns, tag_reject_mask, downsample_rate, min_dist, *bufs[1:])
+            return tuple(self.download(d, a[:m]) for a, d in zip(out, bufs[1:]))
+        finally:
+            for d in bufs:
+                self.device_free(d)
+
     def download(self, d_ptr, out):
         """copy device memory into the contiguous numpy array `out` (its whole size); returns out"""
         if out.nbytes:
@@ -702,6 +764,14 @@ class Localizer:
             self.h, LIDAR_TYPES[lidar], C.byref(layout), C.c_void_p(d_data), int(data_bytes), int(n), int(header_stamp_us),
             int(stamp_beginning), int(offset_beginning), float(full_rotation_time), int(downsample_rate), float(min_dist),
             C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
+            C.c_void_p(d_n_out)))
+
+    def process_livox_device_async(self, d_data, data_bytes, n, timebase_ns, tag_reject_mask, downsample_rate, min_dist, d_xyz, d_time,
+                                   d_n_out, d_intensity=None, d_range=None, d_idx=None):
+        """lv_process_livox_device with the count of kept points written to d_n_out"""
+        return _check(self.L.lv_process_livox_device_async(
+            self.h, C.c_void_p(d_data), int(data_bytes), int(n), C.c_uint64(timebase_ns), int(tag_reject_mask), int(downsample_rate),
+            float(min_dist), C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
             C.c_void_p(d_n_out)))
 
     def compensate_device_async(self, path, Xt2, d_xyz, d_t, d_n, n_max, d_out):

@@ -1658,26 +1658,29 @@ lv_status lv_temporal_downsample(lv_handle h, const float* xyz, int64_t n, int32
 }
 
 /* ---- Accumulator::process ------------------------------------------------------------------------ */
-/* the argument checks and the launches of both forms: d_n_out NULL = the synchronous form (*n_out read back) */
-static lv_status process_cloud_impl(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
-                                    int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
-                                    int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
-                                    int32_t* d_idx, int64_t* n_out, int64_t* d_n_out) {
+/* the argument checks and the launches of both message formats: d_n_out NULL = the synchronous form (*n_out read back).
+ * null_args: a required pointer is NULL (null_what names them); layout_error() runs once the pointers and n are known good;
+ * launch(launches, err) enqueues the pipeline */
+extern "C++" {
+template <class LayoutError, class Launch>
+static lv_status front_end_impl(lv_handle h, const std::string& what, bool null_args, const char* null_what, const uint8_t* d_data,
+                                int64_t data_bytes, int64_t n, int32_t downsample_rate, const CloudOut& o, int64_t* n_out, int64_t* d_n_out,
+                                LayoutError layout_error, Launch launch) {
     /* every check before the first device call */
     if (n_out) *n_out = 0;
-    if (!layout || !d_data || !d_xyz || !d_time || !n_out) { set_error("process cloud: null layout, data, xyz, time or n_out"); return LV_ERR_ARG; }
-    if (n < 0 || n > 0x7fffffff) { set_error("process cloud: n outside [0, 2^31 - 1] (point indices are int32)"); return LV_ERR_ARG; }
-    if (const char* why = cloud_layout_error(type, *layout, n, data_bytes)) { set_error(std::string("process cloud: ") + why); return LV_ERR_ARG; }
+    if (null_args || !n_out) { set_error(what + ": null " + null_what); return LV_ERR_ARG; }
+    if (n < 0 || n > 0x7fffffff) { set_error(what + ": n outside [0, 2^31 - 1] (point indices are int32)"); return LV_ERR_ARG; }
+    if (const char* why = layout_error()) { set_error(what + ": " + why); return LV_ERR_ARG; }
     /* the gather decodes the message while it writes the outputs: an output that overlaps the bytes would be read after it is
      * overwritten */
-    const struct { const void* p; int64_t bytes; } outs[5] = {{d_xyz, 12 * n}, {d_time, 8 * n}, {d_intensity, 4 * n}, {d_range, 4 * n},
-                                                            {d_idx, 4 * n}};
-    for (const auto& o : outs)
-        if (o.p && n > 0 && ranges_overlap(o.p, o.bytes, d_data, data_bytes)) {
-            set_error("process cloud: an output range overlaps the message bytes");
+    const struct { const void* p; int64_t bytes; } outs[5] = {{o.xyz, 12 * n}, {o.time, 8 * n}, {o.intensity, 4 * n}, {o.range, 4 * n},
+                                                            {o.idx, 4 * n}};
+    for (const auto& r : outs)
+        if (r.p && n > 0 && ranges_overlap(r.p, r.bytes, d_data, data_bytes)) {
+            set_error(what + ": an output range overlaps the message bytes");
             return LV_ERR_ARG;
         }
-    if (!h) { set_error("process cloud: null handle"); return LV_ERR_ARG; }
+    if (!h) { set_error(what + ": null handle"); return LV_ERR_ARG; }
     if (cloud_bound(n, downsample_rate) == 0) {                  /* nothing can be kept */
         if (d_n_out) {
             LV_CUDA(cudaSetDevice(h->prm.device));
@@ -1687,19 +1690,32 @@ static lv_status process_cloud_impl(lv_handle h, lv_lidar_type type, const lv_cl
     }
     LV_CUDA(cudaSetDevice(h->prm.device));
     LV_CUDA(ds_reserve(h->ds, n));
-    const CloudArgs a = {d_data, n, *layout, type, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time, downsample_rate, min_dist};
     int launches = 0;
-    LV_CUDA(launch_process_cloud(h->ds, a, CloudOut{d_xyz, d_time, d_intensity, d_range, d_idx}, d_n_out, d_n_out ? &h->d_async->err : nullptr,
-                                 h->stream, &launches));
+    LV_CUDA(launch(&launches, d_n_out ? &h->d_async->err : nullptr));
     h->prof.total_launches += launches;
     if (d_n_out) return LV_OK;
     LV_CUDA(cudaStreamSynchronize(h->stream));
-    if (h->ds.h_count[1]) {
-        set_error("process cloud: a kept point's timestamp is NaN (the time sort has no order for it)");
+    if (h->ds.h_count[1]) {                                       /* PointCloud2 only: a Livox time is never NaN */
+        set_error(what + ": a kept point's timestamp is NaN (the time sort has no order for it)");
         return LV_ERR_ARG;
     }
     *n_out = h->ds.h_count[0];
     return LV_OK;
+}
+}  // extern "C++"
+static lv_status process_cloud_impl(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
+                                    int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
+                                    int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                    int32_t* d_idx, int64_t* n_out, int64_t* d_n_out) {
+    const CloudOut o{d_xyz, d_time, d_intensity, d_range, d_idx};
+    return front_end_impl(
+        h, "process cloud", !layout || !d_data || !d_xyz || !d_time, "layout, data, xyz, time or n_out", d_data, data_bytes, n, downsample_rate,
+        o, n_out, d_n_out, [&] { return cloud_layout_error(type, *layout, n, data_bytes); },
+        [&](int* launches, uint32_t* err) {
+            const CloudArgs a = {d_data, n, *layout, type, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time, downsample_rate,
+                                 min_dist};
+            return launch_process_cloud(h->ds, a, o, d_n_out, err, h->stream, launches);
+        });
 }
 lv_status lv_process_cloud_device(lv_handle h, lv_lidar_type type, const lv_cloud_layout* layout, const uint8_t* d_data, int64_t data_bytes,
                                   int64_t n, uint64_t header_stamp_us, int stamp_beginning, int offset_beginning, double full_rotation_time,
@@ -1716,6 +1732,34 @@ lv_status lv_process_cloud_device_async(lv_handle h, lv_lidar_type type, const l
     if (!d_n_out) { set_error("process cloud: null layout, data, xyz, time or n_out"); return LV_ERR_ARG; }
     return process_cloud_impl(h, type, layout, d_data, data_bytes, n, header_stamp_us, stamp_beginning, offset_beginning, full_rotation_time,
                               downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range, d_idx, &unused, d_n_out);
+}
+
+/* a Livox CustomMsg's records (lv_wire.h): the tag filter, then the decimator on the rank among the tag-kept points */
+static lv_status process_livox_impl(lv_handle h, const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t timebase_ns, uint8_t tag_reject_mask,
+                                    int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                    int32_t* d_idx, int64_t* n_out, int64_t* d_n_out) {
+    const CloudOut o{d_xyz, d_time, d_intensity, d_range, d_idx};
+    return front_end_impl(
+        h, "process livox", !d_data || !d_xyz || !d_time, "data, xyz, time or n_out", d_data, data_bytes, n, downsample_rate, o, n_out, d_n_out,
+        [&] { return livox_layout_error(n, data_bytes, timebase_ns); },
+        [&](int* launches, uint32_t* err) {
+            const LivoxArgs a = {d_data, n, timebase_ns, tag_reject_mask, downsample_rate, min_dist};
+            return launch_process_livox(h->ds, a, o, d_n_out, err, h->stream, launches);
+        });
+}
+lv_status lv_process_livox_device(lv_handle h, const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t timebase_ns, uint8_t tag_reject_mask,
+                                  int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                  int32_t* d_idx, int64_t* n_out) {
+    return process_livox_impl(h, d_data, data_bytes, n, timebase_ns, tag_reject_mask, downsample_rate, min_dist, d_xyz, d_time, d_intensity,
+                              d_range, d_idx, n_out, nullptr);
+}
+lv_status lv_process_livox_device_async(lv_handle h, const uint8_t* d_data, int64_t data_bytes, int64_t n, uint64_t timebase_ns,
+                                        uint8_t tag_reject_mask, int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time,
+                                        float* d_intensity, float* d_range, int32_t* d_idx, int64_t* d_n_out) {
+    int64_t unused = 0;                                           /* the count stays on the device */
+    if (!d_n_out) { set_error("process livox: null data, xyz, time or n_out"); return LV_ERR_ARG; }
+    return process_livox_impl(h, d_data, data_bytes, n, timebase_ns, tag_reject_mask, downsample_rate, min_dist, d_xyz, d_time, d_intensity,
+                              d_range, d_idx, &unused, d_n_out);
 }
 
 /* the deferred errors of the _async calls (AsyncWords::err) and the map's flags; clears the former */

@@ -174,7 +174,7 @@ cudaError_t ds_reserve(DownsampleScratch& s, int64_t n) {
     s.keys64.reset(); s.keys64_sorted.reset();
     s.tmp.reset();
     cudaError_t e;
-    if ((e = s.box.reserve(1)) != cudaSuccess || (e = s.count.reserve(2)) != cudaSuccess || (e = s.h_count.reserve(2)) != cudaSuccess)
+    if ((e = s.box.reserve(1)) != cudaSuccess || (e = s.count.reserve(3)) != cudaSuccess || (e = s.h_count.reserve(2)) != cudaSuccess)
         return e;
     const int64_t cap = n + n / 4 + 1024;
     size_t a = 0, b = 0;
@@ -182,6 +182,9 @@ cudaError_t ds_reserve(DownsampleScratch& s, int64_t n) {
                                     (uint32_t*)nullptr, (int)cap);
     cub::DeviceSelect::Flagged(nullptr, b, cub::CountingInputIterator<int32_t>(0), (const uint8_t*)nullptr, (int32_t*)nullptr,
                                (int*)nullptr, (int)cap);
+    size_t b2 = 0;                            /* the livox front end's second select reads an index array */
+    cub::DeviceSelect::Flagged(nullptr, b2, (const int32_t*)nullptr, (const uint8_t*)nullptr, (int32_t*)nullptr, (int*)nullptr, (int)cap);
+    b = b > b2 ? b : b2;
     size_t c = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, c, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const uint32_t*)nullptr,
                                     (uint32_t*)nullptr, (int)cap);

@@ -199,7 +199,7 @@ struct DownsampleScratch {
     DeviceBuf<int32_t> sel;
     DeviceBuf<uint8_t> tmp;        /* cub's temporary storage: tmp.size() bytes */
     DeviceBuf<GridBox> box;
-    DeviceBuf<int> count;          /* [0] output count, [1] NaN-time flag (lv_cloud.cu) */
+    DeviceBuf<int> count;          /* [0] output count, [1] NaN-time flag, [2] tag-kept count of a livox message (lv_cloud.cu) */
     PinnedBuf<int> h_count;        /* [0] output count, [1] overflow flag (voxel grid) / NaN-time flag (cloud) */
 };
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n);
@@ -240,6 +240,17 @@ int64_t cloud_bound(int64_t n, int rate);
  * kept point's time is NaN (after a stream sync).  d_n_out (may be NULL) receives the count on the device; err (may be NULL)
  * gets kAsyncCloudNaN for a NaN time */
 cudaError_t launch_process_cloud(DownsampleScratch& s, const CloudArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err, cudaStream_t st,
+                                 int* launches);
+/* the same for a livox CustomMsg: the tag filter, then the decimator on the rank among the tag-kept points (lv_wire.h) */
+struct LivoxArgs {
+    const uint8_t* data;       /* the message's 19-byte records (device, any alignment) */
+    int64_t n;
+    uint64_t timebase_ns;
+    uint32_t tag_reject_mask;
+    int32_t rate;
+    double min_dist;
+};
+cudaError_t launch_process_livox(DownsampleScratch& s, const LivoxArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err, cudaStream_t st,
                                  int* launches);
 /* Processor::fill's header stamp (PointCloudProcessor.cpp:125-133): *d_stamp_us = max over the *d_n (clamped to [0, n_max]) times of
  * round(t * 1e6) as uint64 (Conversions::sec2Microsec, Utils.cpp:14-16), 0 for no point.  One launch */

@@ -1,6 +1,6 @@
 /*
- * lv_wire.h — the per-point arithmetic of the LiDAR message, compiled by the host (lv_pointcloud2_to_points) and the device
- * (lv_process_cloud_device, the temporal decimator) alike, so that both give the same bits:
+ * lv_wire.h — the per-point arithmetic of the LiDAR message, compiled by the host (lv_pointcloud2_to_points, lv_livox_to_points)
+ * and the device (lv_process_cloud_device, lv_process_livox_device, the temporal decimator) alike, so that both give the same bits:
  *   PointCloudProcessor::msg2points / get_begin_time   src/Utils/PointCloudProcessor.cpp:24-99
  *   Point(const <driver>::Point&, double time_offset)   src/Objects/Point.cpp:37-111,153-175
  *   Conversions::microsec2Sec / nanosec2Sec             src/Utils/Utils.cpp:18-30
@@ -117,6 +117,34 @@ inline const char* cloud_layout_error(lv_lidar_type type, const lv_cloud_layout&
     for (int k = 0; k < 6; ++k)
         if (offs[k] < 0 || (int64_t)offs[k] + szs[k] > L.point_step) return "a field of the layout lies outside point_step";
     if (n > data_bytes / L.point_step) return "data_bytes is too short for n points of point_step bytes";
+    return nullptr;
+}
+
+/* ---- livox_ros_driver(2)/CustomMsg: one uint64 time base (ns) per message, then packed 19-byte records
+ *   uint32 offset_time (ns after timebase) | float32 x | float32 y | float32 z | uint8 reflectivity | uint8 tag | uint8 line
+ * A record starts at data + 19 i, at any address. */
+enum { kLivoxRecord = 19 };
+/* the largest time base whose sum with any uint32 offset still fits a uint64 */
+constexpr uint64_t kLivoxTimebaseMax = 0xFFFFFFFF00000000ull;
+
+LV_HD const uint8_t* livox_point(const uint8_t* data, int64_t i) { return data + (uint64_t)i * (uint64_t)kLivoxRecord; }
+LV_HD uint32_t livox_tag(const uint8_t* p) { return wire_u8(p + 17); }
+LV_HD float livox_reflectivity(const uint8_t* p) { return (float)wire_u8(p + 16); }
+/* total = timebase + offset_time (ns, uint64), then seconds as Conversions::nanosec2Sec (Utils.cpp:25-30) but with a 64-bit
+ * quotient: the reference's int cast would truncate epoch seconds */
+LV_HD double livox_time(uint64_t timebase, const uint8_t* p) {
+    const uint64_t total = timebase + (uint64_t)wire_u32(p);
+    const uint64_t order = 1000000000ull;
+    return dadd((double)(int64_t)(total / order), dmul((double)(total % order), 1e-9));
+}
+/* the tag filter of msg2points: bits of the tag set in the mask drop the point (0 keeps every point) */
+LV_HD bool livox_tag_keep(const uint8_t* p, uint32_t tag_reject_mask) { return (livox_tag(p) & tag_reject_mask) == 0; }
+
+/* NULL when n records fit data_bytes and the time base cannot wrap, else what is wrong */
+inline const char* livox_layout_error(int64_t n, int64_t data_bytes, uint64_t timebase_ns) {
+    if (n < 0 || data_bytes < 0) return "negative point count or data length";
+    if (n > data_bytes / kLivoxRecord) return "data_bytes is too short for n records of 19 bytes";
+    if (timebase_ns > kLivoxTimebaseMax) return "timebase above 2^64 - 2^32 ns (timebase + offset_time could wrap)";
     return nullptr;
 }
 

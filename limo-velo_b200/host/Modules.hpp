@@ -265,6 +265,25 @@ class Accumulator {
         if (m.n > 0)
             check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.n), "Accumulator::receive_lidar_device_full");
     }
+    /* receive_lidar_device for a Livox CustomMsg (lv_process_livox_device_async: tag filter, decimation on the rank among the tag-kept
+     * points, time sort); the records in device memory, e.g. lv_bag_parse_livox's view uploaded */
+    struct DeviceLivoxMessage {
+        const uint8_t* d_data; int64_t data_bytes, n; uint64_t timebase_ns; uint8_t tag_reject_mask; int32_t downsample_rate; double min_dist;
+    };
+    void receive_livox_device(const DeviceLivoxMessage& m, float* d_xyz, double* d_time, int64_t* d_n) {
+        check(lv_process_livox_device_async(ctx->h, m.d_data, m.data_bytes, m.n, m.timebase_ns, m.tag_reject_mask, m.downsample_rate, m.min_dist,
+                                            d_xyz, d_time, nullptr, nullptr, nullptr, d_n),
+              "Accumulator::receive_livox_device");
+        if (m.n > 0) check(lv_lidar_push_device_async(ctx->h, d_xyz, d_time, d_n, m.n), "Accumulator::receive_livox_device");
+    }
+    /* the same with whole Points: intensity = reflectivity, range = |p| */
+    void receive_livox_device_full(const DeviceLivoxMessage& m, float* d_xyz, double* d_time, float* d_intensity, float* d_range, int64_t* d_n) {
+        check(lv_process_livox_device_async(ctx->h, m.d_data, m.data_bytes, m.n, m.timebase_ns, m.tag_reject_mask, m.downsample_rate, m.min_dist,
+                                            d_xyz, d_time, d_intensity, d_range, nullptr, d_n),
+              "Accumulator::receive_livox_device_full");
+        if (m.n > 0)
+            check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.n), "Accumulator::receive_livox_device_full");
+    }
     /* Accumulator::get_points(t1, t2) (Accumulator.hpp:61-74) into device buffers of n_max points; the count goes to *d_n_out */
     void get_points_device(double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* d_n_out) {
         check(lv_lidar_get_points_device_async(ctx->h, t1, t2, d_xyz, d_time, n_max, d_n_out), "Accumulator::get_points_device");

@@ -19,6 +19,7 @@
  * fields the LiDAR's point struct uses (include/Headers/Common.hpp:109-221: velodyne x y z intensity time(f32); hesai
  * x y z intensity(u8) timestamp(f64); ouster x y z reflectivity(u16) t(u32) range(u32); custom like hesai with f32
  * intensity), ready for lv_pointcloud2_to_points; sensor_msgs/Imu -> stamp, orientation, angular velocity, acceleration.
+ * Livox sensors publish livox_ros_driver/CustomMsg instead of PointCloud2: lv_bag_parse_livox -> a view of its 19-byte records.
  * Everything is host code: a sweep is a few MB per 100 ms.
  */
 #include <stdio.h>
@@ -282,6 +283,31 @@ lv_status lv_bag_parse_imu(const uint8_t* data, int64_t size, lv_imu_sample* out
     for (int i = 0; i < 3; ++i) out->linear_acceleration[i] = r.f64();
     r.take(72);
     return r.ok ? LV_OK : LV_ERR_IO;
+}
+
+lv_status lv_bag_parse_livox(const uint8_t* data, int64_t size, lv_livox_view* out) {
+    if (!data || !out || size < 0) return LV_ERR_ARG;
+    memset(out, 0, sizeof(*out));
+    Rd r(data, size);
+    r.u32();                                          /* std_msgs/Header: seq, stamp, frame_id */
+    const uint32_t sec = r.u32(), nsec = r.u32();
+    r.str();
+    const uint8_t* tb = r.take(8);
+    const uint32_t point_num = r.u32();
+    const uint8_t lidar_id = r.u8();
+    r.take(3);                                        /* uint8[3] rsvd: a fixed-size array, no length prefix */
+    const uint32_t count = r.u32();                   /* CustomPoint[] */
+    const uint8_t* recs = r.take((int64_t)count * lv::kLivoxRecord);
+    if (!r.ok || r.at != size || point_num != count) return LV_ERR_ARG;
+    out->stamp_sec = sec;
+    out->stamp_nsec = nsec;
+    out->timebase = (uint64_t)rd32(tb) | (uint64_t)rd32(tb + 4) << 32;
+    out->point_num = point_num;
+    out->lidar_id = lidar_id;
+    out->n_points = count;
+    out->data = recs;
+    out->data_bytes = (int64_t)count * lv::kLivoxRecord;
+    return LV_OK;
 }
 
 /* lv_pointcloud2_to_points with the bounds pcl::fromROSMsg gets from the message itself (lv::cloud_layout_error, which

@@ -5,7 +5,8 @@
  *   Conversions::microsec2Sec / nanosec2Sec                         src/Utils/Utils.cpp:18-30
  *   PointCloudProcessor::sort_points                                src/Utils/PointCloudProcessor.cpp:114-123
  * One pass over the message bytes per sweep (a few MB); the per-point arithmetic is csrc/lv_wire.h, which
- * lv_process_cloud_device (csrc/lv_cloud.cu) runs on the device.
+ * lv_process_cloud_device (csrc/lv_cloud.cu) runs on the device.  lv_livox_to_points is the same for a Livox CustomMsg
+ * (lv_process_livox_device on the device).
  */
 #include <algorithm>
 #include <numeric>
@@ -31,6 +32,26 @@ lv_status lv_pointcloud2_to_points(lv_lidar_type type, const lv_cloud_layout* la
         if (intensity) intensity[i] = lv::wire_intensity(type, L, p);
         if (range) range[i] = lv::wire_range(type, L, p, x, y, z);
     }
+    return LV_OK;
+}
+
+lv_status lv_livox_to_points(const uint8_t* data, int64_t data_bytes, int64_t n, uint64_t timebase_ns, uint8_t tag_reject_mask,
+                             float* xyz, double* time, float* intensity, float* range, int32_t* idx, int64_t* n_out) {
+    if (n_out) *n_out = 0;
+    if (!data || !xyz || !time || !n_out || n > 0x7fffffff || lv::livox_layout_error(n, data_bytes, timebase_ns)) return LV_ERR_ARG;
+    int64_t m = 0;
+    for (int64_t i = 0; i < n; ++i) {
+        const uint8_t* p = lv::livox_point(data, i);
+        if (!lv::livox_tag_keep(p, tag_reject_mask)) continue;
+        const float x = lv::wire_f32(p + 4), y = lv::wire_f32(p + 8), z = lv::wire_f32(p + 12);
+        xyz[3 * m] = x; xyz[3 * m + 1] = y; xyz[3 * m + 2] = z;
+        time[m] = lv::livox_time(timebase_ns, p);
+        if (intensity) intensity[m] = lv::livox_reflectivity(p);
+        if (range) range[m] = lv::wire_norm(x, y, z);
+        if (idx) idx[m] = (int32_t)i;
+        ++m;
+    }
+    *n_out = m;
     return LV_OK;
 }
 
