@@ -638,6 +638,36 @@ struct lv_lidar_info {
 /* the buffer's fill state; synchronises */
 lv_status lv_lidar_info(lv_handle h, struct lv_lidar_info* out);
 
+/* ---- several LiDARs into one buffer: the time-ordered merge ----------------------------------------------------------------------
+ * The push keeps arrival order, so messages of two sensors whose time spans overlap leave the buffer unsorted, and get's binary
+ * search then answers from whichever points it probes.  The merge puts each message where its times belong instead, after moving
+ * its points into the primary LiDAR's frame (the frame I_Rotation_L / I_Translation_L describe).  Let L be the live points, oldest
+ * first, and B the message (time-sorted, as the message front end leaves it).  The split s is one past the newest live point whose
+ * time is <= B[0].time, and T_tail the live points after it.  When T_tail and B are each non-decreasing in time with no NaN, the
+ * points from s on become std::merge(T_tail, B) by time, buffered points first on equal times, and the points before s do not move.
+ * A message that starts no earlier than the newest live point is exactly the push: the same slots, bits and counters.  Otherwise
+ * (a NaN time, a batch that is not sorted, or T_tail left unsorted by an earlier push) the message is appended as the push does,
+ * and lv_async_status reports that the buffer is no longer time-ordered.  An empty message changes nothing.
+ * Each point is written as rt_apply(T, p) (RotTransl * Point in fp32, unfused); T = NULL writes the points bit for bit unchanged.
+ * Intensity and range move with their points; range stays the sensor-frame value the front end computed (|p| in the sensor's
+ * frame, or the Ouster's range field).  Deferred errors, each leaving the buffer unchanged: T_tail larger than the merge reserve,
+ * and points that do not fit the capacity.  Three launches per call whatever the overlap; no host wait.
+ * Argument errors are LV_ERR_ARG before any device work, also with a null handle: null pointers, n_max outside [1, 2^31 - 1], a
+ * non-finite entry of T, input ranges that overlap each other or the buffer, a merge before lv_lidar_reserve and
+ * lv_lidar_reserve_merge, and a _full merge on a buffer without lanes. */
+/* room for `overlap_points` (1 .. 2^30) buffered points that one merge may move (T_tail); the scratch has lanes when the buffer has
+ * them, and gains them when lv_lidar_reserve_full adds them.  LV_ERR_CAPACITY when the allocation fails (merges are refused until a
+ * reserve succeeds).  Synchronises. */
+lv_status lv_lidar_reserve_merge(lv_handle h, int64_t overlap_points);
+/* merge the *d_n points (clamped to [0, n_max]) of d_xyz (n x 3) / d_time; T: 12 host floats, R row-major then t, mapping the
+ * sensor's frame into the primary LiDAR's frame (L0_T_Lk), or NULL.  On a buffer with lanes the points get intensity 0 and range 0,
+ * as with the push. */
+lv_status lv_lidar_merge_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max,
+                                      const float* T);
+/* the same with the points' intensity and range (n_max each); a buffer reserved with lv_lidar_reserve_full */
+lv_status lv_lidar_merge_full_device_async(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity, const float* d_range,
+                                           const int64_t* d_n, int64_t n_max, const float* T);
+
 /* ---- rosbag reader (format 2.0; replaces roscpp / `rosbag play` in front of Accumulator::receive_lidar / receive_imu,
  * src/main.cpp:27-39, src/Modules/Accumulator.cpp:39-60).  Sequential read of uncompressed bags (bz2 / lz4 chunks are
  * refused with LV_ERR_IO: `rosbag decompress` first).  Host code.                                                       */

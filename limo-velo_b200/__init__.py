@@ -209,6 +209,10 @@ def lib():
                                               C.POINTER(i64)]
         L.lv_process_livox_device_async.argtypes = [vp, vp, i64, i64, C.c_uint64, C.c_uint8, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
         L.lv_bag_parse_livox.argtypes = [vp, i64, C.POINTER(LivoxView)]
+    if hasattr(L, "lv_lidar_reserve_merge"):   # the time-ordered merge of several LiDARs; absent from older builds
+        L.lv_lidar_reserve_merge.argtypes = [vp, i64]
+        L.lv_lidar_merge_device_async.argtypes = [vp, vp, vp, vp, i64, fp]
+        L.lv_lidar_merge_full_device_async.argtypes = [vp, vp, vp, vp, vp, vp, i64, fp]
     if hasattr(L, "lv_prelocalize"):   # start pose search and PCD files; absent from older builds
         L.lv_preloc_count.argtypes = [C.POINTER(PrelocParams)]
         L.lv_preloc_count.restype = i64
@@ -370,6 +374,13 @@ class CloudLayout(C.Structure):
 
 
 LIDAR_TYPES = {"velodyne": 0, "hesai": 1, "ouster": 2, "custom": 3}
+
+
+def _transform12(T):
+    """a rigid transform as lv_lidar_merge_device_async takes it: None, or 12 floats (R row-major, then t)"""
+    if T is None:
+        return None
+    return (C.c_float * 12)(*np.ascontiguousarray(T, np.float32).reshape(12).tolist())
 
 
 def cloud_layout(lidar, dtype):
@@ -835,6 +846,21 @@ class Localizer:
         """lidar_push_async with the points' intensity and range (a buffer reserved with lidar_reserve_full)"""
         return _check(self.L.lv_lidar_push_full_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity),
                                                              C.c_void_p(d_range), C.c_void_p(d_n), int(n_max)))
+
+    def lidar_reserve_merge(self, overlap_points):
+        """room for `overlap_points` buffered points that one merge may move; synchronises"""
+        return _check(self.L.lv_lidar_reserve_merge(self.h, int(overlap_points)))
+
+    def lidar_merge_async(self, d_xyz, d_time, d_n, n_max, T=None):
+        """lv_lidar_merge_device_async: the *d_n points by time into the buffer, through T (12 floats: R row-major, then t) from the
+        sensor's frame into the primary LiDAR's, or unchanged (T None)"""
+        return _check(self.L.lv_lidar_merge_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_n), int(n_max),
+                                                         _transform12(T)))
+
+    def lidar_merge_full_async(self, d_xyz, d_time, d_intensity, d_range, d_n, n_max, T=None):
+        """lidar_merge_async with the points' intensity and range (a buffer reserved with lidar_reserve_full)"""
+        return _check(self.L.lv_lidar_merge_full_device_async(self.h, C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity),
+                                                              C.c_void_p(d_range), C.c_void_p(d_n), int(n_max), _transform12(T)))
 
     def lidar_get_points_full_async(self, t1, t2, d_xyz, d_time, d_intensity, d_range, n_max, d_n_out):
         """lidar_get_points_async with the window's intensity and range"""

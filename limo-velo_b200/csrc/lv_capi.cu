@@ -1776,8 +1776,12 @@ lv_status lv_async_status(lv_handle h) {
         if (err & kAsyncCloudNaN) msg += "process cloud: a kept point's timestamp is NaN (the time sort has no order for it); ";
         if (err & kAsyncDeskewPath) msg += "compensate: a timestamp lies outside the path or the points are not time-sorted; ";
         if (err & kAsyncCount) msg += "a device point count lies outside [0, n_max] (clamped); ";
-        if (err & kAsyncLidarFull) msg += "lidar push: the points do not fit the buffer's capacity (nothing appended; lv_lidar_reserve); ";
+        if (err & kAsyncLidarFull) msg += "lidar push or merge: the points do not fit the buffer's capacity (nothing appended; lv_lidar_reserve); ";
         if (err & kAsyncLidarWindow) msg += "lidar get points: the window holds more than n_max points (count 0); ";
+        if (err & kAsyncLidarUnsorted)
+            msg += "lidar merge: the message or the buffered points after its first time are not time-ordered (appended as a push does); ";
+        if (err & kAsyncLidarOverlap)
+            msg += "lidar merge: the message reaches back over more buffered points than the merge reserve (nothing merged; lv_lidar_reserve_merge); ";
         msg.resize(msg.size() - 2);
         set_error(msg);
         return LV_ERR_ARG;
@@ -1790,7 +1794,11 @@ static bool overlaps_lidar(const lv_context* h, const void* p, int64_t bytes) {
     const LidarRing& r = h->lidar;
     return ranges_overlap(p, bytes, r.xyz, 12 * r.cap) || ranges_overlap(p, bytes, r.time, 8 * r.cap) ||
            ranges_overlap(p, bytes, r.words, (int64_t)sizeof(LidarWords)) ||
-           (r.intensity && (ranges_overlap(p, bytes, r.intensity, 4 * r.cap) || ranges_overlap(p, bytes, r.range, 4 * r.cap)));
+           (r.intensity && (ranges_overlap(p, bytes, r.intensity, 4 * r.cap) || ranges_overlap(p, bytes, r.range, 4 * r.cap))) ||
+           ranges_overlap(p, bytes, r.merge_xyz, 4 * (int64_t)r.merge_xyz.size()) ||
+           ranges_overlap(p, bytes, r.merge_time, 8 * (int64_t)r.merge_time.size()) ||
+           ranges_overlap(p, bytes, r.merge_intensity, 4 * (int64_t)r.merge_intensity.size()) ||
+           ranges_overlap(p, bytes, r.merge_range, 4 * (int64_t)r.merge_range.size());
 }
 /* lv_lidar_reserve (lanes: keep the ring's) and lv_lidar_reserve_full (lanes: always); `what` names the call in the messages */
 static lv_status lidar_resize(lv_handle h, int64_t capacity, bool full, const char* what) {
@@ -1817,7 +1825,9 @@ static lv_status lidar_resize(lv_handle h, int64_t capacity, bool full, const ch
     /* the new arrays are allocated while the old ones still hold the live points */
     DeviceBuf<float> xyz, intensity, range;
     DeviceBuf<double> time;
-    cudaError_t e = xyz.reserve(3 * (size_t)capacity);
+    cudaError_t e = lanes && r.merge_cap ? r.merge_intensity.reserve(r.merge_cap) : cudaSuccess;   /* the merge scratch gains lanes too */
+    if (e == cudaSuccess && lanes && r.merge_cap) e = r.merge_range.reserve(r.merge_cap);
+    if (e == cudaSuccess) e = xyz.reserve(3 * (size_t)capacity);
     if (e == cudaSuccess) e = time.reserve(capacity);
     if (e == cudaSuccess && lanes) e = intensity.reserve(capacity);
     if (e == cudaSuccess && lanes) e = range.reserve(capacity);
@@ -1837,14 +1847,54 @@ static lv_status lidar_resize(lv_handle h, int64_t capacity, bool full, const ch
 }
 lv_status lv_lidar_reserve(lv_handle h, int64_t capacity) { return lidar_resize(h, capacity, false, "lidar reserve"); }
 lv_status lv_lidar_reserve_full(lv_handle h, int64_t capacity) { return lidar_resize(h, capacity, true, "lidar reserve full"); }
-/* the checks after the null-pointer check and the launch of both pushes: intensity / range NULL = the plain push */
+/* lv_lidar_reserve_merge: the overlap scratch of the merge (with lanes when the ring has them); the stream is drained first, since
+ * an enqueued merge may still read the old scratch */
+lv_status lv_lidar_reserve_merge(lv_handle h, int64_t overlap_points) {
+    if (overlap_points < 1 || overlap_points > kLidarMaxCapacity) { set_error("lidar reserve merge: overlap outside [1, 2^30]"); return LV_ERR_ARG; }
+    if (!h) { set_error("lidar reserve merge: null handle"); return LV_ERR_ARG; }
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    LidarRing& r = h->lidar;
+    r.merge_cap = 0;                                              /* until every array fits: a failure leaves merges refused */
+    cudaError_t e = r.merge_xyz.reserve(3 * (size_t)overlap_points);
+    if (e == cudaSuccess) e = r.merge_time.reserve(overlap_points);
+    if (e == cudaSuccess && r.intensity) e = r.merge_intensity.reserve(overlap_points);
+    if (e == cudaSuccess && r.intensity) e = r.merge_range.reserve(overlap_points);
+    if (e != cudaSuccess) {
+        set_error(std::string("lidar reserve merge: ") + cudaGetErrorString(e));
+        return LV_ERR_CAPACITY;
+    }
+    r.merge_cap = overlap_points;
+    return LV_OK;
+}
+/* the checks after the null-pointer check and the launch of both pushes and both merges: intensity / range NULL = the plain form;
+ * merge: the time-ordered merge through the 12 floats of T (NULL: no transform) */
 static lv_status lidar_push_impl(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity, const float* d_range,
-                                 const int64_t* d_n, int64_t n_max, const char* what) {
+                                 const int64_t* d_n, int64_t n_max, const char* what, bool merge = false, const float* T = nullptr) {
     const std::string w(what);
     if (!n_max_ok(what, n_max)) return LV_ERR_ARG;
+    Rt32 rt{};
+    if (merge) {
+        for (int k = 0; T && k < 12; ++k)
+            if (!std::isfinite(T[k])) { set_error(w + ": a transform entry is not finite"); return LV_ERR_ARG; }
+        if (T) {
+            memcpy(rt.R, T, sizeof(rt.R));
+            memcpy(rt.t, T + 9, sizeof(rt.t));
+        }
+        /* the split kernel reads the times and the count while the write kernel reads the points: they must be distinct arrays */
+        const void* const in[5] = {d_xyz, d_time, d_n, d_intensity, d_range};
+        const int64_t bytes[5] = {12 * n_max, 8 * n_max, 8, 4 * n_max, 4 * n_max};
+        for (int a = 1; a < 5; ++a)
+            for (int b = 0; b < a; ++b)
+                if (in[a] && in[b] && ranges_overlap(in[a], bytes[a], in[b], bytes[b])) {
+                    set_error(w + ": the input ranges overlap");
+                    return LV_ERR_ARG;
+                }
+    }
     if (!h) { set_error(w + ": null handle"); return LV_ERR_ARG; }
     if (!h->lidar.cap) { set_error(w + ": the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
     if (d_intensity && !h->lidar.intensity) { set_error(w + ": the buffer has no attribute lanes (lv_lidar_reserve_full first)"); return LV_ERR_ARG; }
+    if (merge && !h->lidar.merge_cap) { set_error(w + ": the buffer has no merge reserve (lv_lidar_reserve_merge first)"); return LV_ERR_ARG; }
     /* the kernel reads the count and the points while it writes the buffer */
     if (overlaps_lidar(h, d_xyz, 12 * n_max) || overlaps_lidar(h, d_time, 8 * n_max) || overlaps_lidar(h, d_n, 8) ||
         (d_intensity && (overlaps_lidar(h, d_intensity, 4 * n_max) || overlaps_lidar(h, d_range, 4 * n_max)))) {
@@ -1853,9 +1903,25 @@ static lv_status lidar_push_impl(lv_handle h, const float* d_xyz, const double* 
     }
     LV_CUDA(cudaSetDevice(h->prm.device));
     int launches = 0;
-    LV_CUDA(launch_lidar_push(h->lidar, d_xyz, d_time, d_n, n_max, &h->d_async->err, h->stream, &launches, d_intensity, d_range));
+    if (merge)
+        LV_CUDA(launch_lidar_merge(h->lidar, d_xyz, d_time, d_n, n_max, T != nullptr, rt, &h->d_async->err, h->stream, &launches, d_intensity,
+                                   d_range));
+    else
+        LV_CUDA(launch_lidar_push(h->lidar, d_xyz, d_time, d_n, n_max, &h->d_async->err, h->stream, &launches, d_intensity, d_range));
     h->prof.total_launches += launches;
     return LV_OK;
+}
+lv_status lv_lidar_merge_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max, const float* T) {
+    if (!d_xyz || !d_time || !d_n) { set_error("lidar merge: null xyz, time or count"); return LV_ERR_ARG; }
+    return lidar_push_impl(h, d_xyz, d_time, nullptr, nullptr, d_n, n_max, "lidar merge", true, T);
+}
+lv_status lv_lidar_merge_full_device_async(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity, const float* d_range,
+                                           const int64_t* d_n, int64_t n_max, const float* T) {
+    if (!d_xyz || !d_time || !d_intensity || !d_range || !d_n) {
+        set_error("lidar merge full: null xyz, time, intensity, range or count");
+        return LV_ERR_ARG;
+    }
+    return lidar_push_impl(h, d_xyz, d_time, d_intensity, d_range, d_n, n_max, "lidar merge full", true, T);
 }
 lv_status lv_lidar_push_device_async(lv_handle h, const float* d_xyz, const double* d_time, const int64_t* d_n, int64_t n_max) {
     if (!d_xyz || !d_time || !d_n) { set_error("lidar push: null xyz, time or count"); return LV_ERR_ARG; }

@@ -20,7 +20,8 @@ enum { kNumSMs = 132 };
 
 /* The stream-ordered (_async) entry points report errors through one device word of the handle, read and cleared by
  * lv_async_status.  Bits: */
-enum : uint32_t { kAsyncCloudNaN = 1u, kAsyncDeskewPath = 2u, kAsyncCount = 4u, kAsyncLidarFull = 8u, kAsyncLidarWindow = 16u };
+enum : uint32_t { kAsyncCloudNaN = 1u, kAsyncDeskewPath = 2u, kAsyncCount = 4u, kAsyncLidarFull = 8u, kAsyncLidarWindow = 16u,
+                  kAsyncLidarUnsorted = 32u, kAsyncLidarOverlap = 64u };
 /* device words of the async tick: the deferred errors and what lv_correct_device_async decided */
 struct AsyncWords {
     uint32_t err;              /* kAsync* bits since the last lv_async_status              */
@@ -268,7 +269,11 @@ struct LidarWords {
     int64_t head, tail;        /* live positions [head, tail); position p in slot p % cap          */
     int64_t window;            /* points the last get's window holds (also when above its n_max)    */
     int64_t count;             /* points the last get wrote (0 when the window was above n_max)     */
-    uint32_t ticket;           /* blocks of a push that have finished                               */
+    uint32_t ticket;           /* blocks of a push or of a merge kernel that have finished          */
+    uint32_t merge_bad;        /* a block of the merge's split kernel found T_tail or B out of order */
+    int64_t merge_split;       /* the last merge's split s, its point count and its mode (kLidarMerge*) */
+    int64_t merge_n;
+    uint32_t merge_mode;
     uint32_t pad;
 };
 struct LidarRing {
@@ -279,6 +284,12 @@ struct LidarRing {
     int64_t cap = 0;           /* 0: not reserved yet */
     DeviceBuf<LidarWords> words;
     PinnedBuf<LidarWords> h_words;
+    /* the merge's overlap scratch (lv_lidar_reserve_merge): T_tail is staged here before the merge overwrites it */
+    DeviceBuf<float> merge_xyz;        /* merge_cap x 3 */
+    DeviceBuf<double> merge_time;      /* merge_cap     */
+    DeviceBuf<float> merge_intensity;  /* merge_cap, when the ring has lanes */
+    DeviceBuf<float> merge_range;
+    int64_t merge_cap = 0;     /* 0: no merge before lv_lidar_reserve_merge */
 };
 /* push *d_n (clamped to [0, n_max]) points; kAsyncLidarFull and nothing appended when they do not fit.  On a ring with lanes the
  * points' intensity and range go with them (NULL: 0) */
@@ -289,6 +300,13 @@ cudaError_t launch_lidar_push(const LidarRing& r, const float* xyz, const double
  * only): the window's lanes too */
 cudaError_t launch_lidar_get(const LidarRing& r, double t1, double t2, float* xyz, double* time, int64_t n_max, int64_t* d_n_out, uint32_t* err,
                              cudaStream_t st, int* launches, float* intensity = nullptr, float* range = nullptr);
+/* merge *d_n (clamped to [0, n_max]) time-ordered points into the ring by time (lv_lidar_buffer.h), each through T when
+ * `transform`: three launches whatever the overlap, the counts and the decision on the device.  Unsorted input is appended with
+ * kAsyncLidarUnsorted; an overlap above merge_cap (kAsyncLidarOverlap) or points that do not fit (kAsyncLidarFull) change nothing.
+ * intensity / range as in launch_lidar_push */
+cudaError_t launch_lidar_merge(const LidarRing& r, const float* xyz, const double* time, const int64_t* d_n, int64_t n_max, bool transform,
+                               const Rt32& T, uint32_t* err, cudaStream_t st, int* launches, const float* intensity = nullptr,
+                               const float* range = nullptr);
 cudaError_t launch_lidar_clear(const LidarRing& r, double t, cudaStream_t st, int* launches);
 /* copy the `live` live points of `from` into the arrays of a ring of capacity cap (the counters stay as they are); intensity /
  * range non-NULL: into those lanes too (0 where `from` has none) */

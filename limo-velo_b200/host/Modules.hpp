@@ -284,6 +284,41 @@ class Accumulator {
         if (m.n > 0)
             check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.n), "Accumulator::receive_livox_device_full");
     }
+    /* Several LiDARs: the same calls with the sensor's extrinsic L0_T_Lk (12 floats, R row-major then t: its frame into the primary
+     * LiDAR's, nullptr for the primary itself) merge the message by time instead of pushing it (lv_lidar_merge_device_async), so
+     * the buffer stays time-ordered when the sensors' messages overlap.  Needs lv_lidar_reserve_merge on the context's handle. */
+    void receive_lidar_device(const DeviceMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, int64_t* d_n) {
+        check(lv_process_cloud_device_async(ctx->h, m.type, m.layout, m.d_data, m.data_bytes, m.n, m.stamp_us, m.stamp_beginning,
+                                            m.offset_beginning, m.full_rotation_time, m.downsample_rate, m.min_dist, d_xyz, d_time,
+                                            nullptr, nullptr, nullptr, d_n),
+              "Accumulator::receive_lidar_device");
+        if (m.n > 0) check(lv_lidar_merge_device_async(ctx->h, d_xyz, d_time, d_n, m.n, L0_T_Lk), "Accumulator::receive_lidar_device");
+    }
+    void receive_lidar_device_full(const DeviceMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, float* d_intensity,
+                                   float* d_range, int64_t* d_n) {
+        check(lv_process_cloud_device_async(ctx->h, m.type, m.layout, m.d_data, m.data_bytes, m.n, m.stamp_us, m.stamp_beginning,
+                                            m.offset_beginning, m.full_rotation_time, m.downsample_rate, m.min_dist, d_xyz, d_time,
+                                            d_intensity, d_range, nullptr, d_n),
+              "Accumulator::receive_lidar_device_full");
+        if (m.n > 0)
+            check(lv_lidar_merge_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.n, L0_T_Lk),
+                  "Accumulator::receive_lidar_device_full");
+    }
+    void receive_livox_device(const DeviceLivoxMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, int64_t* d_n) {
+        check(lv_process_livox_device_async(ctx->h, m.d_data, m.data_bytes, m.n, m.timebase_ns, m.tag_reject_mask, m.downsample_rate, m.min_dist,
+                                            d_xyz, d_time, nullptr, nullptr, nullptr, d_n),
+              "Accumulator::receive_livox_device");
+        if (m.n > 0) check(lv_lidar_merge_device_async(ctx->h, d_xyz, d_time, d_n, m.n, L0_T_Lk), "Accumulator::receive_livox_device");
+    }
+    void receive_livox_device_full(const DeviceLivoxMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, float* d_intensity,
+                                   float* d_range, int64_t* d_n) {
+        check(lv_process_livox_device_async(ctx->h, m.d_data, m.data_bytes, m.n, m.timebase_ns, m.tag_reject_mask, m.downsample_rate, m.min_dist,
+                                            d_xyz, d_time, d_intensity, d_range, nullptr, d_n),
+              "Accumulator::receive_livox_device_full");
+        if (m.n > 0)
+            check(lv_lidar_merge_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.n, L0_T_Lk),
+                  "Accumulator::receive_livox_device_full");
+    }
     /* Accumulator::get_points(t1, t2) (Accumulator.hpp:61-74) into device buffers of n_max points; the count goes to *d_n_out */
     void get_points_device(double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* d_n_out) {
         check(lv_lidar_get_points_device_async(ctx->h, t1, t2, d_xyz, d_time, n_max, d_n_out), "Accumulator::get_points_device");
