@@ -264,6 +264,17 @@ static bool handle_ok(const char* what, const lv_context* h, int64_t n_max) {
 static bool ranges_overlap(const void* a, int64_t a_bytes, const void* b, int64_t b_bytes) {
     return (uintptr_t)a < (uintptr_t)b + (uintptr_t)b_bytes && (uintptr_t)b < (uintptr_t)a + (uintptr_t)a_bytes;
 }
+struct ByteRange {
+    const void* p;
+    int64_t bytes;
+};
+/* two of the n ranges share a byte, NULL pointers skipped; the first `shared` ranges may share bytes with each other */
+static bool any_ranges_overlap(const ByteRange* r, int n, int shared = 0) {
+    for (int b = shared > 1 ? shared : 1; b < n; ++b)
+        for (int a = 0; a < b; ++a)
+            if (r[a].p && r[b].p && ranges_overlap(r[a].p, r[a].bytes, r[b].p, r[b].bytes)) return true;
+    return false;
+}
 
 extern "C" {
 
@@ -887,6 +898,19 @@ static lv_status enqueue_update_kernels(lv_context* h, const float* d_xyz, int64
     return LV_OK;
 }
 
+/* settles map_unknown (an async first build the gate may have left without points) from the map counters, which are fetched
+ * first unless they are already on the host (on_host) */
+static lv_status settle_map_unknown(lv_context* h, bool on_host) {
+    if (!h->map_unknown) return LV_OK;
+    if (!on_host) {
+        LV_CUDA(map_fetch_counters(h->map, h->stream));
+        LV_CUDA(cudaStreamSynchronize(h->stream));
+    }
+    if ((int32_t)h->map.h_counters[kCtrPoints] == 0) h->map.empty = true;
+    h->map_unknown = false;
+    return LV_OK;
+}
+
 static lv_status fetch_results(lv_context* h) {
     LV_CUDA(cudaMemcpyAsync(h->h_ctrl, h->d_ctrl, sizeof(UpdateCtrl), cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(map_fetch_counters(h->map, h->stream));       /* 64 bytes: the map's error flags ride along */
@@ -899,10 +923,7 @@ static lv_status fetch_results(lv_context* h) {
         if (h->h_async->time_set) h->last_time_updated = h->h_async->time_updated;
         h->time_pending = false;
     }
-    if (h->map_unknown) {                                 /* the gate left the async build without a point: no map yet */
-        if ((int32_t)h->map.h_counters[kCtrPoints] == 0) h->map.empty = true;
-        h->map_unknown = false;
-    }
+    settle_map_unknown(h, true);                          /* LV_OK: the counters came with the results */
     const UpdateCtrl* c = h->h_ctrl;
     memcpy(h->x, c->x, sizeof(h->x));
     /* a gated update (LV_TOO_FEW_POINTS, or LV_EMPTY_MAP found on the device) leaves P as it was on the device, which may be
@@ -1094,7 +1115,7 @@ lv_status lv_last_neighbours(lv_handle h, int64_t n, int32_t* nn_idx) {
     return LV_OK;
 }
 
-/* ---- start pose in a saved map (lv_prelocalize) ---------------------------------------------- */
+/* ---- start pose in a saved map (lv_prelocalize, and the host path both searches share) -------- */
 /* NULL when p is valid (I, K and the candidate count filled in), else what is wrong with it */
 static const char* preloc_params_error(const lv_preloc_params* p, int64_t* I, int64_t* K, int64_t* count) {
     if (!(p->radius >= 0.f && p->radius <= 3.402823466e38f)) return "radius outside [0, inf)";
@@ -1114,39 +1135,68 @@ int64_t lv_preloc_count(const lv_preloc_params* p) {
     if (!p || preloc_params_error(p, &I, &K, &c)) return -1;
     return c;
 }
-lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p, lv_preloc_result* out,
-                         int32_t* scores_out) {
-    if (!p || !out || !d_xyz_lidar) { set_error("prelocalize: null params, result or points"); return LV_ERR_ARG; }
-    if (n < 1 || n > 0x7fffffff) { set_error("prelocalize: n outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
-    int64_t I = 0, K = 0, count = 0;
-    if (const char* e = preloc_params_error(p, &I, &K, &count)) { set_error(std::string("prelocalize: ") + e); return LV_ERR_ARG; }
-    if (count > LV_PRELOC_MAX_CANDIDATES) {
-        set_error("prelocalize: " + std::to_string((long long)count) + " candidates, more than 2^24");
+/* the argument checks of both searches, `what` prefixing the messages: LV_OK with I, K and the candidate count filled in when
+ * there are at most max_candidates (a power of two) */
+static lv_status preloc_args(const std::string& what, const float* d_xyz, int64_t n, const lv_preloc_params* p, const lv_preloc_result* out,
+                             int64_t max_candidates, int64_t* I, int64_t* K, int64_t* count) {
+    if (!p || !out || !d_xyz) { set_error(what + ": null params, result or points"); return LV_ERR_ARG; }
+    if (n < 1 || n > 0x7fffffff) { set_error(what + ": n outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
+    if (const char* e = preloc_params_error(p, I, K, count)) { set_error(what + ": " + e); return LV_ERR_ARG; }
+    if (*count > max_candidates) {
+        set_error(what + ": " + std::to_string((long long)*count) + " candidates, more than 2^" + std::to_string(__builtin_ctzll(max_candidates)));
         return LV_ERR_ARG;
     }
-    if (!h) { set_error("prelocalize: null handle"); return LV_ERR_ARG; }
-    if (h->map.empty) { set_error("prelocalize: the map is empty"); return LV_EMPTY_MAP; }
+    return LV_OK;
+}
+/* the handle's checks of both searches, after the argument checks: LV_OK with the base state (what lv_get_state returns) in h->x
+ * and a map that holds points */
+static lv_status preloc_ready(lv_context* h, const std::string& what) {
+    if (!h) { set_error(what + ": null handle"); return LV_ERR_ARG; }
+    if (h->map.empty) { set_error(what + ": the map is empty"); return LV_EMPTY_MAP; }
     LV_CUDA(cudaSetDevice(h->prm.device));
-    sync_mirror(h);                                               /* the base: what lv_get_state returns */
-    if (h->map_unknown) {                                         /* an async first build the gate may have left without points */
-        LV_CUDA(map_fetch_counters(h->map, h->stream));
-        LV_CUDA(cudaStreamSynchronize(h->stream));
-        if ((int32_t)h->map.h_counters[kCtrPoints] == 0) h->map.empty = true;
-        h->map_unknown = false;
-    }
-    if (h->map.empty) { set_error("prelocalize: the map is empty"); return LV_EMPTY_MAP; }
-
-    const int64_t H = 2 * K + 1, W = 2 * I + 1, P = W * W;
-    const int32_t S = (int32_t)(n < p->max_points ? n : p->max_points);
-    double x0[LV_STATE_LEN];
-    memcpy(x0, h->x, sizeof(x0));
-    const PrelocAxes ax = preloc_axes(x0);
-    std::vector<float> frames((size_t)H * 12);
+    sync_mirror(h);
+    if (lv_status s = settle_map_unknown(h, false)) return s;
+    if (h->map.empty) { set_error(what + ": the map is empty"); return LV_EMPTY_MAP; }
+    return LV_OK;
+}
+/* one frame per heading k = -K..K about the base state: R (9 floats), then t (3) */
+static std::vector<float> preloc_frames(const double* x, const PrelocAxes& ax, int64_t K, float yaw_step) {
+    std::vector<float> frames((size_t)(2 * K + 1) * 12);
     for (int64_t k = -K; k <= K; ++k) {
-        const Rt32 F = preloc_heading_frame(x0, ax, (double)k * (double)p->yaw_step);
+        const Rt32 F = preloc_heading_frame(x, ax, (double)k * (double)yaw_step);
         memcpy(&frames[(size_t)(k + K) * 12], F.R, sizeof(float) * 9);
         memcpy(&frames[(size_t)(k + K) * 12 + 9], F.t, sizeof(float) * 3);
     }
+    return frames;
+}
+/* the winning candidate (index idx in heading-major order, its score over S points) into out and into the state, as
+ * lv_set_state(out->x, NULL) */
+static void preloc_finish(lv_context* h, const lv_preloc_params* p, int64_t I, int64_t K, int64_t count, int64_t idx, int32_t score,
+                          int32_t S, lv_preloc_result* out) {
+    const int64_t W = 2 * I + 1, P = W * W, hk = idx / P, q = idx % P;
+    memset(out, 0, sizeof(*out));
+    out->candidates = count;
+    out->index = idx;
+    out->k = (int32_t)(hk - K);
+    out->i = (int32_t)(q / W - I);
+    out->j = (int32_t)(q % W - I);
+    out->score = score;
+    out->points = S;
+    preloc_candidate(h->x, preloc_axes(h->x), (double)out->k * (double)p->yaw_step, (double)out->i * (double)p->step,
+                     (double)out->j * (double)p->step, out->x);
+    memcpy(h->x, out->x, sizeof(h->x));
+    h->state_dirty = true;
+}
+lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p, lv_preloc_result* out,
+                         int32_t* scores_out) {
+    int64_t I = 0, K = 0, count = 0;
+    if (lv_status s = preloc_args("prelocalize", d_xyz_lidar, n, p, out, LV_PRELOC_MAX_CANDIDATES, &I, &K, &count)) return s;
+    if (lv_status s = preloc_ready(h, "prelocalize")) return s;
+
+    const int64_t H = 2 * K + 1, W = 2 * I + 1, P = W * W;
+    const int32_t S = (int32_t)(n < p->max_points ? n : p->max_points);
+    const PrelocAxes ax = preloc_axes(h->x);
+    const std::vector<float> frames = preloc_frames(h->x, ax, K, p->yaw_step);
     std::vector<float4> offsets((size_t)P);
     for (int64_t i = -I; i <= I; ++i)
         for (int64_t j = -I; j <= I; ++j) {
@@ -1183,36 +1233,11 @@ lv_status lv_prelocalize(lv_handle h, const float* d_xyz_lidar, int64_t n, const
     LV_CUDA(cudaMemcpyAsync(&key, base, sizeof(key), cudaMemcpyDeviceToHost, h->stream));
     if (scores_out) LV_CUDA(cudaMemcpyAsync(scores_out, a.scores, sizeof(int32_t) * (size_t)count, cudaMemcpyDeviceToHost, h->stream));
     LV_CUDA(cudaStreamSynchronize(h->stream));
-
-    const int64_t idx = preloc_key_index(key);
-    const int64_t hk = idx / P, q = idx % P;
-    memset(out, 0, sizeof(*out));
-    out->candidates = count;
-    out->index = idx;
-    out->k = (int32_t)(hk - K);
-    out->i = (int32_t)(q / W - I);
-    out->j = (int32_t)(q % W - I);
-    out->score = preloc_key_score(key);
-    out->points = S;
-    preloc_candidate(x0, ax, (double)out->k * (double)p->yaw_step, (double)out->i * (double)p->step, (double)out->j * (double)p->step,
-                     out->x);
-    memcpy(h->x, out->x, sizeof(h->x));                           /* lv_set_state(out->x, NULL) */
-    h->state_dirty = true;
+    preloc_finish(h, p, I, K, count, preloc_key_index(key), preloc_key_score(key), S, out);
     return LV_OK;
 }
 
 /* ---- start pose anywhere in a saved map (lv_prelocalize_global, lv_map_extent) ---------------- */
-/* LV_EMPTY_MAP when the map holds no point (also after an asynchronous first build that the gate left empty) */
-static lv_status pglob_map_empty(lv_context* h, const char* what) {
-    if (h->map_unknown) {
-        LV_CUDA(map_fetch_counters(h->map, h->stream));
-        LV_CUDA(cudaStreamSynchronize(h->stream));
-        if ((int32_t)h->map.h_counters[kCtrPoints] == 0) h->map.empty = true;
-        h->map_unknown = false;
-    }
-    if (h->map.empty) { set_error(std::string(what) + ": the map is empty"); return LV_EMPTY_MAP; }
-    return LV_OK;
-}
 static size_t pglob_align(size_t b) { return (b + 255) & ~(size_t)255; }
 /* the occupancy summary of the map (h->occ: extent, bitmap pyramid in h->d_occ), rebuilt only when the map changed since it
  * was built (map_gen); LV_EMPTY_MAP when no block holds an occupied voxel */
@@ -1248,7 +1273,8 @@ lv_status lv_map_extent(lv_handle h, double lo[3], double hi[3]) {
     if (!h) { set_error("map_extent: null handle"); return LV_ERR_ARG; }
     if (!lo || !hi) { set_error("map_extent: null lo or hi"); return LV_ERR_ARG; }
     LV_CUDA(cudaSetDevice(h->prm.device));
-    if (lv_status s = pglob_map_empty(h, "map_extent")) return s;
+    if (lv_status s = settle_map_unknown(h, false)) return s;
+    if (h->map.empty) { set_error("map_extent: the map is empty"); return LV_EMPTY_MAP; }
     int launches = 0;
     const lv_status s = pglob_occupancy(h, "map_extent", &launches);
     h->prof.total_launches += launches;
@@ -1294,26 +1320,13 @@ struct DevicePrelocEval {
 
 lv_status lv_prelocalize_global(lv_handle h, const float* d_xyz_lidar, int64_t n, const lv_preloc_params* p, lv_preloc_result* out,
                                 lv_preloc_stats* stats) {
-    if (!p || !out || !d_xyz_lidar) { set_error("prelocalize_global: null params, result or points"); return LV_ERR_ARG; }
-    if (n < 1 || n > 0x7fffffff) { set_error("prelocalize_global: n outside [1, 2^31 - 1]"); return LV_ERR_ARG; }
     int64_t I = 0, K = 0, count = 0;
-    if (const char* e = preloc_params_error(p, &I, &K, &count)) {
-        set_error(std::string("prelocalize_global: ") + e);
-        return LV_ERR_ARG;
-    }
-    if (count > LV_PRELOC_GLOBAL_MAX_CANDIDATES) {
-        set_error("prelocalize_global: " + std::to_string((long long)count) + " candidates, more than 2^40");
-        return LV_ERR_ARG;
-    }
+    if (lv_status s = preloc_args("prelocalize_global", d_xyz_lidar, n, p, out, LV_PRELOC_GLOBAL_MAX_CANDIDATES, &I, &K, &count)) return s;
     if (2 * K + 1 > kPrelocMaxTopCells) {
         set_error("prelocalize_global: " + std::to_string((long long)(2 * K + 1)) + " headings, more than 2^20");
         return LV_ERR_ARG;
     }
-    if (!h) { set_error("prelocalize_global: null handle"); return LV_ERR_ARG; }
-    if (h->map.empty) { set_error("prelocalize_global: the map is empty"); return LV_EMPTY_MAP; }
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    sync_mirror(h);                                               /* the base: what lv_get_state returns */
-    if (lv_status s = pglob_map_empty(h, "prelocalize_global")) return s;
+    if (lv_status s = preloc_ready(h, "prelocalize_global")) return s;
 
     int launches = 0;
     {
@@ -1322,17 +1335,9 @@ lv_status lv_prelocalize_global(lv_handle h, const float* d_xyz_lidar, int64_t n
         if (s != LV_OK) return s;
     }
     const PrelocOcc occ = h->occ;
-    const int64_t H = 2 * K + 1;
     const int32_t S = (int32_t)(n < p->max_points ? n : p->max_points);
-    double x0[LV_STATE_LEN];
-    memcpy(x0, h->x, sizeof(x0));
-    const PrelocAxes ax = preloc_axes(x0);
-    std::vector<float> frames((size_t)H * 12);
-    for (int64_t k = -K; k <= K; ++k) {
-        const Rt32 F = preloc_heading_frame(x0, ax, (double)k * (double)p->yaw_step);
-        memcpy(&frames[(size_t)(k + K) * 12], F.R, sizeof(float) * 9);
-        memcpy(&frames[(size_t)(k + K) * 12 + 9], F.t, sizeof(float) * 3);
-    }
+    const PrelocAxes ax = preloc_axes(h->x);
+    const std::vector<float> frames = preloc_frames(h->x, ax, K, p->yaw_step);
     /* scratch: frames, cells, bounds, best */
     const size_t off_frames = 0, off_cells = pglob_align(off_frames + sizeof(float) * frames.size());
     const size_t off_bounds = pglob_align(off_cells + sizeof(PrelocCell) * kPrelocChunk);
@@ -1372,18 +1377,6 @@ lv_status lv_prelocalize_global(lv_handle h, const float* d_xyz_lidar, int64_t n
     h->prof.total_launches += ev.launches;
     LV_CUDA(ev.err);
 
-    const int64_t W = 2 * I + 1, P = W * W, idx = search.best.idx;
-    const int64_t hk = idx / P, q = idx % P;
-    memset(out, 0, sizeof(*out));
-    out->candidates = count;
-    out->index = idx;
-    out->k = (int32_t)(hk - K);
-    out->i = (int32_t)(q / W - I);
-    out->j = (int32_t)(q % W - I);
-    out->score = search.best.score;
-    out->points = S;
-    preloc_candidate(x0, ax, (double)out->k * (double)p->yaw_step, (double)out->i * (double)p->step, (double)out->j * (double)p->step,
-                     out->x);
     if (stats) {
         memset(stats, 0, sizeof(*stats));
         stats->candidates = search.st.candidates;
@@ -1392,8 +1385,7 @@ lv_status lv_prelocalize_global(lv_handle h, const float* d_xyz_lidar, int64_t n
         stats->probes = search.st.probes;
         stats->launches = search.st.launches;
     }
-    memcpy(h->x, out->x, sizeof(h->x));                           /* lv_set_state(out->x, NULL) */
-    h->state_dirty = true;
+    preloc_finish(h, p, I, K, count, search.best.idx, search.best.score, S, out);
     return LV_OK;
 }
 
@@ -1528,6 +1520,40 @@ static lv_status voxelgrid_sync(lv_context* h, const float* d_xyz, int64_t n, fl
     *n_out = h->ds.h_count[0];
     return LV_OK;
 }
+/* both host forms for n > 0 points: xyz (and, when time is given, time and intensity) staged, the synchronous voxel grid, then
+ * whichever outputs are non-NULL copied back */
+static lv_status voxelgrid_host(lv_context* h, const float* xyz, const double* time, const float* intensity, int64_t n, float leaf,
+                                float* xyz_out, double* time_out, float* intensity_out, float* range_out, int64_t* n_out) {
+    LV_CUDA(cudaSetDevice(h->prm.device));
+    lv_status s = ds_stage(h, n);
+    if (s != LV_OK) return s;
+    /* device staging of the attributes, grown with slack as ds_stage: in / out time, then in / out intensity and out range */
+    VoxelLanes lanes;
+    double* t_in = nullptr;
+    float* f = nullptr;
+    if (time) {
+        if (28 * (size_t)n > h->d_ds_lanes.size()) LV_CUDA(h->d_ds_lanes.reserve(28 * (size_t)(n + n / 4 + 1024)));
+        const int64_t c = (int64_t)(h->d_ds_lanes.size() / 28);
+        t_in = reinterpret_cast<double*>(h->d_ds_lanes.get());
+        f = reinterpret_cast<float*>(t_in + 2 * c);
+        lanes.time = t_in; lanes.time_out = t_in + c;
+        lanes.intensity = f; lanes.intensity_out = f + c; lanes.range_out = f + 2 * c;
+    }
+    LV_CUDA(cudaMemcpyAsync(h->d_ds_in, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
+    if (time) {
+        LV_CUDA(cudaMemcpyAsync(t_in, time, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
+        LV_CUDA(cudaMemcpyAsync(f, intensity, sizeof(float) * n, cudaMemcpyHostToDevice, h->stream));
+    }
+    s = voxelgrid_sync(h, h->d_ds_in, n, leaf, h->d_ds_out, time ? &lanes : nullptr, n_out);
+    if (s != LV_OK) return s;
+    const size_t m = (size_t)*n_out;
+    LV_CUDA(cudaMemcpyAsync(xyz_out, h->d_ds_out, sizeof(float) * 3 * m, cudaMemcpyDeviceToHost, h->stream));
+    if (time_out) LV_CUDA(cudaMemcpyAsync(time_out, lanes.time_out, sizeof(double) * m, cudaMemcpyDeviceToHost, h->stream));
+    if (intensity_out) LV_CUDA(cudaMemcpyAsync(intensity_out, lanes.intensity_out, sizeof(float) * m, cudaMemcpyDeviceToHost, h->stream));
+    if (range_out) LV_CUDA(cudaMemcpyAsync(range_out, lanes.range_out, sizeof(float) * m, cudaMemcpyDeviceToHost, h->stream));
+    LV_CUDA(cudaStreamSynchronize(h->stream));
+    return LV_OK;
+}
 lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_t n, float leaf, float* d_xyz_out, int64_t* n_out) {
     /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids: an output
      * range that overlaps the input would be read after it is overwritten */
@@ -1540,18 +1566,10 @@ lv_status lv_voxelgrid_downsample_device(lv_handle h, const float* d_xyz, int64_
     if (n == 0) return LV_OK;
     return voxelgrid_sync(h, d_xyz, n, leaf, d_xyz_out, nullptr, n_out);
 }
-/* the byte ranges of a full voxel grid's n points: inputs [0, 4) (xyz, time, intensity, count), outputs [4, 9); an output may not
- * overlap an input or another output (the centroid kernel reads a leaf's inputs while other threads write) */
-static bool voxel_full_overlap(const void* const p[9], int64_t n) {
-    const int64_t bytes[9] = {12 * n, 8 * n, 4 * n, 8, 12 * n, 8 * n, 4 * n, 4 * n, 8};
-    for (int o = 4; o < 9; ++o)
-        for (int k = 0; k < o; ++k)
-            if (p[o] && p[k] && ranges_overlap(p[o], bytes[o], p[k], bytes[k])) return true;
-    return false;
-}
-/* the launch of both async voxel grids, after their argument checks */
-static lv_status voxelgrid_async(lv_context* h, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf, float* d_xyz_out,
-                                 int64_t* d_n_out, const VoxelLanes* lanes) {
+/* the handle's checks and the launch of both async voxel grids, after their own checks; `what` names the call in the messages */
+static lv_status voxelgrid_async(lv_context* h, const char* what, const float* d_xyz, const int64_t* d_n, int64_t n_max, float leaf,
+                                 float* d_xyz_out, int64_t* d_n_out, const VoxelLanes* lanes) {
+    if (!handle_ok(what, h, n_max)) return LV_ERR_ARG;
     LV_CUDA(cudaSetDevice(h->prm.device));
     LV_CUDA(ds_reserve(h->ds, n_max));
     int launches = 0;
@@ -1566,8 +1584,7 @@ lv_status lv_voxelgrid_downsample_device_async(lv_handle h, const float* d_xyz, 
     if (!(leaf > 0.f)) { set_error("voxel grid async: leaf size must be positive"); return LV_ERR_ARG; }
     /* the centroid kernel reads every input point of a leaf while other threads write their leaves' centroids */
     if (ranges_overlap(d_xyz, 12 * n_max, d_xyz_out, 12 * n_max)) { set_error("voxel grid async: the output range overlaps the input range"); return LV_ERR_ARG; }
-    if (!handle_ok("voxel grid async", h, n_max)) return LV_ERR_ARG;
-    return voxelgrid_async(h, d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, nullptr);
+    return voxelgrid_async(h, "voxel grid async", d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, nullptr);
 }
 lv_status lv_voxelgrid_downsample_full_device_async(lv_handle h, const float* d_xyz, const double* d_time, const float* d_intensity,
                                                     const int64_t* d_n, int64_t n_max, float leaf, float* d_xyz_out, double* d_time_out,
@@ -1578,27 +1595,20 @@ lv_status lv_voxelgrid_downsample_full_device_async(lv_handle h, const float* d_
     }
     if (!n_max_ok("voxel grid full", n_max)) return LV_ERR_ARG;
     if (!(leaf > 0.f)) { set_error("voxel grid full: leaf size must be positive"); return LV_ERR_ARG; }
-    const void* const p[9] = {d_xyz, d_time, d_intensity, d_n, d_xyz_out, d_time_out, d_intensity_out, d_range_out, d_n_out};
-    if (voxel_full_overlap(p, n_max)) { set_error("voxel grid full: an output range overlaps an input or another output"); return LV_ERR_ARG; }
-    if (!handle_ok("voxel grid full", h, n_max)) return LV_ERR_ARG;
+    /* the centroid kernel reads a leaf's inputs while other threads write: an output may overlap no input and no other output */
+    const ByteRange r[9] = {{d_xyz, 12 * n_max}, {d_time, 8 * n_max}, {d_intensity, 4 * n_max}, {d_n, 8}, {d_xyz_out, 12 * n_max},
+                            {d_time_out, 8 * n_max}, {d_intensity_out, 4 * n_max}, {d_range_out, 4 * n_max}, {d_n_out, 8}};
+    if (any_ranges_overlap(r, 9, 4)) { set_error("voxel grid full: an output range overlaps an input or another output"); return LV_ERR_ARG; }
     VoxelLanes lanes;
     lanes.time = d_time; lanes.intensity = d_intensity;
     lanes.time_out = d_time_out; lanes.intensity_out = d_intensity_out; lanes.range_out = d_range_out;
-    return voxelgrid_async(h, d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, &lanes);
+    return voxelgrid_async(h, "voxel grid full", d_xyz, d_n, n_max, leaf, d_xyz_out, d_n_out, &lanes);
 }
 lv_status lv_voxelgrid_downsample(lv_handle h, const float* xyz, int64_t n, float leaf, float* xyz_out, int64_t* n_out) {
     if (!h || !xyz || !xyz_out || !n_out || n < 0 || !(leaf > 0.f) || n > 0x7fffffff) return LV_ERR_ARG;
     *n_out = 0;
     if (n == 0) return LV_OK;
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    lv_status s = ds_stage(h, n);
-    if (s != LV_OK) return s;
-    LV_CUDA(cudaMemcpyAsync(h->d_ds_in, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
-    s = lv_voxelgrid_downsample_device(h, h->d_ds_in, n, leaf, h->d_ds_out, n_out);
-    if (s != LV_OK) return s;
-    LV_CUDA(cudaMemcpyAsync(xyz_out, h->d_ds_out, sizeof(float) * 3 * (size_t)*n_out, cudaMemcpyDeviceToHost, h->stream));
-    LV_CUDA(cudaStreamSynchronize(h->stream));
-    return LV_OK;
+    return voxelgrid_host(h, xyz, nullptr, nullptr, n, leaf, xyz_out, nullptr, nullptr, nullptr, n_out);
 }
 lv_status lv_voxelgrid_downsample_full(lv_handle h, const float* xyz, const double* time, const float* intensity, int64_t n, float leaf,
                                        float* xyz_out, double* time_out, float* intensity_out, float* range_out, int64_t* n_out) {
@@ -1611,29 +1621,7 @@ lv_status lv_voxelgrid_downsample_full(lv_handle h, const float* xyz, const doub
     if (!(leaf > 0.f)) { set_error("voxel grid full: leaf size must be positive"); return LV_ERR_ARG; }
     if (!h) { set_error("voxel grid full: null handle"); return LV_ERR_ARG; }
     if (n == 0) return LV_OK;
-    LV_CUDA(cudaSetDevice(h->prm.device));
-    lv_status s = ds_stage(h, n);
-    if (s != LV_OK) return s;
-    /* device staging of the attributes, grown with slack as ds_stage: in / out time, then in / out intensity and out range */
-    if (28 * (size_t)n > h->d_ds_lanes.size()) LV_CUDA(h->d_ds_lanes.reserve(28 * (size_t)(n + n / 4 + 1024)));
-    const int64_t c = (int64_t)(h->d_ds_lanes.size() / 28);
-    VoxelLanes lanes;
-    double* t_in = reinterpret_cast<double*>(h->d_ds_lanes.get());
-    float* f = reinterpret_cast<float*>(t_in + 2 * c);
-    lanes.time = t_in; lanes.time_out = t_in + c;
-    lanes.intensity = f; lanes.intensity_out = f + c; lanes.range_out = f + 2 * c;
-    LV_CUDA(cudaMemcpyAsync(h->d_ds_in, xyz, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, h->stream));
-    LV_CUDA(cudaMemcpyAsync(t_in, time, sizeof(double) * n, cudaMemcpyHostToDevice, h->stream));
-    LV_CUDA(cudaMemcpyAsync(f, intensity, sizeof(float) * n, cudaMemcpyHostToDevice, h->stream));
-    s = voxelgrid_sync(h, h->d_ds_in, n, leaf, h->d_ds_out, &lanes, n_out);
-    if (s != LV_OK) return s;
-    const size_t m = (size_t)*n_out;
-    LV_CUDA(cudaMemcpyAsync(xyz_out, h->d_ds_out, sizeof(float) * 3 * m, cudaMemcpyDeviceToHost, h->stream));
-    if (time_out) LV_CUDA(cudaMemcpyAsync(time_out, lanes.time_out, sizeof(double) * m, cudaMemcpyDeviceToHost, h->stream));
-    if (intensity_out) LV_CUDA(cudaMemcpyAsync(intensity_out, lanes.intensity_out, sizeof(float) * m, cudaMemcpyDeviceToHost, h->stream));
-    if (range_out) LV_CUDA(cudaMemcpyAsync(range_out, lanes.range_out, sizeof(float) * m, cudaMemcpyDeviceToHost, h->stream));
-    LV_CUDA(cudaStreamSynchronize(h->stream));
-    return LV_OK;
+    return voxelgrid_host(h, xyz, time, intensity, n, leaf, xyz_out, time_out, intensity_out, range_out, n_out);
 }
 lv_status lv_temporal_downsample(lv_handle h, const float* xyz, int64_t n, int32_t rate, double min_dist, float* xyz_out,
                                  int32_t* idx_out, int64_t* n_out) {
@@ -1672,14 +1660,9 @@ static lv_status front_end_impl(lv_handle h, const std::string& what, bool null_
     if (n < 0 || n > 0x7fffffff) { set_error(what + ": n outside [0, 2^31 - 1] (point indices are int32)"); return LV_ERR_ARG; }
     if (const char* why = layout_error()) { set_error(what + ": " + why); return LV_ERR_ARG; }
     /* the gather decodes the message while it writes the outputs: an output that overlaps the bytes would be read after it is
-     * overwritten */
-    const struct { const void* p; int64_t bytes; } outs[5] = {{o.xyz, 12 * n}, {o.time, 8 * n}, {o.intensity, 4 * n}, {o.range, 4 * n},
-                                                            {o.idx, 4 * n}};
-    for (const auto& r : outs)
-        if (r.p && n > 0 && ranges_overlap(r.p, r.bytes, d_data, data_bytes)) {
-            set_error(what + ": an output range overlaps the message bytes");
-            return LV_ERR_ARG;
-        }
+     * overwritten (the outputs may overlap each other) */
+    const ByteRange r[6] = {{o.xyz, 12 * n}, {o.time, 8 * n}, {o.intensity, 4 * n}, {o.range, 4 * n}, {o.idx, 4 * n}, {d_data, data_bytes}};
+    if (n > 0 && any_ranges_overlap(r, 6, 5)) { set_error(what + ": an output range overlaps the message bytes"); return LV_ERR_ARG; }
     if (!h) { set_error(what + ": null handle"); return LV_ERR_ARG; }
     if (cloud_bound(n, downsample_rate) == 0) {                  /* nothing can be kept */
         if (d_n_out) {
@@ -1882,14 +1865,8 @@ static lv_status lidar_push_impl(lv_handle h, const float* d_xyz, const double* 
             memcpy(rt.t, T + 9, sizeof(rt.t));
         }
         /* the split kernel reads the times and the count while the write kernel reads the points: they must be distinct arrays */
-        const void* const in[5] = {d_xyz, d_time, d_n, d_intensity, d_range};
-        const int64_t bytes[5] = {12 * n_max, 8 * n_max, 8, 4 * n_max, 4 * n_max};
-        for (int a = 1; a < 5; ++a)
-            for (int b = 0; b < a; ++b)
-                if (in[a] && in[b] && ranges_overlap(in[a], bytes[a], in[b], bytes[b])) {
-                    set_error(w + ": the input ranges overlap");
-                    return LV_ERR_ARG;
-                }
+        const ByteRange in[5] = {{d_xyz, 12 * n_max}, {d_time, 8 * n_max}, {d_n, 8}, {d_intensity, 4 * n_max}, {d_range, 4 * n_max}};
+        if (any_ranges_overlap(in, 5)) { set_error(w + ": the input ranges overlap"); return LV_ERR_ARG; }
     }
     if (!h) { set_error(w + ": null handle"); return LV_ERR_ARG; }
     if (!h->lidar.cap) { set_error(w + ": the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
@@ -1939,19 +1916,13 @@ static lv_status lidar_get_impl(lv_handle h, double t1, double t2, float* d_xyz,
     if (!d_xyz || !d_time || !count) { set_error(w + ": null xyz, time or count"); return LV_ERR_ARG; }
     if (!n_max_ok(what, n_max)) return LV_ERR_ARG;
     if (isnan(t1) || isnan(t2)) { set_error(w + ": t1 or t2 is NaN"); return LV_ERR_ARG; }
-    const void* const outs[5] = {d_xyz, d_time, d_n_out, d_intensity, d_range};
-    const int64_t bytes[5] = {12 * n_max, 8 * n_max, 8, 4 * n_max, 4 * n_max};
-    for (int a = 1; a < 5; ++a)
-        for (int b = 0; b < a; ++b)
-            if (outs[a] && outs[b] && ranges_overlap(outs[a], bytes[a], outs[b], bytes[b])) {
-                set_error(w + ": the output ranges overlap");
-                return LV_ERR_ARG;
-            }
+    const ByteRange outs[5] = {{d_xyz, 12 * n_max}, {d_time, 8 * n_max}, {d_n_out, 8}, {d_intensity, 4 * n_max}, {d_range, 4 * n_max}};
+    if (any_ranges_overlap(outs, 5)) { set_error(w + ": the output ranges overlap"); return LV_ERR_ARG; }
     if (!h) { set_error(w + ": null handle"); return LV_ERR_ARG; }
     if (!h->lidar.cap) { set_error(w + ": the buffer has no capacity (lv_lidar_reserve first)"); return LV_ERR_ARG; }
     if (d_intensity && !h->lidar.intensity) { set_error(w + ": the buffer has no attribute lanes (lv_lidar_reserve_full first)"); return LV_ERR_ARG; }
-    for (int a = 0; a < 5; ++a)
-        if (outs[a] && overlaps_lidar(h, outs[a], bytes[a])) {
+    for (const ByteRange& o : outs)
+        if (o.p && overlaps_lidar(h, o.p, o.bytes)) {
             set_error(w + ": an output range overlaps the buffer");
             return LV_ERR_ARG;
         }

@@ -8,8 +8,8 @@
  *
  *     content[k] = ring[tail - 1 - k],   size = tail - head,   content.back() = ring[head].
  *
- * Everything here compiles for the device (lv_lidar_buffer.cu) and for the host (tests/cpu_shim/lidar_ring.cpp and, for the
- * merge, tests/cpu_shim_merge/lidar_merge.cpp; both test-only), so the kernels and the host build share the probe sequence of the binary search, the predicates of the walk and of clear, and the
+ * Everything here compiles for the device (lv_lidar_buffer.cu) and for the host (tests/cpu_shim/lidar_ring.cpp, test-only), so the
+ * kernels and the host build share the probe sequence of the binary search, the predicates of the walk and of clear, and the
  * rules of the time-ordered merge.  Comparisons are written exactly as in the reference, so a NaN point time behaves as it does there.
  */
 #ifndef LV_LIDAR_BUFFER_H_

@@ -7,7 +7,7 @@
  * (lv_preloc.cu) only reads those tables and the map.  For heading 0 and offset 0 the world points are those of
  * lv_match_all at the base state (rt_apply of make_frame's lidar_to_world), bit for bit.
  *
- * tests/cpu_shim_preloc runs these functions serially on the host.
+ * tests/cpu_shim/preloc.cpp runs these functions serially on the host.
  */
 #ifndef LV_PRELOC_H_
 #define LV_PRELOC_H_

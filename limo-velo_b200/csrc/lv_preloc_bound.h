@@ -39,7 +39,7 @@
  *     the box is wide in x and y and one or two voxels tall).  The box is cut to the extent, then tested against the at most
  *     2 x 2 coarse columns that cover it at the finest level where it fits: conservative.
  *
- * The schedule (PrelocSearch, host code shared by lv_capi.cu and tests/cpu_shim_preloc_global): bound every top-level cell
+ * The schedule (PrelocSearch, host code shared by lv_capi.cu and tests/cpu_shim/preloc.cpp): bound every top-level cell
  * and order the cells by bound (descending, ties by cell index); find a first score by diving from the first cell through
  * the child of highest bound at each level; then take the cells in batches and descend level by level, each level's
  * survivors highest bound first, scoring the surviving level-1 cells exactly; stop when the next top cell's bound is below

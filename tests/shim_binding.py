@@ -1,5 +1,5 @@
 """ctypes binding of tests/cpu_shim/liblv_cpushim.so (TEST-ONLY host build of the product headers): the map, search and
-filter (shim.cpp), the LiDAR buffer (lidar_ring.cpp), the start-pose searches (preloc.cpp) and the buffer and event owners over
+filter (shim.cpp), the LiDAR buffer and its time-ordered merge (lidar_ring.cpp), the start-pose searches (preloc.cpp) and the buffer and event owners over
 a fake CUDA runtime (buffers.cpp)."""
 import ctypes as C
 import os
@@ -67,6 +67,9 @@ def lib():
         L.shim_lidar_get.restype = i64
         L.shim_lidar_clear.argtypes = [vp, C.c_double]
         L.shim_lidar_clear.restype = None
+        L.shim_lidar_content_full.argtypes = [vp, fp, dp, fp, fp]
+        L.shim_lidar_content_full.restype = None
+        L.shim_lidar_merge.argtypes = [vp, fp, dp, fp, fp, i64, fp, i64]
 
         L.shim_preloc_scores.argtypes = [dp, fp, i64, fp, i64, f, f, f, f, f, f, C.c_int32, i32p, fp, fp]
         L.shim_preloc_scores.restype = i64

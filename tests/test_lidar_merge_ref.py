@@ -3,7 +3,7 @@
 1. tests/lidar_merge_ref.py (the restatement): on time-ordered buffers and messages the merge is a stable sort of the
    concatenation with the buffered points first on equal times; messages that do not reach back into the buffer are the push; an
    unsorted message or buffer is appended and reported; the refusals leave the buffer unchanged; rt_apply rounds every step in fp32.
-2. The host build of csrc/lv_lidar_buffer.h's merge (tests/cpu_shim_merge/lidar_merge.cpp: the walk, the order rule, the mode, the merge
+2. The host build of csrc/lv_lidar_buffer.h's merge (tests/cpu_shim/lidar_ring.cpp: the walk, the order rule, the mode, the merge
    path of every diagonal, the transform) equals the restatement bit for bit over seeded random sequences of merges, pushes and
    clears on small rings that wrap, with and without lanes and transforms: ties across sensors, empty messages, empty T_tail,
    overlaps at and just above the reserve, full rings, NaN times and unsorted batches.
@@ -16,7 +16,7 @@ import pytest
 import full_points_ref as FP
 import lidar_buffer_ref as R
 import lidar_merge_ref as M
-import lidar_merge_shim as S
+import shim_binding as S
 
 f32 = np.float32
 MODES = ["write", "append", "full", "overlap"]                 # kLidarMerge* in lv_lidar_buffer.h
