@@ -496,6 +496,63 @@ lv_status lv_process_livox_device(lv_handle h, const uint8_t* d_data, int64_t da
                                   uint8_t tag_reject_mask, int32_t downsample_rate, double min_dist,
                                   float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out);
 
+/* ---- Velodyne packets: velodyne_msgs/VelodyneScan of a VLP-16 or Puck Hi-Res (single return) --------------------------------------
+ * The raw UDP packets of one rotation, as the Velodyne driver records them on /velodyne_packets; lv_bag_parse_velodyne_scan finds
+ * them in a bag.  Packet k starts at packets + 1214 k (any alignment): uint32 stamp.sec | uint32 stamp.nsec | uint8[1206] data.
+ * data: 12 blocks of 100 bytes, each a uint16 flag (0xEEFF), a uint16 azimuth A_b (0.01 deg) and 32 channels of (uint16 distance
+ * in 2 mm, uint8 reflectivity); then the sensor's uint32 us timestamp (not read), the return mode (byte 1204: 0x37 strongest, 0x38
+ * last, 0x39 dual) and the product id (not read).  All little endian.  The arithmetic follows the VLP-16 manual and the structure
+ * of velodyne_pointcloud's RawData::unpack_vlp16; bit parity with that driver is not claimed.
+ *   slots      message slot i: packet k = i / 384, r = i % 384, block b = r / 32, firing f = (r % 32) / 16, laser l = r % 16 (the
+ *              driver's ring is a caller-side mapping of l); 384 n_packets slots, idx reports the slot
+ *   points     a slot is a point when its packet's return mode is not 0x39, its block and every earlier block of the packet carry
+ *              the flag 0xEEFF (the driver stops at the first bad block), and its distance is not 0
+ *   azimuth    D_b = (A_{b+1} + 36000 - A_b) mod 36000 for b < 11 (from block b+1's raw bytes whatever its flag), D_11 = D_10;
+ *              a = A_b + D_b (l 2.304 + f 55.296) / 110.592 in fp32, each product, sum and the quotient rounded, no contraction;
+ *              q = round(a) (half away from zero) mod 36000
+ *   tables     C[q] = (float)cos(q 0.01 pi / 180), S[q] = (float)sin(...) in double, rounded; per laser cv, sv, cr, sr = the
+ *              floats of cos / sin of the vertical angle and the rotational correction, and the floats of dist, vo, ho
+ *   xyz        fp32, each product and sum rounded, in this order:
+ *                d = raw 0.002f + dist;  cosr = C[q] cr + S[q] sr;  sinr = S[q] cr - C[q] sr;  xy = d cv - vo sv
+ *                X = xy sinr - ho cosr;  Y = xy cosr + ho sinr;  Z = d sv + vo cv;  (x, y, z) = (Y, -X, Z) (ROS: x forward, y left)
+ *              so with zero calibration a return at range d, elevation e and azimuth A (clockwise from +x, seen from above) lies
+ *              at d (cos e cos A, -cos e sin A, sin e)
+ *   time       the packet stamp is the time of its first firing: total = sec 10^9 + nsec + (2b + f) 55296 + l 2304 ns (uint64),
+ *              then seconds as for Livox.  nsec >= 10^9 cannot be converted.
+ *   outputs    intensity = (float)reflectivity, range = the fp32 |p| (Point.cpp:166-169)
+ * Out of scope: dual-return decoding, the HDL-32E / VLP-32C / HDL-64 block layouts, calibration files (a sensor's factory values go
+ * in through lv_velodyne_calibration), the sensor's us timestamp and GPS time. */
+typedef enum lv_velodyne_model { LV_VELODYNE_VLP16 = 0, LV_VELODYNE_PUCK_HIRES = 1 } lv_velodyne_model;
+/* the fields of velodyne_pointcloud's calibration YAML, by laser id (= l) */
+typedef struct lv_velodyne_calibration {
+    double vert_correction[16];          /* vertical angle (rad)         */
+    double rot_correction[16];           /* rotational correction (rad)  */
+    double dist_correction[16];          /* distance correction (m)      */
+    double vert_offset_correction[16];   /* vertical offset (m)          */
+    double horiz_offset_correction[16];  /* horizontal offset (m)        */
+} lv_velodyne_calibration;
+/* the nominal calibration of a model: the vertical angles of its manual (VLP-16: -15, 1, -13, 3, ... 15 deg; Puck Hi-Res: -10,
+ * 0.67, -8.67, 2, ... 10 deg), every other term 0.  LV_ERR_ARG for an unknown model or a null out. */
+lv_status lv_velodyne_default_calibration(lv_velodyne_model model, lv_velodyne_calibration* out);
+/* msg2points on the host: the points of the message, in slot order, into xyz (3 x 384 n_packets), time, intensity, range and idx
+ * (384 n_packets each; intensity, range and idx may be NULL); *n_out = their count.  A dual-return packet contributes no points.
+ * LV_ERR_ARG for null packets / cal / xyz / time / n_out, n_packets outside [0, (2^31 - 1) / 384], data_bytes < 1214 n_packets, a
+ * non-finite calibration entry, or a packet stamp with nsec >= 10^9. */
+lv_status lv_velodyne_to_points(const uint8_t* packets, int64_t data_bytes, int64_t n_packets, const lv_velodyne_calibration* cal,
+                                float* xyz, double* time, float* intensity, float* range, int32_t* idx, int64_t* n_out);
+/* Accumulator::process on the device for a VelodyneScan: msg2points -> temporal_downsample on the RANK of the point among the
+ * msg2points points (not its slot) -> sort_points (stable in time, equal times in slot order).  d_packets: DEVICE copy of the
+ * packets (data_bytes long, any alignment).  Outputs as lv_process_livox_device, DEVICE buffers with room for 384 n_packets points.
+ * Bit for bit lv_velodyne_to_points, then lv_temporal_downsample on its output, then lv_time_sort_indices on the kept times, then
+ * the gathers.  The first call on a handle uploads the 2 x 36000-float rotation tables (and waits for that copy); lv_destroy frees
+ * them.  LV_ERR_ARG, before any device work and also with a null handle, for the host decoder's argument errors except the stamp,
+ * or an output range that overlaps [d_packets, d_packets + data_bytes).  LV_ERR_ARG after the device work when a packet is a
+ * dual-return one or its stamp has nsec >= 10^9 (the other packets' points are written, *n_out stays 0).  When 384 n_packets <
+ * downsample_rate nothing can be kept and the packets are not read.  Synchronises (n_out). */
+lv_status lv_process_velodyne_device(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                     const lv_velodyne_calibration* cal, int32_t downsample_rate, double min_dist,
+                                     float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out);
+
 /* ---- the tick without a host wait (main.cpp:76-105) ------------------------------------------------------------------------
  * Stream-ordered forms of the tick's device calls.  Each takes its input count from DEVICE memory (d_n, an int64_t) and writes
  * its output count to device memory (d_n_out), so that one stage hands its count to the next without the host: none of them
@@ -518,6 +575,13 @@ lv_status lv_process_livox_device_async(lv_handle h, const uint8_t* d_data, int6
                                         uint8_t tag_reject_mask, int32_t downsample_rate, double min_dist,
                                         float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
                                         int64_t* d_n_out);
+/* lv_process_velodyne_device with *d_n_out = points kept; feeds lv_lidar_push_full_device_async or lv_lidar_merge_device_async
+ * directly.  The output buffers have room for 384 n_packets points.  A dual-return packet or a stamp with nsec >= 10^9 is a deferred
+ * error (the other packets' points are kept). */
+lv_status lv_process_velodyne_device_async(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                           const lv_velodyne_calibration* cal, int32_t downsample_rate, double min_dist,
+                                           float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
+                                           int64_t* d_n_out);
 /* Compensator::compensate (Compensator.cpp:123-146) as lv_compensate_device over *d_n points.  The path and Xt2 stay host-built
  * (Compensator::upsample / get_t2); they are staged through pinned memory, so the host buffers may be reused on return.  A
  * timestamp outside the path (or out of order) is a deferred error.  d_xyz_out may equal d_xyz; other overlaps of the
@@ -719,6 +783,15 @@ typedef struct lv_livox_view {
     int64_t data_bytes;                  /* 19 x n_points                                         */
 } lv_livox_view;
 lv_status lv_bag_parse_livox(const uint8_t* msg, int64_t size, lv_livox_view* out);
+/* velodyne_msgs/VelodyneScan -> a view of its packets, ready for lv_velodyne_to_points / lv_process_velodyne_device (packets,
+ * data_bytes, n_packets).  LV_ERR_ARG for a null argument, a truncated message or bytes after the packets. */
+typedef struct lv_velodyne_view {
+    uint32_t stamp_sec, stamp_nsec;      /* header.stamp                                          */
+    int64_t n_packets;
+    const uint8_t* packets;              /* the first packet's stamp (any alignment)              */
+    int64_t data_bytes;                  /* 1214 x n_packets                                      */
+} lv_velodyne_view;
+lv_status lv_bag_parse_velodyne_scan(const uint8_t* msg, int64_t size, lv_velodyne_view* out);
 
 /* ---- PCD map files (the map format of PCL, pcl::io::savePCDFileBinary, and of most LiDAR SLAM tools).  Host code.
  * Saving the device map: lv_map_points -> lv_pcd_write.  Loading it: lv_pcd_read -> lv_map_build (KD_TREE::Build: file order

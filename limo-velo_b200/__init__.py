@@ -209,6 +209,13 @@ def lib():
                                               C.POINTER(i64)]
         L.lv_process_livox_device_async.argtypes = [vp, vp, i64, i64, C.c_uint64, C.c_uint8, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
         L.lv_bag_parse_livox.argtypes = [vp, i64, C.POINTER(LivoxView)]
+    if hasattr(L, "lv_process_velodyne_device"):   # the Velodyne packet front end; absent from older builds
+        cp = C.POINTER(VelodyneCalibration)
+        L.lv_velodyne_default_calibration.argtypes = [C.c_int, cp]
+        L.lv_velodyne_to_points.argtypes = [vp, i64, i64, cp, vp, vp, vp, vp, vp, C.POINTER(i64)]
+        L.lv_process_velodyne_device.argtypes = [vp, vp, i64, i64, cp, C.c_int32, C.c_double, vp, vp, vp, vp, vp, C.POINTER(i64)]
+        L.lv_process_velodyne_device_async.argtypes = [vp, vp, i64, i64, cp, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
+        L.lv_bag_parse_velodyne_scan.argtypes = [vp, i64, C.POINTER(VelodyneView)]
     if hasattr(L, "lv_lidar_reserve_merge"):   # the time-ordered merge of several LiDARs; absent from older builds
         L.lv_lidar_reserve_merge.argtypes = [vp, i64]
         L.lv_lidar_merge_device_async.argtypes = [vp, vp, vp, vp, i64, fp]
@@ -440,6 +447,51 @@ def livox_to_points(records, timebase_ns, tag_reject_mask):
     m = C.c_int64(0)
     _check(lib().lv_livox_to_points(raw.ctypes.data_as(C.c_void_p), len(raw), n, C.c_uint64(timebase_ns), int(tag_reject_mask),
                                     *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
+    return tuple(a[:m.value].copy() for a in out)
+
+
+# velodyne_msgs/VelodyneScan of a VLP-16 / Puck Hi-Res: packets of 1214 bytes, 384 slots each (include/limovelo_b200.h)
+VELODYNE_PACKET = 1214
+VELODYNE_SLOTS = 384
+VELODYNE_MODELS = {"vlp16": 0, "puck_hires": 1}
+
+
+class VelodyneCalibration(C.Structure):
+    _fields_ = [("vert_correction", C.c_double * 16), ("rot_correction", C.c_double * 16), ("dist_correction", C.c_double * 16),
+                ("vert_offset_correction", C.c_double * 16), ("horiz_offset_correction", C.c_double * 16)]
+
+
+class VelodyneView(C.Structure):
+    _fields_ = [("stamp_sec", C.c_uint32), ("stamp_nsec", C.c_uint32), ("n_packets", C.c_int64), ("packets", C.c_void_p),
+                ("data_bytes", C.c_int64)]
+
+
+def velodyne_calibration(model="vlp16"):
+    """lv_velodyne_default_calibration: the nominal calibration of "vlp16" or "puck_hires" (a VelodyneCalibration)"""
+    cal = VelodyneCalibration()
+    _check(lib().lv_velodyne_default_calibration(VELODYNE_MODELS[model], C.byref(cal)))
+    return cal
+
+
+def bag_parse_velodyne_scan(msg):
+    """lv_bag_parse_velodyne_scan on a serialised VelodyneScan (bytes): returns (VelodyneView, the packets as uint8 bytes)"""
+    v = VelodyneView()
+    buf = C.create_string_buffer(bytes(msg), len(msg))
+    _check(lib().lv_bag_parse_velodyne_scan(buf, len(msg), C.byref(v)))
+    off = v.packets - C.addressof(buf) if v.n_packets else 0
+    return v, np.frombuffer(buf.raw[off:off + v.data_bytes], np.uint8).copy()
+
+
+def velodyne_to_points(packets, cal):
+    """msg2points of a VelodyneScan on the host (packets: their bytes, 1214 per packet): returns (xyz, time, intensity, range, slot)
+    of the points, in slot order"""
+    raw = np.ascontiguousarray(np.frombuffer(bytes(memoryview(packets)), np.uint8))
+    k = len(raw) // VELODYNE_PACKET
+    n = VELODYNE_SLOTS * k
+    out = (np.empty((n, 3), np.float32), np.empty(n), np.empty(n, np.float32), np.empty(n, np.float32), np.empty(n, np.int32))
+    m = C.c_int64(0)
+    _check(lib().lv_velodyne_to_points(raw.ctypes.data_as(C.c_void_p), len(raw), k, C.byref(cal),
+                                       *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
     return tuple(a[:m.value].copy() for a in out)
 
 
@@ -744,6 +796,32 @@ class Localizer:
             for d in bufs:
                 self.device_free(d)
 
+    def process_velodyne_device(self, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity=None,
+                                d_range=None, d_idx=None):
+        """Accumulator::process on the packets of a VelodyneScan already in device memory (raw pointers); returns the points kept"""
+        m = C.c_int64(0)
+        _check(self.L.lv_process_velodyne_device(self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal),
+                                                 int(downsample_rate), float(min_dist), C.c_void_p(d_xyz), C.c_void_p(d_time),
+                                                 C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx), C.byref(m)))
+        return m.value
+
+    def process_velodyne(self, packets, cal, downsample_rate, min_dist):
+        """Accumulator::process on a VelodyneScan's packets (their bytes): uploads them, returns (xyz, time, intensity, range, slot)
+        of the kept points in time order"""
+        raw = np.frombuffer(bytes(memoryview(packets)), np.uint8)
+        k = len(raw) // VELODYNE_PACKET
+        n = VELODYNE_SLOTS * k
+        out = (np.empty((n, 3), np.float32), np.empty(n, np.float64), np.empty(n, np.float32), np.empty(n, np.float32),
+               np.empty(n, np.int32))
+        bufs = [self.device_alloc(max(raw.nbytes, 1))] + [self.device_alloc(max(a.nbytes, 1)) for a in out]
+        try:
+            _check(self.L.lv_memcpy_h2d(self.h, bufs[0], raw.ctypes.data_as(C.c_void_p), raw.nbytes))
+            m = self.process_velodyne_device(bufs[0], raw.nbytes, k, cal, downsample_rate, min_dist, *bufs[1:])
+            return tuple(self.download(d, a[:m]) for a, d in zip(out, bufs[1:]))
+        finally:
+            for d in bufs:
+                self.device_free(d)
+
     def download(self, d_ptr, out):
         """copy device memory into the contiguous numpy array `out` (its whole size); returns out"""
         if out.nbytes:
@@ -783,6 +861,14 @@ class Localizer:
         return _check(self.L.lv_process_livox_device_async(
             self.h, C.c_void_p(d_data), int(data_bytes), int(n), C.c_uint64(timebase_ns), int(tag_reject_mask), int(downsample_rate),
             float(min_dist), C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
+            C.c_void_p(d_n_out)))
+
+    def process_velodyne_device_async(self, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_n_out,
+                                      d_intensity=None, d_range=None, d_idx=None):
+        """lv_process_velodyne_device with the count of kept points written to d_n_out"""
+        return _check(self.L.lv_process_velodyne_device_async(
+            self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal), int(downsample_rate), float(min_dist),
+            C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
             C.c_void_p(d_n_out)))
 
     def compensate_device_async(self, path, Xt2, d_xyz, d_t, d_n, n_max, d_out):

@@ -99,6 +99,8 @@ struct lv_context {
     DeviceBuf<int> d_bad;
     PinnedBuf<int> h_bad;
     DownsampleScratch ds;              /* downsamplers: grows with the largest cloud seen */
+    DeviceBuf<float> d_velodyne_tables;   /* cos then sin of the 36000 azimuths (velodyne_tables): the first Velodyne call */
+    bool velodyne_tables_ok = false;      /* uploaded: a failed upload is retried on the next call */
     DeviceBuf<float> d_ds_in;          /* staging for the host-buffer variants (ds_stage) */
     DeviceBuf<float> d_ds_out;
     DeviceBuf<uint8_t> d_ds_lanes;     /* attribute staging of lv_voxelgrid_downsample_full: 28 B per point */
@@ -1646,14 +1648,15 @@ lv_status lv_temporal_downsample(lv_handle h, const float* xyz, int64_t n, int32
 }
 
 /* ---- Accumulator::process ------------------------------------------------------------------------ */
-/* the argument checks and the launches of both message formats: d_n_out NULL = the synchronous form (*n_out read back).
+/* the argument checks and the launches of every message format: d_n_out NULL = the synchronous form (*n_out read back).
  * null_args: a required pointer is NULL (null_what names them); layout_error() runs once the pointers and n are known good;
- * launch(launches, err) enqueues the pipeline */
+ * launch(launches, err) enqueues the pipeline; `deferred` says what the pipeline's flag word (ds.count[1]) means */
+static const char* const kCloudNaN = "a kept point's timestamp is NaN (the time sort has no order for it)";
 extern "C++" {
 template <class LayoutError, class Launch>
 static lv_status front_end_impl(lv_handle h, const std::string& what, bool null_args, const char* null_what, const uint8_t* d_data,
                                 int64_t data_bytes, int64_t n, int32_t downsample_rate, const CloudOut& o, int64_t* n_out, int64_t* d_n_out,
-                                LayoutError layout_error, Launch launch) {
+                                LayoutError layout_error, Launch launch, const char* deferred = kCloudNaN) {
     /* every check before the first device call */
     if (n_out) *n_out = 0;
     if (null_args || !n_out) { set_error(what + ": null " + null_what); return LV_ERR_ARG; }
@@ -1678,8 +1681,8 @@ static lv_status front_end_impl(lv_handle h, const std::string& what, bool null_
     h->prof.total_launches += launches;
     if (d_n_out) return LV_OK;
     LV_CUDA(cudaStreamSynchronize(h->stream));
-    if (h->ds.h_count[1]) {                                       /* PointCloud2 only: a Livox time is never NaN */
-        set_error(what + ": a kept point's timestamp is NaN (the time sort has no order for it)");
+    if (h->ds.h_count[1]) {                                       /* never raised for Livox: its times are never NaN */
+        set_error(what + ": " + deferred);
         return LV_ERR_ARG;
     }
     *n_out = h->ds.h_count[0];
@@ -1745,6 +1748,55 @@ lv_status lv_process_livox_device_async(lv_handle h, const uint8_t* d_data, int6
                               d_range, d_idx, &unused, d_n_out);
 }
 
+/* a VelodyneScan's packets (lv_wire.h): msg2points, then the decimator on the rank among its points.  The first call uploads the
+ * rotation tables, which the context keeps */
+static const char* const kVelodyneDeferred = "a packet is a dual-return one (not decoded) or its stamp has nsec >= 10^9";
+static cudaError_t velodyne_tables_ready(lv_handle h) {
+    if (h->velodyne_tables_ok) return cudaSuccess;
+    std::vector<float> t(2 * kVelodyneTable);
+    velodyne_tables(t.data(), t.data() + kVelodyneTable);
+    cudaError_t e = h->d_velodyne_tables.reserve(t.size());
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->d_velodyne_tables, t.data(), t.size() * sizeof(float), cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);   /* t is pageable and goes out of scope */
+    h->velodyne_tables_ok = e == cudaSuccess;
+    return e;
+}
+static lv_status process_velodyne_impl(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                       const lv_velodyne_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz,
+                                       double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out, int64_t* d_n_out) {
+    const CloudOut o{d_xyz, d_time, d_intensity, d_range, d_idx};
+    /* n_packets out of range leaves n at 0 here, and velodyne_layout_error names it */
+    const int64_t n = n_packets >= 0 && n_packets <= kVelodyneMaxPackets ? n_packets * kVelodyneSlots : 0;
+    return front_end_impl(
+        h, "process velodyne", !d_packets || !cal || !d_xyz || !d_time, "packets, cal, xyz, time or n_out", d_packets, data_bytes, n,
+        downsample_rate, o, n_out, d_n_out,
+        [&]() -> const char* {
+            if (const char* why = velodyne_layout_error(n_packets, data_bytes)) return why;
+            return velodyne_calib_finite(*cal) ? nullptr : "a calibration entry is not finite";
+        },
+        [&](int* launches, uint32_t* err) {
+            const cudaError_t e = velodyne_tables_ready(h);
+            if (e != cudaSuccess) return e;
+            const VelodyneArgs a = {d_packets, n_packets, n, h->d_velodyne_tables, velodyne_calib(*cal), downsample_rate, min_dist};
+            return launch_process_velodyne(h->ds, a, o, d_n_out, err, h->stream, launches);
+        },
+        kVelodyneDeferred);
+}
+lv_status lv_process_velodyne_device(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                     const lv_velodyne_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz,
+                                     double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out) {
+    return process_velodyne_impl(h, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range,
+                                 d_idx, n_out, nullptr);
+}
+lv_status lv_process_velodyne_device_async(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                           const lv_velodyne_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz,
+                                           double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* d_n_out) {
+    int64_t unused = 0;                                           /* the count stays on the device */
+    if (!d_n_out) { set_error("process velodyne: null packets, cal, xyz, time or n_out"); return LV_ERR_ARG; }
+    return process_velodyne_impl(h, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range,
+                                 d_idx, &unused, d_n_out);
+}
+
 /* the deferred errors of the _async calls (AsyncWords::err) and the map's flags; clears the former */
 lv_status lv_async_status(lv_handle h) {
     if (!h) return LV_ERR_ARG;
@@ -1765,6 +1817,7 @@ lv_status lv_async_status(lv_handle h) {
             msg += "lidar merge: the message or the buffered points after its first time are not time-ordered (appended as a push does); ";
         if (err & kAsyncLidarOverlap)
             msg += "lidar merge: the message reaches back over more buffered points than the merge reserve (nothing merged; lv_lidar_reserve_merge); ";
+        if (err & kAsyncVelodyne) msg += std::string("process velodyne: ") + kVelodyneDeferred + "; ";
         msg.resize(msg.size() - 2);
         set_error(msg);
         return LV_ERR_ARG;

@@ -1,8 +1,8 @@
 /*
  * lv_cloud.cu — Accumulator::process (src/Modules/Accumulator.cpp:142-151) on the device: the raw bytes of a LiDAR message in
  * HBM -> msg2points (PointCloudProcessor.cpp:24-99) -> temporal_downsample (:101-112) -> sort_points (:114-123), with the
- * per-point arithmetic of lv_wire.h that the host decoders run too.  One pipeline serves two message formats; a point source
- * (Pc2Source, LivoxSource) says where a point's fields are and how its time is computed.
+ * per-point arithmetic of lv_wire.h that the host decoders run too.  One pipeline serves three message formats; a point source
+ * (Pc2Source, LivoxSource, VelodyneSource) says where a point's fields are and how its time is computed.
  *
  *   flag     every point of the message: xyz from its bytes -> temporal_keep on the rank
  *   select   cub::DeviceSelect::Flagged: indices of the kept points, in message order
@@ -12,8 +12,10 @@
  *   gather   every output point: xyz / time / intensity / range decoded again from its bytes, and its raw index
  * sensor_msgs/PointCloud2: the rank is the message index.  livox CustomMsg: msg2points drops points by tag first, so a tag flag
  * and its select come first, and the rank is the position among the tag-kept points (Accumulator.cpp:143-151 decimates the list
- * msg2points returns).  The bytes of a kept point are read twice (flag + key, gather), those of a dropped point once.  Every value
- * is assembled from single bytes (lv_wire.h): fields sit at any offset and the message at any address.  Byte offsets are
+ * msg2points returns).  velodyne_msgs/VelodyneScan likewise: a validity flag (return mode, block flags, distance) and its select
+ * come first, and the key kernel also checks every packet for a dual return or a stamp that does not convert (the flag kernel
+ * resets that word, so the first kernel cannot raise it).  The bytes of a kept point are read twice (flag + key, gather), those
+ * of a dropped point once.  Every value is assembled from single bytes (lv_wire.h): fields sit at any offset and the message at any address.  Byte offsets are
  * 64-bit: n < 2^31 points of up to 2^31 bytes each.
  *
  * Also Processor::fill's header stamp (PointCloudProcessor.cpp:125-133) of a cloud the publishers send: one block, a max-reduction.
@@ -41,6 +43,7 @@ struct Pc2Source {
     }
     __device__ __forceinline__ float intensity(const uint8_t* p) const { return wire_intensity(a.type, a.layout, p); }
     __device__ __forceinline__ float range(const uint8_t* p, float x, float y, float z) const { return wire_range(a.type, a.layout, p, x, y, z); }
+    __device__ __forceinline__ void check(int64_t, int64_t, int*, uint32_t*) const {}
 };
 
 /* livox CustomMsg: 19-byte records, time = timebase + offset_time, intensity = reflectivity, range = |p| */
@@ -53,6 +56,35 @@ struct LivoxSource {
     __device__ __forceinline__ double time(const uint8_t* p) const { return livox_time(a.timebase_ns, p); }
     __device__ __forceinline__ float intensity(const uint8_t* p) const { return livox_reflectivity(p); }
     __device__ __forceinline__ float range(const uint8_t*, float x, float y, float z) const { return wire_norm(x, y, z); }
+    __device__ __forceinline__ void check(int64_t, int64_t, int*, uint32_t*) const {}
+};
+
+/* velodyne_msgs/VelodyneScan: a point is a slot (its packet and r), decoded through the rotation tables and the calibration */
+struct VelodyneSlot {
+    const uint8_t* pkt;
+    int r;
+};
+struct VelodyneSource {
+    VelodyneArgs a;
+    __device__ __forceinline__ VelodyneSlot point(int64_t i) const {
+        return {velodyne_packet(a.data, i / kVelodyneSlots), (int)(i % kVelodyneSlots)};
+    }
+    __device__ __forceinline__ void xyz(const VelodyneSlot& p, float& x, float& y, float& z) const {
+        velodyne_xyz(p.pkt, p.r, a.table, a.table + kVelodyneTable, a.cal, x, y, z);
+    }
+    __device__ __forceinline__ double time(const VelodyneSlot& p) const { return velodyne_time(p.pkt, p.r); }
+    __device__ __forceinline__ float intensity(const VelodyneSlot& p) const { return velodyne_reflectivity(p.pkt, p.r); }
+    __device__ __forceinline__ float range(const VelodyneSlot&, float x, float y, float z) const { return wire_norm(x, y, z); }
+    /* packets k = j, j + stride, ...: a dual-return packet or a stamp that does not convert raises s.count[1] and kAsyncVelodyne */
+    __device__ __forceinline__ void check(int64_t j, int64_t stride, int* count, uint32_t* err) const {
+        for (int64_t k = j; k < a.n_packets; k += stride) {
+            const uint8_t* pkt = velodyne_packet(a.data, k);
+            if (velodyne_mode(pkt) == kVelodyneDualReturn || !velodyne_stamp_ok(pkt)) {
+                count[1] = 1;
+                if (err) atomicOr(err, kAsyncVelodyne);
+            }
+        }
+    }
 };
 
 /* std::stable_sort with `<` on doubles: -0.0 and +0.0 are equal (message order), so -0.0 is folded onto +0.0; then the
@@ -77,6 +109,13 @@ __global__ void __launch_bounds__(256) lv_cloud_flag_kernel(Src s, const int32_t
     keep[j] = temporal_keep(j, s.a.rate, s.a.min_dist, x, y, z) ? 1 : 0;
 }
 
+/* msg2points of a VelodyneScan: the slots that are points (velodyne_slot_valid) */
+__global__ void __launch_bounds__(256) lv_velodyne_valid_kernel(VelodyneArgs a, uint8_t* __restrict__ keep) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    keep[i] = velodyne_slot_valid(velodyne_packet(a.data, i / kVelodyneSlots), (int)(i % kVelodyneSlots)) ? 1 : 0;
+}
+
 /* msg2points' tag filter of a livox message */
 __global__ void __launch_bounds__(256) lv_livox_tag_kernel(LivoxArgs a, uint8_t* __restrict__ keep) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -90,6 +129,7 @@ __global__ void __launch_bounds__(256) lv_cloud_key_kernel(Src s, const int32_t*
                                                            uint32_t* __restrict__ err) {
     const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= bound) return;
+    s.check(j, bound, count, err);            /* the message's own deferred errors (VelodyneScan: per packet) */
     if (j >= count[0]) {                      /* padding: sorts behind every kept point */
         keys[j] = ~0ull;
         vals[j] = 0xffffffffu;
@@ -114,7 +154,7 @@ __global__ void __launch_bounds__(256) lv_cloud_gather_kernel(Src s, const uint3
     if (r == 0 && n_out) *n_out = count[0];
     if (r >= count[0]) return;
     const uint32_t i = order[r];
-    const uint8_t* p = s.point(i);
+    const auto p = s.point(i);
     float x, y, z;
     s.xyz(p, x, y, z);
     xyz[3 * r] = x; xyz[3 * r + 1] = y; xyz[3 * r + 2] = z;
@@ -166,6 +206,23 @@ cudaError_t launch_process_livox(DownsampleScratch& s, const LivoxArgs& a, const
     if (e != cudaSuccess) return e;
     lv_cloud_flag_kernel<<<grid, 256, 0, st>>>(src, tag_sel, s.count.get() + 2, s.flags, s.count);
     e = launch_select_sort_gather(s, src, static_cast<const int32_t*>(tag_sel), o, d_n_out, err, st);
+    if (e == cudaSuccess && launches) *launches += 9;
+    return e;
+}
+
+cudaError_t launch_process_velodyne(DownsampleScratch& s, const VelodyneArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err,
+                                    cudaStream_t st, int* launches) {
+    const VelodyneSource src{a};
+    const unsigned grid = (unsigned)((a.n + 255) / 256);
+    /* as for livox: the msg2points slots live in vals_sorted until the second select has read them */
+    int32_t* valid_sel = reinterpret_cast<int32_t*>(s.vals_sorted.get());
+    lv_velodyne_valid_kernel<<<grid, 256, 0, st>>>(a, s.flags);
+    size_t tmp = s.tmp.size();
+    cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags.get(), valid_sel, s.count.get() + 2,
+                                               (int)a.n, st);
+    if (e != cudaSuccess) return e;
+    lv_cloud_flag_kernel<<<grid, 256, 0, st>>>(src, valid_sel, s.count.get() + 2, s.flags, s.count);
+    e = launch_select_sort_gather(s, src, static_cast<const int32_t*>(valid_sel), o, d_n_out, err, st);
     if (e == cudaSuccess && launches) *launches += 9;
     return e;
 }

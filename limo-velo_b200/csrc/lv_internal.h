@@ -12,6 +12,7 @@
 #include "lv_ieskf.h"
 #include "lv_preloc_bound.h"
 #include "lv_voxel_search.h"
+#include "lv_wire.h"
 
 namespace lv {
 
@@ -21,7 +22,7 @@ enum { kNumSMs = 132 };
 /* The stream-ordered (_async) entry points report errors through one device word of the handle, read and cleared by
  * lv_async_status.  Bits: */
 enum : uint32_t { kAsyncCloudNaN = 1u, kAsyncDeskewPath = 2u, kAsyncCount = 4u, kAsyncLidarFull = 8u, kAsyncLidarWindow = 16u,
-                  kAsyncLidarUnsorted = 32u, kAsyncLidarOverlap = 64u };
+                  kAsyncLidarUnsorted = 32u, kAsyncLidarOverlap = 64u, kAsyncVelodyne = 128u };
 /* device words of the async tick: the deferred errors and what lv_correct_device_async decided */
 struct AsyncWords {
     uint32_t err;              /* kAsync* bits since the last lv_async_status              */
@@ -200,8 +201,9 @@ struct DownsampleScratch {
     DeviceBuf<int32_t> sel;
     DeviceBuf<uint8_t> tmp;        /* cub's temporary storage: tmp.size() bytes */
     DeviceBuf<GridBox> box;
-    DeviceBuf<int> count;          /* [0] output count, [1] NaN-time flag, [2] tag-kept count of a livox message (lv_cloud.cu) */
-    PinnedBuf<int> h_count;        /* [0] output count, [1] overflow flag (voxel grid) / NaN-time flag (cloud) */
+    DeviceBuf<int> count;          /* [0] output count, [1] NaN-time flag (velodyne: packet flag), [2] tag-kept count of a livox
+                                    * message / point count of a velodyne one (lv_cloud.cu) */
+    PinnedBuf<int> h_count;        /* [0] output count, [1] overflow flag (voxel grid) / NaN-time or packet flag (cloud) */
 };
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n);
 /* the attribute lanes of a full voxel grid (lv_voxelgrid_downsample_full): the inputs (intensity summed per leaf; time read by
@@ -253,6 +255,20 @@ struct LivoxArgs {
 };
 cudaError_t launch_process_livox(DownsampleScratch& s, const LivoxArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err, cudaStream_t st,
                                  int* launches);
+/* the same for a velodyne_msgs/VelodyneScan: msg2points (return mode, block flags, distance), then the decimator on the rank among
+ * its points (lv_wire.h).  s.h_count[1] = 1 (after a stream sync) and err gets kAsyncVelodyne when a packet is a dual-return one or
+ * its stamp does not convert */
+struct VelodyneArgs {
+    const uint8_t* data;       /* the packets (device, any alignment) */
+    int64_t n_packets;
+    int64_t n;                 /* 384 n_packets slots */
+    const float* table;        /* C then S, kVelodyneTable floats each (velodyne_tables, device) */
+    VelodyneCalib cal;
+    int32_t rate;
+    double min_dist;
+};
+cudaError_t launch_process_velodyne(DownsampleScratch& s, const VelodyneArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err,
+                                    cudaStream_t st, int* launches);
 /* Processor::fill's header stamp (PointCloudProcessor.cpp:125-133): *d_stamp_us = max over the *d_n (clamped to [0, n_max]) times of
  * round(t * 1e6) as uint64 (Conversions::sec2Microsec, Utils.cpp:14-16), 0 for no point.  One launch */
 cudaError_t launch_cloud_stamp(const double* d_time, const int64_t* d_n, int64_t n_max, uint64_t* d_stamp_us, uint32_t* err, cudaStream_t st,

@@ -1,6 +1,7 @@
 /*
- * lv_wire.h — the per-point arithmetic of the LiDAR message, compiled by the host (lv_pointcloud2_to_points, lv_livox_to_points)
- * and the device (lv_process_cloud_device, lv_process_livox_device, the temporal decimator) alike, so that both give the same bits:
+ * lv_wire.h — the per-point arithmetic of the LiDAR message, compiled by the host (lv_pointcloud2_to_points, lv_livox_to_points,
+ * lv_velodyne_to_points) and the device (lv_process_cloud_device, lv_process_livox_device, lv_process_velodyne_device, the temporal
+ * decimator) alike, so that both give the same bits:
  *   PointCloudProcessor::msg2points / get_begin_time   src/Utils/PointCloudProcessor.cpp:24-99
  *   Point(const <driver>::Point&, double time_offset)   src/Objects/Point.cpp:37-111,153-175
  *   Conversions::microsec2Sec / nanosec2Sec             src/Utils/Utils.cpp:18-30
@@ -120,6 +121,13 @@ inline const char* cloud_layout_error(lv_lidar_type type, const lv_cloud_layout&
     return nullptr;
 }
 
+/* an absolute time in uint64 ns -> seconds as Conversions::nanosec2Sec (Utils.cpp:25-30) but with a 64-bit quotient: the
+ * reference's int cast would truncate epoch seconds */
+LV_HD double wire_ns_to_sec(uint64_t total) {
+    const uint64_t order = 1000000000ull;
+    return dadd((double)(int64_t)(total / order), dmul((double)(total % order), 1e-9));
+}
+
 /* ---- livox_ros_driver(2)/CustomMsg: one uint64 time base (ns) per message, then packed 19-byte records
  *   uint32 offset_time (ns after timebase) | float32 x | float32 y | float32 z | uint8 reflectivity | uint8 tag | uint8 line
  * A record starts at data + 19 i, at any address. */
@@ -130,13 +138,8 @@ constexpr uint64_t kLivoxTimebaseMax = 0xFFFFFFFF00000000ull;
 LV_HD const uint8_t* livox_point(const uint8_t* data, int64_t i) { return data + (uint64_t)i * (uint64_t)kLivoxRecord; }
 LV_HD uint32_t livox_tag(const uint8_t* p) { return wire_u8(p + 17); }
 LV_HD float livox_reflectivity(const uint8_t* p) { return (float)wire_u8(p + 16); }
-/* total = timebase + offset_time (ns, uint64), then seconds as Conversions::nanosec2Sec (Utils.cpp:25-30) but with a 64-bit
- * quotient: the reference's int cast would truncate epoch seconds */
-LV_HD double livox_time(uint64_t timebase, const uint8_t* p) {
-    const uint64_t total = timebase + (uint64_t)wire_u32(p);
-    const uint64_t order = 1000000000ull;
-    return dadd((double)(int64_t)(total / order), dmul((double)(total % order), 1e-9));
-}
+/* total = timebase + offset_time (ns, uint64), in seconds */
+LV_HD double livox_time(uint64_t timebase, const uint8_t* p) { return wire_ns_to_sec(timebase + (uint64_t)wire_u32(p)); }
 /* the tag filter of msg2points: bits of the tag set in the mask drop the point (0 keeps every point) */
 LV_HD bool livox_tag_keep(const uint8_t* p, uint32_t tag_reject_mask) { return (livox_tag(p) & tag_reject_mask) == 0; }
 
@@ -145,6 +148,107 @@ inline const char* livox_layout_error(int64_t n, int64_t data_bytes, uint64_t ti
     if (n < 0 || data_bytes < 0) return "negative point count or data length";
     if (n > data_bytes / kLivoxRecord) return "data_bytes is too short for n records of 19 bytes";
     if (timebase_ns > kLivoxTimebaseMax) return "timebase above 2^64 - 2^32 ns (timebase + offset_time could wrap)";
+    return nullptr;
+}
+
+/* ---- velodyne_msgs/VelodyneScan of a VLP-16 / Puck Hi-Res (include/limovelo_b200.h, "Velodyne packets"): packets of 1214 bytes
+ *   uint32 stamp.sec | uint32 stamp.nsec | uint8[1206] data
+ * at packets + 1214 k, any alignment.  data: 12 blocks of 100 bytes (uint16 flag 0xEEFF, uint16 azimuth in 0.01 deg, 32 x (uint16
+ * distance in 2 mm, uint8 reflectivity)), then uint32 sensor us (unused), uint8 return mode, uint8 product id (unused).
+ * Slot i of the message: packet k = i / 384, r = i % 384, block b = r / 32, firing f = (r % 32) / 16, laser l = r % 16. */
+enum { kVelodynePacket = 1214, kVelodyneSlots = 384, kVelodyneLasers = 16, kVelodyneTable = 36000 };
+enum : uint32_t { kVelodyneBlockFlag = 0xEEFFu, kVelodyneDualReturn = 0x39u };
+constexpr int64_t kVelodyneMaxPackets = 0x7fffffff / kVelodyneSlots;   /* slot indices are int32 */
+
+/* the calibration in the fp32 terms the point arithmetic reads (velodyne_calib), per laser */
+struct VelodyneCalib {
+    float cv[kVelodyneLasers], sv[kVelodyneLasers];   /* cos / sin of the vertical angle   */
+    float cr[kVelodyneLasers], sr[kVelodyneLasers];   /* cos / sin of the rotational correction */
+    float dist[kVelodyneLasers], vo[kVelodyneLasers], ho[kVelodyneLasers];
+};
+
+LV_HD const uint8_t* velodyne_packet(const uint8_t* packets, int64_t k) { return packets + (uint64_t)k * (uint64_t)kVelodynePacket; }
+LV_HD const uint8_t* velodyne_block(const uint8_t* pkt, int b) { return pkt + 8 + 100 * b; }
+LV_HD uint32_t velodyne_mode(const uint8_t* pkt) { return wire_u8(pkt + 8 + 1204); }
+LV_HD const uint8_t* velodyne_channel(const uint8_t* pkt, int r) { return velodyne_block(pkt, r / 32) + 4 + 3 * (r % 32); }
+
+/* msg2points: the packet is not a dual-return one, blocks 0 .. b all carry the flag and the slot has a return */
+LV_HD bool velodyne_slot_valid(const uint8_t* pkt, int r) {
+    if (velodyne_mode(pkt) == kVelodyneDualReturn) return false;
+    for (int c = 0; c <= r / 32; ++c)
+        if (wire_u16(velodyne_block(pkt, c)) != kVelodyneBlockFlag) return false;
+    return wire_u16(velodyne_channel(pkt, r)) != 0;
+}
+/* the packet's stamp converts: nsec < 10^9 (with 32-bit seconds the ns sum below cannot wrap a uint64) */
+LV_HD bool velodyne_stamp_ok(const uint8_t* pkt) { return wire_u32(pkt + 4) < 1000000000u; }
+
+/* the table index of slot r's azimuth: A_b plus the part of the block's azimuth step its firing time covers, rounded to 0.01 deg */
+LV_HD int velodyne_azimuth(const uint8_t* pkt, int r) {
+    const int b = r / 32, f = (r % 32) / 16, l = r % 16;
+    const int nb = b < 11 ? b + 1 : 11, pb = b < 11 ? b : 10;           /* block 11 takes block 10's step */
+    const int a_b = (int)wire_u16(velodyne_block(pkt, b) + 2);
+    int delta = ((int)wire_u16(velodyne_block(pkt, nb) + 2) + kVelodyneTable - (int)wire_u16(velodyne_block(pkt, pb) + 2)) % kVelodyneTable;
+    if (delta < 0) delta += kVelodyneTable;                            /* a raw azimuth above 36000 (not a valid packet) */
+    const float a = fadd((float)a_b, fdiv(fmul((float)delta, fadd(fmul((float)l, 2.304f), fmul((float)f, 55.296f))), 110.592f));
+    return (int)(((int64_t)roundf(a)) % kVelodyneTable);              /* a >= 0: roundf is half away from zero */
+}
+/* the point of slot r (C, S: the cos / sin tables of velodyne_tables), in the ROS frame (x forward, y left, z up) */
+LV_HD void velodyne_xyz(const uint8_t* pkt, int r, const float* C, const float* S, const VelodyneCalib& k, float& x, float& y, float& z) {
+    const int l = r % 16, q = velodyne_azimuth(pkt, r);
+    const float d = fadd(fmul((float)wire_u16(velodyne_channel(pkt, r)), 0.002f), k.dist[l]);
+    const float c = C[q], s = S[q];
+    const float cosr = fadd(fmul(c, k.cr[l]), fmul(s, k.sr[l])), sinr = fsub(fmul(s, k.cr[l]), fmul(c, k.sr[l]));
+    const float xy = fsub(fmul(d, k.cv[l]), fmul(k.vo[l], k.sv[l]));
+    const float X = fsub(fmul(xy, sinr), fmul(k.ho[l], cosr)), Y = fadd(fmul(xy, cosr), fmul(k.ho[l], sinr));
+    x = Y;
+    y = -X;
+    z = fadd(fmul(d, k.sv[l]), fmul(k.vo[l], k.cv[l]));
+}
+LV_HD float velodyne_reflectivity(const uint8_t* pkt, int r) { return (float)wire_u8(velodyne_channel(pkt, r) + 2); }
+/* the packet stamp is its first firing's time; firing sequence 2b + f starts 55.296 us after the previous, laser l fires 2.304 us
+ * into it */
+LV_HD double velodyne_time(const uint8_t* pkt, int r) {
+    const int b = r / 32, f = (r % 32) / 16, l = r % 16;
+    const uint64_t total = (uint64_t)wire_u32(pkt) * 1000000000ull + (uint64_t)wire_u32(pkt + 4) + (uint64_t)(2 * b + f) * 55296ull +
+                           (uint64_t)l * 2304ull;
+    return wire_ns_to_sec(total);
+}
+
+/* host code from here.  C[q] = cos(q 0.01 deg), S[q] = sin(q 0.01 deg) for q in [0, 36000): computed in double, rounded to float.  The host decoder and
+ * the device tables both come from here, so both read the same bits */
+inline void velodyne_tables(float* C, float* S) {
+    for (int q = 0; q < kVelodyneTable; ++q) {
+        const double a = (double)q * 0.01 * M_PI / 180.0;
+        C[q] = (float)cos(a);
+        S[q] = (float)sin(a);
+    }
+}
+inline bool velodyne_calib_finite(const lv_velodyne_calibration& c) {
+    for (int l = 0; l < kVelodyneLasers; ++l)
+        if (!isfinite(c.vert_correction[l]) || !isfinite(c.rot_correction[l]) || !isfinite(c.dist_correction[l]) ||
+            !isfinite(c.vert_offset_correction[l]) || !isfinite(c.horiz_offset_correction[l]))
+            return false;
+    return true;
+}
+inline VelodyneCalib velodyne_calib(const lv_velodyne_calibration& c) {
+    VelodyneCalib k;
+    for (int l = 0; l < kVelodyneLasers; ++l) {
+        k.cv[l] = (float)cos(c.vert_correction[l]);
+        k.sv[l] = (float)sin(c.vert_correction[l]);
+        k.cr[l] = (float)cos(c.rot_correction[l]);
+        k.sr[l] = (float)sin(c.rot_correction[l]);
+        k.dist[l] = (float)c.dist_correction[l];
+        k.vo[l] = (float)c.vert_offset_correction[l];
+        k.ho[l] = (float)c.horiz_offset_correction[l];
+    }
+    return k;
+}
+
+/* NULL when n_packets is in range and its packets fit data_bytes, else what is wrong */
+inline const char* velodyne_layout_error(int64_t n_packets, int64_t data_bytes) {
+    if (n_packets < 0 || data_bytes < 0) return "negative packet count or data length";
+    if (n_packets > kVelodyneMaxPackets) return "n_packets above (2^31 - 1) / 384 (slot indices are int32)";
+    if (n_packets > data_bytes / kVelodynePacket) return "data_bytes is too short for n_packets packets of 1214 bytes";
     return nullptr;
 }
 

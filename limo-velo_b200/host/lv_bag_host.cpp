@@ -20,6 +20,7 @@
  * x y z intensity(u8) timestamp(f64); ouster x y z reflectivity(u16) t(u32) range(u32); custom like hesai with f32
  * intensity), ready for lv_pointcloud2_to_points; sensor_msgs/Imu -> stamp, orientation, angular velocity, acceleration.
  * Livox sensors publish livox_ros_driver/CustomMsg instead of PointCloud2: lv_bag_parse_livox -> a view of its 19-byte records.
+ * A Velodyne driver that records packets publishes velodyne_msgs/VelodyneScan: lv_bag_parse_velodyne_scan -> a view of its packets.
  * Everything is host code: a sweep is a few MB per 100 ms.
  */
 #include <stdio.h>
@@ -307,6 +308,24 @@ lv_status lv_bag_parse_livox(const uint8_t* data, int64_t size, lv_livox_view* o
     out->n_points = count;
     out->data = recs;
     out->data_bytes = (int64_t)count * lv::kLivoxRecord;
+    return LV_OK;
+}
+
+lv_status lv_bag_parse_velodyne_scan(const uint8_t* data, int64_t size, lv_velodyne_view* out) {
+    if (!data || !out || size < 0) return LV_ERR_ARG;
+    memset(out, 0, sizeof(*out));
+    Rd r(data, size);
+    r.u32();                                          /* std_msgs/Header: seq, stamp, frame_id */
+    const uint32_t sec = r.u32(), nsec = r.u32();
+    r.str();
+    const uint32_t count = r.u32();                   /* VelodynePacket[]: time stamp, uint8[1206] data (fixed, no length prefix) */
+    const uint8_t* packets = r.take((int64_t)count * lv::kVelodynePacket);
+    if (!r.ok || r.at != size) return LV_ERR_ARG;
+    out->stamp_sec = sec;
+    out->stamp_nsec = nsec;
+    out->n_packets = count;
+    out->packets = packets;
+    out->data_bytes = (int64_t)count * lv::kVelodynePacket;
     return LV_OK;
 }
 

@@ -6,10 +6,13 @@
  *   PointCloudProcessor::sort_points                                src/Utils/PointCloudProcessor.cpp:114-123
  * One pass over the message bytes per sweep (a few MB); the per-point arithmetic is csrc/lv_wire.h, which
  * lv_process_cloud_device (csrc/lv_cloud.cu) runs on the device.  lv_livox_to_points is the same for a Livox CustomMsg
- * (lv_process_livox_device on the device).
+ * (lv_process_livox_device on the device), lv_velodyne_to_points for a VelodyneScan's packets (lv_process_velodyne_device).
  */
+#include <math.h>
+
 #include <algorithm>
 #include <numeric>
+#include <vector>
 
 #include "../../include/limovelo_b200.h"
 #include "../csrc/lv_wire.h"
@@ -47,6 +50,47 @@ lv_status lv_livox_to_points(const uint8_t* data, int64_t data_bytes, int64_t n,
         xyz[3 * m] = x; xyz[3 * m + 1] = y; xyz[3 * m + 2] = z;
         time[m] = lv::livox_time(timebase_ns, p);
         if (intensity) intensity[m] = lv::livox_reflectivity(p);
+        if (range) range[m] = lv::wire_norm(x, y, z);
+        if (idx) idx[m] = (int32_t)i;
+        ++m;
+    }
+    *n_out = m;
+    return LV_OK;
+}
+
+lv_status lv_velodyne_default_calibration(lv_velodyne_model model, lv_velodyne_calibration* out) {
+    static const double vlp16[16] = {-15, 1, -13, 3, -11, 5, -9, 7, -7, 9, -5, 11, -3, 13, -1, 15};
+    static const double hires[16] = {-10, 0.67, -8.67, 2, -7.33, 3.33, -6, 4.67, -4.67, 6, -3.33, 7.33, -2, 8.67, -0.67, 10};
+    if (!out || (model != LV_VELODYNE_VLP16 && model != LV_VELODYNE_PUCK_HIRES)) return LV_ERR_ARG;
+    *out = lv_velodyne_calibration{};
+    for (int l = 0; l < 16; ++l) out->vert_correction[l] = (model == LV_VELODYNE_VLP16 ? vlp16 : hires)[l] * M_PI / 180.0;
+    return LV_OK;
+}
+
+lv_status lv_velodyne_to_points(const uint8_t* packets, int64_t data_bytes, int64_t n_packets, const lv_velodyne_calibration* cal,
+                                float* xyz, double* time, float* intensity, float* range, int32_t* idx, int64_t* n_out) {
+    if (n_out) *n_out = 0;
+    if (!packets || !cal || !xyz || !time || !n_out || lv::velodyne_layout_error(n_packets, data_bytes) || !lv::velodyne_calib_finite(*cal))
+        return LV_ERR_ARG;
+    for (int64_t k = 0; k < n_packets; ++k)
+        if (!lv::velodyne_stamp_ok(lv::velodyne_packet(packets, k))) return LV_ERR_ARG;
+    static const std::vector<float> tables = [] {
+        std::vector<float> t(2 * lv::kVelodyneTable);
+        lv::velodyne_tables(t.data(), t.data() + lv::kVelodyneTable);
+        return t;
+    }();
+    const float *C = tables.data(), *S = C + lv::kVelodyneTable;
+    const lv::VelodyneCalib k = lv::velodyne_calib(*cal);
+    int64_t m = 0;
+    for (int64_t i = 0; i < n_packets * lv::kVelodyneSlots; ++i) {
+        const uint8_t* pkt = lv::velodyne_packet(packets, i / lv::kVelodyneSlots);
+        const int r = (int)(i % lv::kVelodyneSlots);
+        if (!lv::velodyne_slot_valid(pkt, r)) continue;
+        float x, y, z;
+        lv::velodyne_xyz(pkt, r, C, S, k, x, y, z);
+        xyz[3 * m] = x; xyz[3 * m + 1] = y; xyz[3 * m + 2] = z;
+        time[m] = lv::velodyne_time(pkt, r);
+        if (intensity) intensity[m] = lv::velodyne_reflectivity(pkt, r);
         if (range) range[m] = lv::wire_norm(x, y, z);
         if (idx) idx[m] = (int32_t)i;
         ++m;

@@ -106,3 +106,27 @@ for d in (d_t, d_n, d_s):
     loc.device_free(d)
 loc.close()
 print("sanitize target: full points ok", flush=True)
+
+# the Velodyne packet front end (lv_process_velodyne_device, both forms): packets at an odd device address, a bad block flag, a
+# dual-return packet and a stamp that does not convert (the deferred flag), against the restatement
+import ctypes as C
+import velodyne_cases as VC
+loc = lv.Localizer(lv.default_params(max_points=1 << 14, max_map_points=1 << 13))
+cal = lv.velodyne_calibration()
+outs = [loc.device_alloc(k * 384 * 20) for k in (12, 8, 4, 4, 4)]
+d_msg, d_n = loc.device_alloc(1214 * 20 + 8), loc.device_alloc(8)
+for name, pk in (("scan", VC.packets(rng, 20)), ("flags", VC.edge_packets(rng)["bad_flags"]), ("dual", VC.dual_packets(rng))):
+    ref = VC.process(pk, cal, 2, 0.5)
+    raw = np.frombuffer(pk.tobytes(), np.uint8)
+    assert loc.L.lv_memcpy_h2d(loc.h, C.c_void_p(d_msg + 1), raw.ctypes.data_as(C.c_void_p), raw.nbytes) == 0
+    loc.process_velodyne_device_async(d_msg + 1, raw.nbytes, len(pk), cal, 2, 0.5, outs[0], outs[1], d_n, *outs[2:])
+    m = int(loc.download(d_n, np.zeros(1, np.int64))[0])
+    got = [loc.download(d, np.empty_like(a)) for d, a in zip(outs, ref)]
+    assert m == len(ref[0]) and all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(got, ref)), name
+    assert loc.async_status()[0] == (lv.ERR_ARG if name == "dual" else lv.OK), name
+    if name != "dual":
+        assert loc.process_velodyne_device(d_msg + 1, raw.nbytes, len(pk), cal, 2, 0.5, *outs) == len(ref[0])
+for d in outs + [d_msg, d_n]:
+    loc.device_free(d)
+loc.close()
+print("sanitize target: process velodyne ok", flush=True)
