@@ -216,6 +216,14 @@ def lib():
         L.lv_process_velodyne_device.argtypes = [vp, vp, i64, i64, cp, C.c_int32, C.c_double, vp, vp, vp, vp, vp, C.POINTER(i64)]
         L.lv_process_velodyne_device_async.argtypes = [vp, vp, i64, i64, cp, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
         L.lv_bag_parse_velodyne_scan.argtypes = [vp, i64, C.POINTER(VelodyneView)]
+    if hasattr(L, "lv_process_ouster_device"):   # the Ouster packet front end; absent from older builds
+        cp = C.POINTER(OusterCalibration)
+        L.lv_ouster_calibration_from_json.argtypes = [C.c_char_p, i64, cp]
+        L.lv_ouster_to_points.argtypes = [vp, i64, i64, cp, vp, vp, vp, vp, vp, C.POINTER(i64)]
+        L.lv_process_ouster_device.argtypes = [vp, vp, i64, i64, cp, C.c_int32, C.c_double, vp, vp, vp, vp, vp, C.POINTER(i64)]
+        L.lv_process_ouster_device_async.argtypes = [vp, vp, i64, i64, cp, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
+        L.lv_bag_parse_ouster_packet.argtypes = [vp, i64, C.POINTER(OusterPacketView)]
+        L.lv_ouster_imu_packet.argtypes = [vp, i64, C.POINTER(ImuSample)]
     if hasattr(L, "lv_lidar_reserve_merge"):   # the time-ordered merge of several LiDARs; absent from older builds
         L.lv_lidar_reserve_merge.argtypes = [vp, i64]
         L.lv_lidar_merge_device_async.argtypes = [vp, vp, vp, vp, i64, fp]
@@ -492,6 +500,78 @@ def velodyne_to_points(packets, cal):
     m = C.c_int64(0)
     _check(lib().lv_velodyne_to_points(raw.ctypes.data_as(C.c_void_p), len(raw), k, C.byref(cal),
                                        *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
+    return tuple(a[:m.value].copy() for a in out)
+
+
+# ouster_ros/PacketMsg of an Ouster in the LEGACY profile: packets of 16 columns of 20 + 12 H bytes (include/limovelo_b200.h)
+OUSTER_COLUMNS = 16
+OUSTER_IMU_PACKET = 48
+
+
+def ouster_packet_bytes(H):
+    return OUSTER_COLUMNS * (20 + 12 * H)
+
+
+class OusterCalibration(C.Structure):
+    _fields_ = [("columns_per_frame", C.c_int32), ("pixels_per_column", C.c_int32), ("beam_altitude_angles", C.c_double * 128),
+                ("beam_azimuth_angles", C.c_double * 128), ("lidar_origin_to_beam_origin_mm", C.c_double)]
+
+
+class OusterPacketView(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("bytes", C.c_int64)]
+
+
+class ImuSample(C.Structure):
+    """lv_imu_sample: what Accumulator::receive_imu reads"""
+    _fields_ = [("stamp_sec", C.c_uint32), ("stamp_nsec", C.c_uint32), ("orientation", C.c_double * 4),
+                ("angular_velocity", C.c_double * 3), ("linear_acceleration", C.c_double * 3)]
+
+
+def ouster_calibration(W, altitude_deg, azimuth_deg, origin_mm=0.0):
+    """an OusterCalibration from W (columns per frame) and the per-beam angles in degrees (H = their count)"""
+    cal = OusterCalibration()
+    cal.columns_per_frame, cal.pixels_per_column = int(W), len(altitude_deg)
+    for p, (a, z) in enumerate(zip(altitude_deg, azimuth_deg)):
+        cal.beam_altitude_angles[p], cal.beam_azimuth_angles[p] = float(a), float(z)
+    cal.lidar_origin_to_beam_origin_mm = float(origin_mm)
+    return cal
+
+
+def ouster_calibration_from_json(text):
+    """lv_ouster_calibration_from_json on the sensor metadata (str or bytes): an OusterCalibration"""
+    raw = text.encode() if isinstance(text, str) else bytes(text)
+    cal = OusterCalibration()
+    _check(lib().lv_ouster_calibration_from_json(raw, len(raw), C.byref(cal)))
+    return cal
+
+
+def bag_parse_ouster_packet(msg):
+    """lv_bag_parse_ouster_packet on a serialised PacketMsg (bytes): the packet's bytes"""
+    v = OusterPacketView()
+    buf = C.create_string_buffer(bytes(msg), len(msg))
+    _check(lib().lv_bag_parse_ouster_packet(buf, len(msg), C.byref(v)))
+    off = v.data - C.addressof(buf) if v.bytes else 0
+    return buf.raw[off:off + v.bytes]
+
+
+def ouster_imu_packet(pkt):
+    """lv_ouster_imu_packet on the 48 bytes of an IMU packet: an ImuSample"""
+    raw = bytes(pkt)
+    s = ImuSample()
+    _check(lib().lv_ouster_imu_packet(raw, len(raw), C.byref(s)))
+    return s
+
+
+def ouster_to_points(packets, cal):
+    """msg2points of Ouster LEGACY packets on the host (packets: their bytes): returns (xyz, time, intensity, range, slot) of the
+    points, in slot order"""
+    raw = np.ascontiguousarray(np.frombuffer(bytes(memoryview(packets)), np.uint8))
+    k = len(raw) // ouster_packet_bytes(cal.pixels_per_column)
+    n = OUSTER_COLUMNS * cal.pixels_per_column * k
+    out = (np.empty((n, 3), np.float32), np.empty(n), np.empty(n, np.float32), np.empty(n, np.float32), np.empty(n, np.int32))
+    m = C.c_int64(0)
+    _check(lib().lv_ouster_to_points(raw.ctypes.data_as(C.c_void_p), len(raw), k, C.byref(cal),
+                                     *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
     return tuple(a[:m.value].copy() for a in out)
 
 
@@ -822,6 +902,32 @@ class Localizer:
             for d in bufs:
                 self.device_free(d)
 
+    def process_ouster_device(self, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity=None,
+                              d_range=None, d_idx=None):
+        """Accumulator::process on Ouster LEGACY packets already in device memory (raw pointers); returns the points kept"""
+        m = C.c_int64(0)
+        _check(self.L.lv_process_ouster_device(self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal),
+                                               int(downsample_rate), float(min_dist), C.c_void_p(d_xyz), C.c_void_p(d_time),
+                                               C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx), C.byref(m)))
+        return m.value
+
+    def process_ouster(self, packets, cal, downsample_rate, min_dist):
+        """Accumulator::process on Ouster LEGACY packets (their bytes): uploads them, returns (xyz, time, intensity, range, slot) of the
+        kept points in time order"""
+        raw = np.frombuffer(bytes(memoryview(packets)), np.uint8)
+        k = len(raw) // ouster_packet_bytes(cal.pixels_per_column)
+        n = OUSTER_COLUMNS * cal.pixels_per_column * k
+        out = (np.empty((n, 3), np.float32), np.empty(n, np.float64), np.empty(n, np.float32), np.empty(n, np.float32),
+               np.empty(n, np.int32))
+        bufs = [self.device_alloc(max(raw.nbytes, 1))] + [self.device_alloc(max(a.nbytes, 1)) for a in out]
+        try:
+            _check(self.L.lv_memcpy_h2d(self.h, bufs[0], raw.ctypes.data_as(C.c_void_p), raw.nbytes))
+            m = self.process_ouster_device(bufs[0], raw.nbytes, k, cal, downsample_rate, min_dist, *bufs[1:])
+            return tuple(self.download(d, a[:m]) for a, d in zip(out, bufs[1:]))
+        finally:
+            for d in bufs:
+                self.device_free(d)
+
     def download(self, d_ptr, out):
         """copy device memory into the contiguous numpy array `out` (its whole size); returns out"""
         if out.nbytes:
@@ -867,6 +973,14 @@ class Localizer:
                                       d_intensity=None, d_range=None, d_idx=None):
         """lv_process_velodyne_device with the count of kept points written to d_n_out"""
         return _check(self.L.lv_process_velodyne_device_async(
+            self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal), int(downsample_rate), float(min_dist),
+            C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
+            C.c_void_p(d_n_out)))
+
+    def process_ouster_device_async(self, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_n_out,
+                                    d_intensity=None, d_range=None, d_idx=None):
+        """lv_process_ouster_device with the count of kept points written to d_n_out"""
+        return _check(self.L.lv_process_ouster_device_async(
             self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal), int(downsample_rate), float(min_dist),
             C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
             C.c_void_p(d_n_out)))

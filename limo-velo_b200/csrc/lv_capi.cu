@@ -101,6 +101,8 @@ struct lv_context {
     DownsampleScratch ds;              /* downsamplers: grows with the largest cloud seen */
     DeviceBuf<float> d_velodyne_tables;   /* cos then sin of the 36000 azimuths (velodyne_tables): the first Velodyne call */
     bool velodyne_tables_ok = false;      /* uploaded: a failed upload is retried on the next call */
+    DeviceBuf<float> d_ouster_table;      /* cos then sin of the 2048 column angles (ouster_table): the first Ouster call */
+    bool ouster_table_ok = false;         /* uploaded: a failed upload is retried on the next call */
     DeviceBuf<float> d_ds_in;          /* staging for the host-buffer variants (ds_stage) */
     DeviceBuf<float> d_ds_out;
     DeviceBuf<uint8_t> d_ds_lanes;     /* attribute staging of lv_voxelgrid_downsample_full: 28 B per point */
@@ -1795,6 +1797,55 @@ lv_status lv_process_velodyne_device_async(lv_handle h, const uint8_t* d_packets
     if (!d_n_out) { set_error("process velodyne: null packets, cal, xyz, time or n_out"); return LV_ERR_ARG; }
     return process_velodyne_impl(h, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range,
                                  d_idx, &unused, d_n_out);
+}
+
+/* Ouster LEGACY packets (lv_wire.h): msg2points, then the decimator on the rank among its points.  The first call uploads the column
+ * table, which the context keeps */
+static cudaError_t ouster_table_ready(lv_handle h) {
+    if (h->ouster_table_ok) return cudaSuccess;
+    std::vector<float> t(2 * kOusterTable);
+    ouster_table(t.data(), t.data() + kOusterTable);
+    cudaError_t e = h->d_ouster_table.reserve(t.size());
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->d_ouster_table, t.data(), t.size() * sizeof(float), cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);   /* t is pageable and goes out of scope */
+    h->ouster_table_ok = e == cudaSuccess;
+    return e;
+}
+static lv_status process_ouster_impl(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                     const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz,
+                                     double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out, int64_t* d_n_out) {
+    const CloudOut o{d_xyz, d_time, d_intensity, d_range, d_idx};
+    /* a calibration or n_packets out of range leaves n at 0 here, and the layout check names it */
+    const bool cal_ok = cal && !ouster_calib_error(*cal);
+    const int H = cal_ok ? cal->pixels_per_column : 0;
+    const int64_t n = cal_ok && n_packets >= 0 && n_packets <= ouster_max_packets(H) ? n_packets * kOusterColumns * H : 0;
+    return front_end_impl(
+        h, "process ouster", !d_packets || !cal || !d_xyz || !d_time, "packets, cal, xyz, time or n_out", d_packets, data_bytes, n,
+        downsample_rate, o, n_out, d_n_out,
+        [&]() -> const char* {
+            if (const char* why = ouster_calib_error(*cal)) return why;
+            return ouster_layout_error(n_packets, data_bytes, H);
+        },
+        [&](int* launches, uint32_t* err) {
+            const cudaError_t e = ouster_table_ready(h);
+            if (e != cudaSuccess) return e;
+            const OusterArgs a = {d_packets, n, h->d_ouster_table, ouster_calib(*cal), downsample_rate, min_dist};
+            return launch_process_ouster(h->ds, a, o, d_n_out, err, h->stream, launches);
+        });
+}
+lv_status lv_process_ouster_device(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                   const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time,
+                                   float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out) {
+    return process_ouster_impl(h, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range, d_idx,
+                               n_out, nullptr);
+}
+lv_status lv_process_ouster_device_async(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                         const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz,
+                                         double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* d_n_out) {
+    int64_t unused = 0;                                           /* the count stays on the device */
+    if (!d_n_out) { set_error("process ouster: null packets, cal, xyz, time or n_out"); return LV_ERR_ARG; }
+    return process_ouster_impl(h, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range, d_idx,
+                               &unused, d_n_out);
 }
 
 /* the deferred errors of the _async calls (AsyncWords::err) and the map's flags; clears the former */

@@ -1,8 +1,8 @@
 /*
  * lv_cloud.cu — Accumulator::process (src/Modules/Accumulator.cpp:142-151) on the device: the raw bytes of a LiDAR message in
  * HBM -> msg2points (PointCloudProcessor.cpp:24-99) -> temporal_downsample (:101-112) -> sort_points (:114-123), with the
- * per-point arithmetic of lv_wire.h that the host decoders run too.  One pipeline serves three message formats; a point source
- * (Pc2Source, LivoxSource, VelodyneSource) says where a point's fields are and how its time is computed.
+ * per-point arithmetic of lv_wire.h that the host decoders run too.  One pipeline serves four message formats; a point source
+ * (Pc2Source, LivoxSource, VelodyneSource, OusterSource) says where a point's fields are and how its time is computed.
  *
  *   flag     every point of the message: xyz from its bytes -> temporal_keep on the rank
  *   select   cub::DeviceSelect::Flagged: indices of the kept points, in message order
@@ -14,7 +14,8 @@
  * and its select come first, and the rank is the position among the tag-kept points (Accumulator.cpp:143-151 decimates the list
  * msg2points returns).  velodyne_msgs/VelodyneScan likewise: a validity flag (return mode, block flags, distance) and its select
  * come first, and the key kernel also checks every packet for a dual return or a stamp that does not convert (the flag kernel
- * resets that word, so the first kernel cannot raise it).  The bytes of a kept point are read twice (flag + key, gather), those
+ * resets that word, so the first kernel cannot raise it).  Ouster LEGACY packets the same way: a validity flag (column status,
+ * measurement id, range) and its select, with no per-packet check: a column's time always converts.  The bytes of a kept point are read twice (flag + key, gather), those
  * of a dropped point once.  Every value is assembled from single bytes (lv_wire.h): fields sit at any offset and the message at any address.  Byte offsets are
  * 64-bit: n < 2^31 points of up to 2^31 bytes each.
  *
@@ -87,6 +88,25 @@ struct VelodyneSource {
     }
 };
 
+/* ouster LEGACY packets: a point is a slot (its column and pixel), decoded through the column table and the beam terms */
+struct OusterSlot {
+    const uint8_t* col;
+    int p;
+};
+struct OusterSource {
+    OusterArgs a;
+    __device__ __forceinline__ OusterSlot point(int64_t i) const {
+        return {ouster_column(a.data, i, a.cal.H), (int)(i % a.cal.H)};
+    }
+    __device__ __forceinline__ void xyz(const OusterSlot& p, float& x, float& y, float& z) const {
+        ouster_xyz(p.col, p.p, a.table, a.table + kOusterTable, a.cal, x, y, z);
+    }
+    __device__ __forceinline__ double time(const OusterSlot& p) const { return ouster_time(p.col); }
+    __device__ __forceinline__ float intensity(const OusterSlot& p) const { return ouster_reflectivity(p.col, p.p); }
+    __device__ __forceinline__ float range(const OusterSlot& p, float, float, float) const { return ouster_range(p.col, p.p); }
+    __device__ __forceinline__ void check(int64_t, int64_t, int*, uint32_t*) const {}
+};
+
 /* std::stable_sort with `<` on doubles: -0.0 and +0.0 are equal (message order), so -0.0 is folded onto +0.0; then the
  * sign-magnitude bits become an unsigned order (negatives reversed, positives above them) */
 __device__ __forceinline__ uint64_t time_key(double t) {
@@ -114,6 +134,13 @@ __global__ void __launch_bounds__(256) lv_velodyne_valid_kernel(VelodyneArgs a, 
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n) return;
     keep[i] = velodyne_slot_valid(velodyne_packet(a.data, i / kVelodyneSlots), (int)(i % kVelodyneSlots)) ? 1 : 0;
+}
+
+/* msg2points of ouster packets: the slots that are points (ouster_slot_valid) */
+__global__ void __launch_bounds__(256) lv_ouster_valid_kernel(OusterArgs a, uint8_t* __restrict__ keep) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    keep[i] = ouster_slot_valid(ouster_column(a.data, i, a.cal.H), (int)(i % a.cal.H), a.cal.W, a.cal.H) ? 1 : 0;
 }
 
 /* msg2points' tag filter of a livox message */
@@ -217,6 +244,23 @@ cudaError_t launch_process_velodyne(DownsampleScratch& s, const VelodyneArgs& a,
     /* as for livox: the msg2points slots live in vals_sorted until the second select has read them */
     int32_t* valid_sel = reinterpret_cast<int32_t*>(s.vals_sorted.get());
     lv_velodyne_valid_kernel<<<grid, 256, 0, st>>>(a, s.flags);
+    size_t tmp = s.tmp.size();
+    cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags.get(), valid_sel, s.count.get() + 2,
+                                               (int)a.n, st);
+    if (e != cudaSuccess) return e;
+    lv_cloud_flag_kernel<<<grid, 256, 0, st>>>(src, valid_sel, s.count.get() + 2, s.flags, s.count);
+    e = launch_select_sort_gather(s, src, static_cast<const int32_t*>(valid_sel), o, d_n_out, err, st);
+    if (e == cudaSuccess && launches) *launches += 9;
+    return e;
+}
+
+cudaError_t launch_process_ouster(DownsampleScratch& s, const OusterArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err,
+                                  cudaStream_t st, int* launches) {
+    const OusterSource src{a};
+    const unsigned grid = (unsigned)((a.n + 255) / 256);
+    /* as for livox: the msg2points slots live in vals_sorted until the second select has read them */
+    int32_t* valid_sel = reinterpret_cast<int32_t*>(s.vals_sorted.get());
+    lv_ouster_valid_kernel<<<grid, 256, 0, st>>>(a, s.flags);
     size_t tmp = s.tmp.size();
     cudaError_t e = cub::DeviceSelect::Flagged(s.tmp, tmp, cub::CountingInputIterator<int32_t>(0), s.flags.get(), valid_sel, s.count.get() + 2,
                                                (int)a.n, st);

@@ -202,7 +202,7 @@ struct DownsampleScratch {
     DeviceBuf<uint8_t> tmp;        /* cub's temporary storage: tmp.size() bytes */
     DeviceBuf<GridBox> box;
     DeviceBuf<int> count;          /* [0] output count, [1] NaN-time flag (velodyne: packet flag), [2] tag-kept count of a livox
-                                    * message / point count of a velodyne one (lv_cloud.cu) */
+                                    * message / point count of a velodyne or ouster one (lv_cloud.cu) */
     PinnedBuf<int> h_count;        /* [0] output count, [1] overflow flag (voxel grid) / NaN-time or packet flag (cloud) */
 };
 cudaError_t ds_reserve(DownsampleScratch& s, int64_t n);
@@ -269,6 +269,18 @@ struct VelodyneArgs {
 };
 cudaError_t launch_process_velodyne(DownsampleScratch& s, const VelodyneArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err,
                                     cudaStream_t st, int* launches);
+/* the same for Ouster LEGACY packets: msg2points (column status, measurement id, range), then the decimator on the rank among its
+ * points (lv_wire.h).  No deferred error of its own: a column's time always converts */
+struct OusterArgs {
+    const uint8_t* data;       /* the packets (device, any alignment) */
+    int64_t n;                 /* 16 H n_packets slots */
+    const float* table;        /* C then S, kOusterTable floats each (ouster_table, device) */
+    OusterCalib cal;           /* the beam terms, by value: the kernels read them from the parameter bank */
+    int32_t rate;
+    double min_dist;
+};
+cudaError_t launch_process_ouster(DownsampleScratch& s, const OusterArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err,
+                                  cudaStream_t st, int* launches);
 /* Processor::fill's header stamp (PointCloudProcessor.cpp:125-133): *d_stamp_us = max over the *d_n (clamped to [0, n_max]) times of
  * round(t * 1e6) as uint64 (Conversions::sec2Microsec, Utils.cpp:14-16), 0 for no point.  One launch */
 cudaError_t launch_cloud_stamp(const double* d_time, const int64_t* d_n, int64_t n_max, uint64_t* d_stamp_us, uint32_t* err, cudaStream_t st,

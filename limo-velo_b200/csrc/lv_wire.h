@@ -1,7 +1,7 @@
 /*
  * lv_wire.h — the per-point arithmetic of the LiDAR message, compiled by the host (lv_pointcloud2_to_points, lv_livox_to_points,
- * lv_velodyne_to_points) and the device (lv_process_cloud_device, lv_process_livox_device, lv_process_velodyne_device, the temporal
- * decimator) alike, so that both give the same bits:
+ * lv_velodyne_to_points, lv_ouster_to_points) and the device (lv_process_cloud_device, lv_process_livox_device,
+ * lv_process_velodyne_device, lv_process_ouster_device, the temporal decimator) alike, so that both give the same bits:
  *   PointCloudProcessor::msg2points / get_begin_time   src/Utils/PointCloudProcessor.cpp:24-99
  *   Point(const <driver>::Point&, double time_offset)   src/Objects/Point.cpp:37-111,153-175
  *   Conversions::microsec2Sec / nanosec2Sec             src/Utils/Utils.cpp:18-30
@@ -249,6 +249,100 @@ inline const char* velodyne_layout_error(int64_t n_packets, int64_t data_bytes) 
     if (n_packets < 0 || data_bytes < 0) return "negative packet count or data length";
     if (n_packets > kVelodyneMaxPackets) return "n_packets above (2^31 - 1) / 384 (slot indices are int32)";
     if (n_packets > data_bytes / kVelodynePacket) return "data_bytes is too short for n_packets packets of 1214 bytes";
+    return nullptr;
+}
+
+/* ---- ouster_ros/PacketMsg of an OS0 / OS1 / OS2 in the LEGACY profile (include/limovelo_b200.h, "Ouster packets"): packets of 16
+ * columns of 20 + 12 H bytes
+ *   uint64 timestamp (ns) | uint16 measurement_id m | uint16 frame_id | uint32 encoder (unused) | H x 12-byte pixels | uint32 status
+ * pixel: uint32 range word (low 20 bits: range in mm) | uint16 reflectivity | 6 bytes of signal and noise (unused).
+ * The packets are contiguous, so column g = k 16 + c of the message starts at packets + g (20 + 12 H), any alignment.
+ * Slot i of the message: column g = i / H, pixel p = i % H. */
+enum { kOusterColumns = 16, kOusterMaxBeams = 128, kOusterTable = 2048 };
+constexpr uint32_t kOusterRangeMask = 0xFFFFFu;
+
+/* the calibration in the fp32 terms the point arithmetic reads (ouster_calib): per beam, cos / sin of the altitude and the azimuth */
+struct OusterCalib {
+    float ce[kOusterMaxBeams], se[kOusterMaxBeams];   /* cos / sin of the beam altitude  */
+    float ca[kOusterMaxBeams], sa[kOusterMaxBeams];   /* cos / sin of the beam azimuth   */
+    float nf;                                         /* lidar_origin_to_beam_origin in m */
+    int32_t W, H;                                     /* columns per frame, pixels per column */
+};
+
+LV_HD uint64_t wire_u64(const uint8_t* p) { return (uint64_t)wire_u32(p) | (uint64_t)wire_u32(p + 4) << 32; }
+LV_HD int64_t ouster_column_bytes(int H) { return 20 + 12 * (int64_t)H; }
+LV_HD int64_t ouster_packet_bytes(int H) { return kOusterColumns * ouster_column_bytes(H); }
+/* the column of slot i and its pixel p */
+LV_HD const uint8_t* ouster_column(const uint8_t* packets, int64_t i, int H) {
+    return packets + (uint64_t)(i / H) * (uint64_t)ouster_column_bytes(H);
+}
+LV_HD const uint8_t* ouster_pixel(const uint8_t* col, int p) { return col + 16 + 12 * p; }
+LV_HD uint32_t ouster_measurement_id(const uint8_t* col) { return wire_u16(col + 8); }
+LV_HD uint32_t ouster_status(const uint8_t* col, int H) { return wire_u32(col + 16 + 12 * H); }
+LV_HD uint32_t ouster_range_mm(const uint8_t* col, int p) { return wire_u32(ouster_pixel(col, p)) & kOusterRangeMask; }
+
+/* msg2points: the column's status has bit 0 set, its measurement id is a column of the frame, and the pixel has a return */
+LV_HD bool ouster_slot_valid(const uint8_t* col, int p, int W, int H) {
+    return (ouster_status(col, H) & 1u) && ouster_measurement_id(col) < (uint32_t)W && ouster_range_mm(col, p) != 0;
+}
+/* the point of pixel p of a valid column (C, S: the column table of ouster_table), in the LiDAR frame (os_lidar), fp32, each
+ * product and sum rounded, in the order of the header */
+LV_HD void ouster_xyz(const uint8_t* col, int p, const float* C, const float* S, const OusterCalib& k, float& x, float& y, float& z) {
+    const int q = (int)ouster_measurement_id(col) * (kOusterTable / k.W);
+    const float c = C[q], s = S[q];
+    const float e = fsub(fmul((float)ouster_range_mm(col, p), 0.001f), k.nf);
+    const float ch = fsub(fmul(c, k.ca[p]), fmul(s, k.sa[p])), sh = fadd(fmul(s, k.ca[p]), fmul(c, k.sa[p]));
+    const float ee = fmul(e, k.ce[p]);
+    x = fadd(fmul(ee, ch), fmul(k.nf, c));
+    y = -fadd(fmul(ee, sh), fmul(k.nf, s));
+    z = fmul(e, k.se[p]);
+}
+LV_HD float ouster_reflectivity(const uint8_t* col, int p) { return (float)wire_u16(ouster_pixel(col, p) + 4); }
+LV_HD float ouster_range(const uint8_t* col, int p) { return (float)ouster_range_mm(col, p); }
+/* the column's own timestamp, absolute */
+LV_HD double ouster_time(const uint8_t* col) { return wire_ns_to_sec(wire_u64(col)); }
+
+/* host code from here.  C[q] = cos(2 pi q / 2048), S[q] = sin(...) for q in [0, 2048): computed in double, rounded to float.  The host
+ * decoder and the device table both come from here, so both read the same bits */
+inline void ouster_table(float* C, float* S) {
+    for (int q = 0; q < kOusterTable; ++q) {
+        const double a = 2.0 * M_PI * (double)q / (double)kOusterTable;
+        C[q] = (float)cos(a);
+        S[q] = (float)sin(a);
+    }
+}
+/* NULL when W and H are in their sets and the entries the decoder reads (the first H angles of each array, and n) are finite */
+inline const char* ouster_calib_error(const lv_ouster_calibration& c) {
+    const int W = c.columns_per_frame, H = c.pixels_per_column;
+    if (W != 512 && W != 1024 && W != 2048) return "columns_per_frame is not 512, 1024 or 2048";
+    if (H != 16 && H != 32 && H != 64 && H != 128) return "pixels_per_column is not 16, 32, 64 or 128";
+    for (int p = 0; p < H; ++p)
+        if (!isfinite(c.beam_altitude_angles[p]) || !isfinite(c.beam_azimuth_angles[p])) return "a calibration entry is not finite";
+    return isfinite(c.lidar_origin_to_beam_origin_mm) ? nullptr : "a calibration entry is not finite";
+}
+/* the fp32 terms of a calibration ouster_calib_error accepts */
+inline OusterCalib ouster_calib(const lv_ouster_calibration& c) {
+    OusterCalib k = {};
+    k.W = c.columns_per_frame;
+    k.H = c.pixels_per_column;
+    for (int p = 0; p < k.H; ++p) {
+        const double alt = c.beam_altitude_angles[p] * M_PI / 180.0, az = c.beam_azimuth_angles[p] * M_PI / 180.0;
+        k.ce[p] = (float)cos(alt);
+        k.se[p] = (float)sin(alt);
+        k.ca[p] = (float)cos(az);
+        k.sa[p] = (float)sin(az);
+    }
+    k.nf = (float)(c.lidar_origin_to_beam_origin_mm * 0.001);
+    return k;
+}
+/* the most packets whose slot indices fit an int32 */
+inline int64_t ouster_max_packets(int H) { return 0x7fffffff / (kOusterColumns * (int64_t)H); }
+
+/* NULL when n_packets is in range and its packets fit data_bytes (H from a calibration ouster_calib_error accepts), else what is wrong */
+inline const char* ouster_layout_error(int64_t n_packets, int64_t data_bytes, int H) {
+    if (n_packets < 0 || data_bytes < 0) return "negative packet count or data length";
+    if (n_packets > ouster_max_packets(H)) return "n_packets above (2^31 - 1) / (16 pixels_per_column) (slot indices are int32)";
+    if (n_packets > data_bytes / ouster_packet_bytes(H)) return "data_bytes is too short for n_packets packets of 16 (20 + 12 pixels_per_column) bytes";
     return nullptr;
 }
 

@@ -306,6 +306,29 @@ class Accumulator {
             check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, 384 * m.n_packets),
                   "Accumulator::receive_velodyne_device_full");
     }
+    /* receive_lidar_device for Ouster LEGACY packets (lv_process_ouster_device_async: the packets decoded through the beam intrinsics,
+     * decimation on the rank among the points, time sort); the packets in device memory, e.g. the PacketMsgs of one frame batched
+     * into one upload.  The output buffers hold 16 H n_packets points (H = cal->pixels_per_column). */
+    struct DeviceOusterMessage {
+        const uint8_t* d_packets; int64_t data_bytes, n_packets; const lv_ouster_calibration* cal; int32_t downsample_rate; double min_dist;
+        int64_t slots() const { return 16 * (int64_t)cal->pixels_per_column * n_packets; }
+    };
+    void receive_ouster_device(const DeviceOusterMessage& m, float* d_xyz, double* d_time, int64_t* d_n) {
+        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
+                                             d_time, nullptr, nullptr, nullptr, d_n),
+              "Accumulator::receive_ouster_device");
+        if (m.n_packets > 0) check(lv_lidar_push_device_async(ctx->h, d_xyz, d_time, d_n, m.slots()), "Accumulator::receive_ouster_device");
+    }
+    /* the same with whole Points: intensity = reflectivity, range = the range in mm */
+    void receive_ouster_device_full(const DeviceOusterMessage& m, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                    int64_t* d_n) {
+        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
+                                             d_time, d_intensity, d_range, nullptr, d_n),
+              "Accumulator::receive_ouster_device_full");
+        if (m.n_packets > 0)
+            check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.slots()),
+                  "Accumulator::receive_ouster_device_full");
+    }
     /* Several LiDARs: the same calls with the sensor's extrinsic L0_T_Lk (12 floats, R row-major then t: its frame into the primary
      * LiDAR's, nullptr for the primary itself) merge the message by time instead of pushing it (lv_lidar_merge_device_async), so
      * the buffer stays time-ordered when the sensors' messages overlap.  Needs lv_lidar_reserve_merge on the context's handle. */
@@ -356,6 +379,22 @@ class Accumulator {
         if (m.n_packets > 0)
             check(lv_lidar_merge_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, 384 * m.n_packets, L0_T_Lk),
                   "Accumulator::receive_velodyne_device_full");
+    }
+    void receive_ouster_device(const DeviceOusterMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, int64_t* d_n) {
+        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
+                                             d_time, nullptr, nullptr, nullptr, d_n),
+              "Accumulator::receive_ouster_device");
+        if (m.n_packets > 0)
+            check(lv_lidar_merge_device_async(ctx->h, d_xyz, d_time, d_n, m.slots(), L0_T_Lk), "Accumulator::receive_ouster_device");
+    }
+    void receive_ouster_device_full(const DeviceOusterMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, float* d_intensity,
+                                    float* d_range, int64_t* d_n) {
+        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
+                                             d_time, d_intensity, d_range, nullptr, d_n),
+              "Accumulator::receive_ouster_device_full");
+        if (m.n_packets > 0)
+            check(lv_lidar_merge_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.slots(), L0_T_Lk),
+                  "Accumulator::receive_ouster_device_full");
     }
     /* Accumulator::get_points(t1, t2) (Accumulator.hpp:61-74) into device buffers of n_max points; the count goes to *d_n_out */
     void get_points_device(double t1, double t2, float* d_xyz, double* d_time, int64_t n_max, int64_t* d_n_out) {

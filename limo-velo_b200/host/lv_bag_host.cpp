@@ -21,6 +21,8 @@
  * intensity), ready for lv_pointcloud2_to_points; sensor_msgs/Imu -> stamp, orientation, angular velocity, acceleration.
  * Livox sensors publish livox_ros_driver/CustomMsg instead of PointCloud2: lv_bag_parse_livox -> a view of its 19-byte records.
  * A Velodyne driver that records packets publishes velodyne_msgs/VelodyneScan: lv_bag_parse_velodyne_scan -> a view of its packets.
+ * An Ouster driver that records packets publishes ouster_ros/PacketMsg, one LiDAR or IMU packet each: lv_bag_parse_ouster_packet ->
+ * a view of the packet; lv_ouster_imu_packet decodes an IMU packet into the sample sensor_msgs/Imu would give.
  * Everything is host code: a sweep is a few MB per 100 ms.
  */
 #include <stdio.h>
@@ -326,6 +328,32 @@ lv_status lv_bag_parse_velodyne_scan(const uint8_t* data, int64_t size, lv_velod
     out->n_packets = count;
     out->packets = packets;
     out->data_bytes = (int64_t)count * lv::kVelodynePacket;
+    return LV_OK;
+}
+
+lv_status lv_bag_parse_ouster_packet(const uint8_t* data, int64_t size, lv_ouster_packet_view* out) {
+    if (!data || !out || size < 0) return LV_ERR_ARG;
+    memset(out, 0, sizeof(*out));
+    Rd r(data, size);
+    const uint32_t bytes = r.u32();                   /* uint8[] buf */
+    const uint8_t* buf = r.take(bytes);
+    if (!r.ok || r.at != size) return LV_ERR_ARG;
+    out->data = buf;
+    out->bytes = bytes;
+    return LV_OK;
+}
+
+lv_status lv_ouster_imu_packet(const uint8_t* pkt, int64_t bytes, lv_imu_sample* out) {
+    if (!pkt || !out || bytes != 48) return LV_ERR_ARG;
+    const uint64_t gyro_ts = lv::wire_u64(pkt + 16);
+    if (gyro_ts / 1000000000ull > 0xFFFFFFFFull) return LV_ERR_ARG;
+    memset(out, 0, sizeof(*out));                     /* orientation {0, 0, 0, 0}: none (IMU::has_orientation) */
+    out->stamp_sec = (uint32_t)(gyro_ts / 1000000000ull);
+    out->stamp_nsec = (uint32_t)(gyro_ts % 1000000000ull);
+    for (int k = 0; k < 3; ++k) {
+        out->linear_acceleration[k] = (double)lv::wire_f32(pkt + 24 + 4 * k) * 9.80665;     /* g -> m/s^2 */
+        out->angular_velocity[k] = ((double)lv::wire_f32(pkt + 36 + 4 * k) * M_PI) / 180.0;  /* deg/s -> rad/s */
+    }
     return LV_OK;
 }
 

@@ -4,6 +4,7 @@
  * a plain file parser; same keys, same defaults, unknown keys ignored like rosparam does).
  */
 #include <ctype.h>
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -157,5 +158,107 @@ extern "C" lv_status lv_params_from_yaml(const char* path, lv_params* p) {
     }
     /* device tuning keys are optional extensions */
     numf("voxel_size", &p->voxel_size);
+    return LV_OK;
+}
+
+/* ---- the Ouster sensor metadata JSON (lv_ouster_calibration_from_json): a scanner for the few keys the decoder needs, not a JSON
+ * library.  A key is a string followed by ':'; its value starts after the ':'.  Keys are taken at any depth, the first occurrence
+ * counts, and string values are skipped whole, so text inside them is never read as a key. */
+namespace {
+
+struct JsonScan {
+    const std::string& t;
+    std::map<std::string, size_t> at;   /* key -> position of its value */
+    explicit JsonScan(const std::string& text) : t(text) {
+        size_t i = 0;
+        while (i < t.size()) {
+            if (t[i] != '"') { ++i; continue; }
+            std::string key;
+            if (!string_at(i, &key, &i)) return;
+            size_t j = skip(i);
+            if (j < t.size() && t[j] == ':' && !at.count(key)) at[key] = skip(j + 1);
+        }
+    }
+    size_t skip(size_t i) const {
+        while (i < t.size() && isspace((unsigned char)t[i])) ++i;
+        return i;
+    }
+    /* the string starting at t[i] == '"' (escapes kept as written); *end = one past its closing quote */
+    bool string_at(size_t i, std::string* out, size_t* end) const {
+        if (i >= t.size() || t[i] != '"') return false;
+        for (size_t j = i + 1; j < t.size(); ++j) {
+            if (t[j] == '\\') { ++j; continue; }
+            if (t[j] == '"') { *out = t.substr(i + 1, j - i - 1); *end = j + 1; return true; }
+        }
+        return false;
+    }
+    /* a finite JSON number at t[i]; *end = one past it */
+    bool number_at(size_t i, double* out, size_t* end) const {
+        if (i >= t.size() || !(t[i] == '-' || isdigit((unsigned char)t[i]))) return false;
+        char* e = nullptr;
+        *out = strtod(t.c_str() + i, &e);
+        if (e == t.c_str() + i || !isfinite(*out)) return false;
+        *end = (size_t)(e - t.c_str());
+        return true;
+    }
+    bool has(const char* k) const { return at.count(k) != 0; }
+    bool number(const char* k, double* out) const { size_t e; return has(k) && number_at(at.at(k), out, &e); }
+    bool str(const char* k, std::string* out) const { size_t e; return has(k) && string_at(at.at(k), out, &e); }
+    bool numbers(const char* k, std::vector<double>* out) const {
+        if (!has(k)) return false;
+        size_t i = at.at(k);
+        if (i >= t.size() || t[i] != '[') return false;
+        i = skip(i + 1);
+        if (i < t.size() && t[i] == ']') return true;
+        for (;;) {
+            double d;
+            if (!number_at(i, &d, &i)) return false;
+            out->push_back(d);
+            i = skip(i);
+            if (i < t.size() && t[i] == ']') return true;
+            if (i >= t.size() || t[i] != ',') return false;
+            i = skip(i + 1);
+        }
+    }
+};
+
+/* "<W>x<rate>", e.g. "1024x10" -> W */
+bool lidar_mode_columns(const std::string& mode, int32_t* W) {
+    const size_t x = mode.find('x');
+    if (x == 0 || x == std::string::npos || x + 1 == mode.size() || x > 4) return false;
+    for (size_t i = 0; i < mode.size(); ++i)
+        if (i != x && !isdigit((unsigned char)mode[i])) return false;
+    *W = (int32_t)atoi(mode.substr(0, x).c_str());
+    return true;
+}
+
+}  // namespace
+
+extern "C" lv_status lv_ouster_calibration_from_json(const char* text, int64_t len, lv_ouster_calibration* out) {
+    if (!text || len < 0 || !out) return LV_ERR_ARG;
+    memset(out, 0, sizeof(*out));
+    const std::string t(text, (size_t)len);
+    const JsonScan j(t);
+    std::vector<double> alt, az;
+    std::string mode, profile;
+    int32_t W = 0;
+    if (!j.numbers("beam_altitude_angles", &alt) || !j.numbers("beam_azimuth_angles", &az) || alt.size() != az.size() ||
+        !j.str("lidar_mode", &mode) || !lidar_mode_columns(mode, &W))
+        return LV_ERR_ARG;
+    const int32_t H = (int32_t)alt.size();
+    if ((W != 512 && W != 1024 && W != 2048) || (H != 16 && H != 32 && H != 64 && H != 128)) return LV_ERR_ARG;
+    double v = 0;
+    if (j.has("pixels_per_column") && (!j.number("pixels_per_column", &v) || v != H)) return LV_ERR_ARG;
+    if (j.has("columns_per_packet") && (!j.number("columns_per_packet", &v) || v != 16)) return LV_ERR_ARG;
+    if (j.has("udp_profile_lidar") && (!j.str("udp_profile_lidar", &profile) || profile != "LEGACY")) return LV_ERR_ARG;
+    double n = 0;
+    if (j.has("lidar_origin_to_beam_origin_mm") && !j.number("lidar_origin_to_beam_origin_mm", &n)) return LV_ERR_ARG;
+    out->columns_per_frame = W;
+    out->pixels_per_column = H;
+    for (int32_t p = 0; p < H; ++p) {
+        out->beam_altitude_angles[p] = alt[p];
+        out->beam_azimuth_angles[p] = az[p];
+    }
+    out->lidar_origin_to_beam_origin_mm = n;
     return LV_OK;
 }
