@@ -300,32 +300,34 @@ static lv_status create_buffers(lv_context* h) {
     LV_CUDA(h->d_ref.reserve(p->max_points));
     LV_CUDA(h->d_redo.reserve(p->max_points + 64));   /* + one block of slack: read speculatively */
     /* hand-over buffers start defined: lv_search_kernel<.., LIST> reads redo_list[] before it knows the list's length, and a
-     * first update's reuse kernel must not see stale neighbours (also keeps compute-sanitizer initcheck quiet) */
-    LV_CUDA(cudaMemset(h->d_redo, 0, sizeof(uint32_t) * (p->max_points + 64)));
-    LV_CUDA(cudaMemset(h->d_nn_a, 0xFF, sizeof(int4) * p->max_points));
-    LV_CUDA(cudaMemset(h->d_nn_b, 0xFF, sizeof(int2) * p->max_points));
-    LV_CUDA(cudaMemset(h->d_ref, 0, sizeof(float4) * p->max_points));
-    LV_CUDA(cudaMemset(h->d_hard_list, 0, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters)));
+     * first update's reuse kernel must not see stale neighbours (also keeps compute-sanitizer initcheck quiet).  Every clear of
+     * a context runs on its own stream: the stream orders it before the context's first kernel, and no clear touches the legacy
+     * stream, which would wait for (or, while one is being captured, break) other threads' work on blocking streams */
+    LV_CUDA(cudaMemsetAsync(h->d_redo, 0, sizeof(uint32_t) * (p->max_points + 64), h->stream));
+    LV_CUDA(cudaMemsetAsync(h->d_nn_a, 0xFF, sizeof(int4) * p->max_points, h->stream));
+    LV_CUDA(cudaMemsetAsync(h->d_nn_b, 0xFF, sizeof(int2) * p->max_points, h->stream));
+    LV_CUDA(cudaMemsetAsync(h->d_ref, 0, sizeof(float4) * p->max_points, h->stream));
+    LV_CUDA(cudaMemsetAsync(h->d_hard_list, 0, sizeof(uint32_t) * ((size_t)kHardBuckets * hard_segment(p->max_points) + kCounters), h->stream));
     h->use_reuse = getenv("LV_NO_REUSE") == nullptr;
     h->use_pdl = getenv("LV_NO_PDL") == nullptr;
     LV_CUDA(h->d_job.reserve(1));
-    measure_init();
+    LV_CUDA(measure_init(h->stream));
     h->use_graph = getenv("LV_NO_GRAPH") == nullptr;
     LV_CUDA(h->d_ctrl.reserve(1));
-    LV_CUDA(cudaMemset(h->d_ctrl, 0, sizeof(UpdateCtrl)));
+    LV_CUDA(cudaMemsetAsync(h->d_ctrl, 0, sizeof(UpdateCtrl), h->stream));
     LV_CUDA(h->h_ctrl.reserve(1));
     LV_CUDA(h->imu_copied.create());
     LV_CUDA(h->ctrl_copied.create());
     LV_CUDA(h->path_copied.create());
     LV_CUDA(h->d_async.reserve(1));
-    LV_CUDA(cudaMemset(h->d_async, 0, sizeof(AsyncWords)));
+    LV_CUDA(cudaMemsetAsync(h->d_async, 0, sizeof(AsyncWords), h->stream));
     LV_CUDA(h->h_async.reserve(1));
     LV_CUDA(h->d_partials.reserve((size_t)kPartialStride * (kMeasureGridCap + 8)));
-    LV_CUDA(cudaMemset(h->d_partials, 0, sizeof(double) * kPartialStride * (kMeasureGridCap + 8)));
+    LV_CUDA(cudaMemsetAsync(h->d_partials, 0, sizeof(double) * kPartialStride * (kMeasureGridCap + 8), h->stream));
     LV_CUDA(h->d_group_rows.reserve((size_t)kPartialStride * 32));
-    LV_CUDA(cudaMemset(h->d_group_rows, 0, sizeof(double) * kPartialStride * 32));
+    LV_CUDA(cudaMemsetAsync(h->d_group_rows, 0, sizeof(double) * kPartialStride * 32, h->stream));
     LV_CUDA(h->d_group_tickets.reserve(32));
-    LV_CUDA(cudaMemset(h->d_group_tickets, 0, sizeof(uint32_t) * 32));
+    LV_CUDA(cudaMemsetAsync(h->d_group_tickets, 0, sizeof(uint32_t) * 32, h->stream));
     LV_CUDA(h->d_reduced.reserve(160));
     LV_CUDA(h->h_reduced.reserve(160));
     LV_CUDA(h->h_nevals.reserve(kNevalsRing));

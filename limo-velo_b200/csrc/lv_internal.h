@@ -181,7 +181,10 @@ cudaError_t launch_measure(const MeasureArgs& a, int grid, cudaStream_t st, cons
 cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz, int n, uint32_t* counters, const UpdateGate& gate,
                                cudaStream_t st);
 const void* ieskf_begin_kernel_ptr();
-void measure_init();                          /* constant tables; call once before any capture           */
+/* the constant tables of the fit and step kernels on the current device: copied on st and waited for by the first call per
+ * device (thread-safe); the launchers above and below need it done, so lv_create calls it on the handle's stream, never inside
+ * a capture.  Without a stream (a harness that runs the launchers on the legacy stream) the copy runs on the legacy stream */
+cudaError_t measure_init(cudaStream_t st = 0);
 cudaError_t launch_ieskf_step(UpdateCtrl* c, const IeskfParams& prm, const double* partials, int n_partials,
                               cudaStream_t st, int pdl = 0);
 /* stand-alone reduction of the partials (operator-boundary calls): out[0:144) HTH, [144:156) HTh, [156] Nm */

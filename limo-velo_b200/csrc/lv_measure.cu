@@ -26,6 +26,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <mutex>
+
 #ifdef LV_STEP_TIMING
 __device__ unsigned long long g_probes[2];     /* total hash probes, number of lookups that needed more than 8 */
 #ifdef __CUDA_ARCH__
@@ -65,21 +67,29 @@ namespace lv {
  * (b = 12 selects h) */
 __constant__ uint8_t c_pair_a[90];
 __constant__ uint8_t c_pair_b[90];
-static bool g_pairs_ready[64] = {false};    /* constant memory is per device */
+/* constant memory is per device: the first handle created on a device copies the table on its own stream and waits for the
+ * copy before it marks the device ready, all under the lock, so a handle created at the same time by another thread either
+ * waits for that copy or finds it on the device */
+static std::mutex g_pairs_mutex;
+static bool g_pairs_ready[64] = {false};    /* guarded by g_pairs_mutex */
 
-static void init_pairs() {
+static cudaError_t init_pairs(cudaStream_t st) {
     int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) dev = 0;
-    if (g_pairs_ready[dev]) return;
+    cudaError_t err = cudaGetDevice(&dev);
+    if (err != cudaSuccess) return err;
+    if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+    std::lock_guard<std::mutex> lock(g_pairs_mutex);
+    if (g_pairs_ready[dev]) return cudaSuccess;
     uint8_t a[90], b[90];
     int e = 0;
     for (int i = 0; i < 12; ++i)
         for (int j = i; j < 12; ++j) { a[e] = (uint8_t)i; b[e] = (uint8_t)j; ++e; }
     for (int i = 0; i < 12; ++i) { a[e] = (uint8_t)i; b[e] = 12; ++e; }
-    cudaMemcpyToSymbol(c_pair_a, a, sizeof(a));
-    cudaMemcpyToSymbol(c_pair_b, b, sizeof(b));
-    g_pairs_ready[dev] = true;
+    err = cudaMemcpyToSymbolAsync(c_pair_a, a, sizeof(a), 0, cudaMemcpyHostToDevice, st);
+    if (err == cudaSuccess) err = cudaMemcpyToSymbolAsync(c_pair_b, b, sizeof(b), 0, cudaMemcpyHostToDevice, st);
+    if (err == cudaSuccess) err = cudaStreamSynchronize(st);       /* a and b live on this stack */
+    if (err == cudaSuccess) g_pairs_ready[dev] = true;
+    return err;
 }
 
 /* Programmatic dependent launch: every kernel of an update lets its successor's blocks be scheduled early
@@ -649,7 +659,7 @@ int measure_grid(int n) {
     return tiles < kMeasureGridCap ? (tiles > 0 ? tiles : 1) : kMeasureGridCap;
 }
 
-void measure_init() { init_pairs(); }
+cudaError_t measure_init(cudaStream_t st) { return init_pairs(st); }
 
 /* K1 variant of one launch: lanes per query (4 or 8).
  * 4 lanes per query issue a quarter fewer instructions per query than 8 (the prologue is shared by eight queries of a warp
@@ -696,7 +706,6 @@ static void launch_search(const MeasureArgs& a, int group, int sgrid, cudaStream
 }
 
 cudaError_t launch_measure(const MeasureArgs& a, int grid, cudaStream_t st, const MeasureProbe* probe, int reuse, int pdl) {
-    init_pairs();
     const int group = search_group(a, reuse);          /* reuse = index of the evaluation within its update */
     const int sgrid = search_grid(a, group);
     /* work-list length, a spare word, redo-list length; inside an update with pdl the kernels
@@ -730,12 +739,10 @@ cudaError_t launch_ieskf_begin(UpdateCtrl* c, MeasureJob* job, const float* xyz,
 const void* ieskf_begin_kernel_ptr() { return (const void*)lv_ieskf_begin_kernel; }
 cudaError_t launch_ieskf_step(UpdateCtrl* c, const IeskfParams& prm, const double* partials, int n_partials,
                               cudaStream_t st, int pdl) {
-    init_pairs();
     launch_k(lv_ieskf_step_kernel, 1, kStepThreads, st, pdl != 0, c, prm, partials, n_partials);
     return cudaGetLastError();
 }
 cudaError_t launch_reduce_partials(const double* partials, int n_partials, double* out, cudaStream_t st) {
-    init_pairs();
     lv_reduce_partials_kernel<<<1, kStepThreads, 0, st>>>(partials, n_partials, out);
     return cudaGetLastError();
 }
