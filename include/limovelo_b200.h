@@ -553,17 +553,30 @@ lv_status lv_process_velodyne_device(lv_handle h, const uint8_t* d_packets, int6
                                      const lv_velodyne_calibration* cal, int32_t downsample_rate, double min_dist,
                                      float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out);
 
-/* ---- Ouster packets: ouster_ros/PacketMsg of an OS0 / OS1 / OS2 in the LEGACY UDP profile -----------------------------------------
+/* ---- Ouster packets: ouster_ros/PacketMsg of an OS0 / OS1 / OS2 -----------------------------------------------------------------
  * The raw UDP packets the Ouster driver records on .../lidar_packets (one packet per message) and .../imu_packets, with the
- * sensor's metadata JSON; lv_bag_parse_ouster_packet finds a packet in a bag, lv_ouster_calibration_from_json reads the metadata.
- * A LEGACY packet holds 16 columns of 20 + 12 H bytes (H = pixels_per_column), so packet k starts at packets + k 16 (20 + 12 H)
- * (12 608 bytes for H = 64), at any alignment.  Column: uint64 timestamp (ns) | uint16 measurement_id m | uint16 frame_id | uint32
- * encoder count (not read) | H pixels of 12 bytes | uint32 status.  Pixel: uint32 range word (its low 20 bits are the range r in
- * mm) | uint16 reflectivity | signal and noise (not read).  All little endian.  The geometry is that of the Ouster driver's
- * make_xyz_lut in the LiDAR frame (os_lidar); bit parity with ouster_ros is not claimed.
+ * sensor's metadata JSON; lv_bag_parse_ouster_packet finds a packet in a bag, lv_ouster_sensor_from_json reads the metadata and
+ * its lidar UDP profile.  A packet holds 16 columns; packet k starts at packets + k B (B = the profile's packet bytes), at any
+ * alignment.  All little endian.  H = pixels_per_column.
+ *   LEGACY (firmware 1.x, and 2.x by default): B = 16 (20 + 12 H) (12 608 bytes for H = 64).  Column: uint64 timestamp (ns) |
+ *              uint16 measurement_id m | uint16 frame_id | uint32 encoder count (not read) | H pixels of 12 bytes | uint32 status.
+ *              Pixel: uint32 range word (r = its low 20 bits, mm) | uint16 reflectivity | signal and noise (not read).
+ *   the profiles of firmware 2.2+ (RNG19_RFL8_SIG16_NIR16 is the default of firmware 3.x): B = 64 + 16 (12 + s H): a 32-byte
+ *              packet header (not read) | 16 columns | a 32-byte packet footer (not read, so its CRC64 is not checked).  Column:
+ *              uint64 timestamp (ns) | uint16 measurement_id m | uint16 status | H pixels of s bytes.  Pixel, by profile:
+ *                profile                        s    r (mm)                      reflectivity   B for H = 64
+ *                RNG19_RFL8_SIG16_NIR16         12   u32 @0 & 0x7FFFF            u8 @4          12 544
+ *                RNG19_RFL8_SIG16_NIR16_DUAL    16   u32 @0 & 0x7FFFF (first)    u8 @3 (first)  16 640
+ *                RNG15_RFL8_NIR8 (low data)     4    (u16 @0 & 0x7FFF) << 3      u8 @2          4 352
+ *              The bits above each range mask (flags) are ignored.  Dual return gives the first return's points only: those of
+ *              os_cloud_node's `points` topic; the second return is not read.  Low data gives ranges on an 8 mm grid.
+ * These layouts follow the Ouster firmware manual's packet tables and the field table of ouster_client's packet_format; nobody
+ * has checked the non-LEGACY ones against a recording from a real sensor.  The geometry is that of the Ouster driver's
+ * make_xyz_lut in the LiDAR frame (os_lidar); bit parity with ouster_ros is not claimed.  Every profile decodes by the same rules:
  *   slots      message slot i = k 16 H + c H + p (packet k, column c, pixel p); idx reports the slot (the ring is i % H);
  *              16 H n_packets slots, and n_packets <= (2^31 - 1) / (16 H) (slot indices are int32)
- *   points     a slot is a point when its column's status has bit 0 set (0xFFFFFFFF is valid, 0 is not), m < W and r != 0
+ *   points     a slot is a point when bit 0 of its column's status is set (for LEGACY 0xFFFFFFFF is valid, 0 is not), m < W and
+ *              r != 0
  *   tables     one column table for every W: C[q] = (float)cos(2 pi q / 2048), S[q] = (float)sin(...) for q in [0, 2048), in
  *              double, rounded; column m reads q = m (2048 / W).  Per beam p: ce, se, ca, sa = the floats of cos / sin of
  *              beam_altitude_angles[p] and beam_azimuth_angles[p] (degrees, times pi / 180 in double); nf = (float)(n 0.001)
@@ -576,8 +589,15 @@ lv_status lv_process_velodyne_device(lv_handle h, const uint8_t* d_packets, int6
  *              full_rotation_time do not apply.  The conversion cannot fail
  *   outputs    intensity = (float)reflectivity, range = (float)r in mm: the range field os_cloud_node writes, which the Ouster
  *              PointCloud2 path passes through (lv_cloud_layout.off_range), so both Ouster paths give the buffer the same lanes
- * Out of scope: the other UDP profiles (RNG19_RFL8_SIG16_NIR16, dual return, low data) and the packet header / footer of
- * firmware 2.2+, lidar_to_sensor_transform, signal and NIR, the driver's frame-id dedup of late packets. */
+ * Out of scope: the second return of the dual profile, the FUSA profiles, the packet CRC, the packet header's init_id / serial
+ * number checked against the metadata, columns_per_packet != 16, lidar_to_sensor_transform, signal and NIR, the driver's frame-id
+ * dedup of late packets. */
+typedef enum lv_ouster_profile {
+    LV_OUSTER_LEGACY = 0,
+    LV_OUSTER_RNG19_RFL8_SIG16_NIR16 = 1,
+    LV_OUSTER_RNG19_RFL8_SIG16_NIR16_DUAL = 2,
+    LV_OUSTER_RNG15_RFL8_NIR8 = 3
+} lv_ouster_profile;
 typedef struct lv_ouster_calibration {
     int32_t columns_per_frame;           /* W: 512, 1024 or 2048 (lidar_mode "1024x10" -> 1024)     */
     int32_t pixels_per_column;           /* H: 16, 32, 64 or 128                                     */
@@ -585,28 +605,41 @@ typedef struct lv_ouster_calibration {
     double beam_azimuth_angles[128];     /* degrees, the first H are read                           */
     double lidar_origin_to_beam_origin_mm;   /* n; 0 for firmware that does not report it          */
 } lv_ouster_calibration;
-/* the sensor metadata JSON (len bytes of text, no terminator needed) -> *out.  A narrow reader, not a JSON library: the keys are
- * found at any depth (firmware 1.x puts them at the top level, 2.x nests them under beam_intrinsics, config_params and
+/* the sensor metadata JSON (len bytes of text, no terminator needed) -> *out and *profile.  A narrow reader, not a JSON library: the
+ * keys are found at any depth (firmware 1.x puts them at the top level, 2.x nests them under beam_intrinsics, config_params and
  * lidar_data_format), the first occurrence counts.  Required: beam_altitude_angles and beam_azimuth_angles (arrays of equal
- * length H, finite numbers) and lidar_mode ("<W>x<rate>").  Optional: lidar_origin_to_beam_origin_mm (0 when absent).  Checked
- * when present: pixels_per_column == H, columns_per_packet == 16, udp_profile_lidar == "LEGACY".  LV_ERR_ARG for a null argument,
- * len < 0, a missing or malformed required key, W or H outside its set, or a check that fails (*out is then zeroed).  Host code. */
+ * length H, finite numbers) and lidar_mode ("<W>x<rate>").  Optional: lidar_origin_to_beam_origin_mm (0 when absent) and
+ * udp_profile_lidar ("LEGACY", "RNG19_RFL8_SIG16_NIR16", "RNG19_RFL8_SIG16_NIR16_DUAL" or "RNG15_RFL8_NIR8"; LEGACY when absent,
+ * as on firmware 1.x).  Checked when present: pixels_per_column == H, columns_per_packet == 16.  LV_ERR_ARG for a null argument,
+ * len < 0, a missing or malformed required key, W or H outside its set, any other profile (the FUSA ones, a misspelt name), or a
+ * check that fails (*out and *profile are then zeroed).  Host code. */
+lv_status lv_ouster_sensor_from_json(const char* text, int64_t len, lv_ouster_calibration* out, lv_ouster_profile* profile);
+/* lv_ouster_sensor_from_json for LEGACY sensors: a profile other than LEGACY is LV_ERR_ARG, with *out zeroed. */
 lv_status lv_ouster_calibration_from_json(const char* text, int64_t len, lv_ouster_calibration* out);
 /* msg2points on the host: the points of the packets, in slot order, into xyz (3 x 16 H n_packets), time, intensity, range and idx
  * (16 H n_packets each; intensity, range and idx may be NULL); *n_out = their count.  LV_ERR_ARG for null packets / cal / xyz /
- * time / n_out, W or H outside its set, a non-finite calibration entry (the first H angles, n), n_packets outside [0, (2^31 - 1) /
- * (16 H)] or data_bytes < 16 (20 + 12 H) n_packets. */
+ * time / n_out, a profile outside lv_ouster_profile, W or H outside its set, a non-finite calibration entry (the first H angles,
+ * n), n_packets outside [0, (2^31 - 1) / (16 H)] or data_bytes below n_packets packets of the profile. */
+lv_status lv_ouster_packets_to_points(const uint8_t* packets, int64_t data_bytes, int64_t n_packets, const lv_ouster_calibration* cal,
+                                      lv_ouster_profile profile, float* xyz, double* time, float* intensity, float* range, int32_t* idx,
+                                      int64_t* n_out);
+/* lv_ouster_packets_to_points with LV_OUSTER_LEGACY */
 lv_status lv_ouster_to_points(const uint8_t* packets, int64_t data_bytes, int64_t n_packets, const lv_ouster_calibration* cal,
                               float* xyz, double* time, float* intensity, float* range, int32_t* idx, int64_t* n_out);
-/* Accumulator::process on the device for Ouster packets: msg2points -> temporal_downsample on the RANK of the point among the
- * msg2points points (not its slot) -> sort_points (stable in time, equal times in slot order, so within a column the points stay
- * in pixel order).  d_packets: DEVICE copy of the packets (data_bytes long, any alignment), e.g. the packets of one frame batched
- * into one upload.  Outputs as lv_process_livox_device, DEVICE buffers with room for 16 H n_packets points.  Bit for bit
- * lv_ouster_to_points, then lv_temporal_downsample on its output, then lv_time_sort_indices on the kept times, then the gathers.
- * The first call on a handle uploads the 2 x 2048-float column table (and waits for that copy); lv_destroy frees it.  LV_ERR_ARG,
- * before any device work and also with a null handle, for the host decoder's argument errors or an output range that overlaps
- * [d_packets, d_packets + data_bytes).  When 16 H n_packets < downsample_rate nothing can be kept and the packets are not read.
- * Synchronises (n_out). */
+/* Accumulator::process on the device for Ouster packets of the given profile: msg2points -> temporal_downsample on the RANK of the
+ * point among the msg2points points (not its slot) -> sort_points (stable in time, equal times in slot order, so within a column the
+ * points stay in pixel order).  d_packets: DEVICE copy of the packets (data_bytes long, any alignment), e.g. the packets of one frame
+ * batched into one upload.  Outputs as lv_process_livox_device, DEVICE buffers with room for 16 H n_packets points.  Bit for bit
+ * lv_ouster_packets_to_points, then lv_temporal_downsample on its output, then lv_time_sort_indices on the kept times, then the
+ * gathers.  The first call on a handle uploads the 2 x 2048-float column table (and waits for that copy); lv_destroy frees it.
+ * LV_ERR_ARG, before any device work and also with a null handle, for the host decoder's argument errors or an output range that
+ * overlaps [d_packets, d_packets + data_bytes).  When 16 H n_packets < downsample_rate nothing can be kept and the packets are not
+ * read.  Synchronises (n_out). */
+lv_status lv_process_ouster_packets_device(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                           const lv_ouster_calibration* cal, lv_ouster_profile profile, int32_t downsample_rate,
+                                           double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                           int32_t* d_idx, int64_t* n_out);
+/* lv_process_ouster_packets_device with LV_OUSTER_LEGACY */
 lv_status lv_process_ouster_device(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
                                    const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist,
                                    float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out);
@@ -640,8 +673,13 @@ lv_status lv_process_velodyne_device_async(lv_handle h, const uint8_t* d_packets
                                            const lv_velodyne_calibration* cal, int32_t downsample_rate, double min_dist,
                                            float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
                                            int64_t* d_n_out);
-/* lv_process_ouster_device with *d_n_out = points kept; feeds lv_lidar_push_full_device_async or lv_lidar_merge_device_async
- * directly.  The output buffers have room for 16 H n_packets points.  No deferred error of its own. */
+/* lv_process_ouster_packets_device with *d_n_out = points kept; feeds lv_lidar_push_full_device_async or
+ * lv_lidar_merge_device_async directly.  The output buffers have room for 16 H n_packets points.  No deferred error of its own. */
+lv_status lv_process_ouster_packets_device_async(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                                 const lv_ouster_calibration* cal, lv_ouster_profile profile, int32_t downsample_rate,
+                                                 double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                                 int32_t* d_idx, int64_t* d_n_out);
+/* lv_process_ouster_packets_device_async with LV_OUSTER_LEGACY */
 lv_status lv_process_ouster_device_async(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
                                          const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist,
                                          float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx,
@@ -857,7 +895,8 @@ typedef struct lv_velodyne_view {
 } lv_velodyne_view;
 lv_status lv_bag_parse_velodyne_scan(const uint8_t* msg, int64_t size, lv_velodyne_view* out);
 /* ouster_ros/PacketMsg (uint8[] buf: a uint32 length, then the bytes) -> a view of its one packet: a LiDAR packet for
- * lv_ouster_to_points / lv_process_ouster_device, or an IMU packet for lv_ouster_imu_packet.  LV_ERR_ARG for a null argument, a
+ * lv_ouster_packets_to_points / lv_process_ouster_packets_device, or an IMU packet for lv_ouster_imu_packet.  LV_ERR_ARG for a
+ * null argument, a
  * truncated message or bytes after the packet. */
 typedef struct lv_ouster_packet_view {
     const uint8_t* data;                 /* the packet's first byte (any alignment)               */

@@ -224,6 +224,14 @@ def lib():
         L.lv_process_ouster_device_async.argtypes = [vp, vp, i64, i64, cp, C.c_int32, C.c_double, vp, vp, vp, vp, vp, vp]
         L.lv_bag_parse_ouster_packet.argtypes = [vp, i64, C.POINTER(OusterPacketView)]
         L.lv_ouster_imu_packet.argtypes = [vp, i64, C.POINTER(ImuSample)]
+    if hasattr(L, "lv_process_ouster_packets_device"):   # the Ouster UDP profiles of firmware 2.2+; absent from older builds
+        cp = C.POINTER(OusterCalibration)
+        L.lv_ouster_sensor_from_json.argtypes = [C.c_char_p, i64, cp, C.POINTER(C.c_int)]
+        L.lv_ouster_packets_to_points.argtypes = [vp, i64, i64, cp, C.c_int, vp, vp, vp, vp, vp, C.POINTER(i64)]
+        L.lv_process_ouster_packets_device.argtypes = [vp, vp, i64, i64, cp, C.c_int, C.c_int32, C.c_double, vp, vp, vp, vp, vp,
+                                                       C.POINTER(i64)]
+        L.lv_process_ouster_packets_device_async.argtypes = [vp, vp, i64, i64, cp, C.c_int, C.c_int32, C.c_double, vp, vp, vp, vp,
+                                                             vp, vp]
     if hasattr(L, "lv_lidar_reserve_merge"):   # the time-ordered merge of several LiDARs; absent from older builds
         L.lv_lidar_reserve_merge.argtypes = [vp, i64]
         L.lv_lidar_merge_device_async.argtypes = [vp, vp, vp, vp, i64, fp]
@@ -503,13 +511,20 @@ def velodyne_to_points(packets, cal):
     return tuple(a[:m.value].copy() for a in out)
 
 
-# ouster_ros/PacketMsg of an Ouster in the LEGACY profile: packets of 16 columns of 20 + 12 H bytes (include/limovelo_b200.h)
+# ouster_ros/PacketMsg of an Ouster: packets of 16 columns in one of four lidar UDP profiles (include/limovelo_b200.h, lv_ouster_profile)
 OUSTER_COLUMNS = 16
 OUSTER_IMU_PACKET = 48
+OUSTER_LEGACY, OUSTER_RNG19_RFL8_SIG16_NIR16, OUSTER_RNG19_RFL8_SIG16_NIR16_DUAL, OUSTER_RNG15_RFL8_NIR8 = range(4)
+OUSTER_PROFILES = {"LEGACY": OUSTER_LEGACY, "RNG19_RFL8_SIG16_NIR16": OUSTER_RNG19_RFL8_SIG16_NIR16,
+                   "RNG19_RFL8_SIG16_NIR16_DUAL": OUSTER_RNG19_RFL8_SIG16_NIR16_DUAL, "RNG15_RFL8_NIR8": OUSTER_RNG15_RFL8_NIR8}
+_OUSTER_PIXEL_BYTES = {OUSTER_RNG19_RFL8_SIG16_NIR16: 12, OUSTER_RNG19_RFL8_SIG16_NIR16_DUAL: 16, OUSTER_RNG15_RFL8_NIR8: 4}
 
 
-def ouster_packet_bytes(H):
-    return OUSTER_COLUMNS * (20 + 12 * H)
+def ouster_packet_bytes(H, profile=OUSTER_LEGACY):
+    """bytes per lidar packet: 16 (20 + 12 H) for LEGACY, 32 + 16 (12 + s H) + 32 for the others (s: the profile's pixel bytes)"""
+    if profile == OUSTER_LEGACY:
+        return OUSTER_COLUMNS * (20 + 12 * H)
+    return 64 + OUSTER_COLUMNS * (12 + _OUSTER_PIXEL_BYTES[profile] * H)
 
 
 class OusterCalibration(C.Structure):
@@ -545,6 +560,14 @@ def ouster_calibration_from_json(text):
     return cal
 
 
+def ouster_sensor_from_json(text):
+    """lv_ouster_sensor_from_json on the sensor metadata (str or bytes): (OusterCalibration, profile)"""
+    raw = text.encode() if isinstance(text, str) else bytes(text)
+    cal, profile = OusterCalibration(), C.c_int(-1)
+    _check(lib().lv_ouster_sensor_from_json(raw, len(raw), C.byref(cal), C.byref(profile)))
+    return cal, profile.value
+
+
 def bag_parse_ouster_packet(msg):
     """lv_bag_parse_ouster_packet on a serialised PacketMsg (bytes): the packet's bytes"""
     v = OusterPacketView()
@@ -562,16 +585,16 @@ def ouster_imu_packet(pkt):
     return s
 
 
-def ouster_to_points(packets, cal):
-    """msg2points of Ouster LEGACY packets on the host (packets: their bytes): returns (xyz, time, intensity, range, slot) of the
-    points, in slot order"""
+def ouster_to_points(packets, cal, profile=OUSTER_LEGACY):
+    """msg2points of Ouster packets of a lidar UDP profile on the host (packets: their bytes): returns (xyz, time, intensity, range,
+    slot) of the points, in slot order"""
     raw = np.ascontiguousarray(np.frombuffer(bytes(memoryview(packets)), np.uint8))
-    k = len(raw) // ouster_packet_bytes(cal.pixels_per_column)
+    k = len(raw) // ouster_packet_bytes(cal.pixels_per_column, profile)
     n = OUSTER_COLUMNS * cal.pixels_per_column * k
     out = (np.empty((n, 3), np.float32), np.empty(n), np.empty(n, np.float32), np.empty(n, np.float32), np.empty(n, np.int32))
     m = C.c_int64(0)
-    _check(lib().lv_ouster_to_points(raw.ctypes.data_as(C.c_void_p), len(raw), k, C.byref(cal),
-                                     *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
+    _check(lib().lv_ouster_packets_to_points(raw.ctypes.data_as(C.c_void_p), len(raw), k, C.byref(cal), int(profile),
+                                             *(a.ctypes.data_as(C.c_void_p) for a in out), C.byref(m)))
     return tuple(a[:m.value].copy() for a in out)
 
 
@@ -903,26 +926,28 @@ class Localizer:
                 self.device_free(d)
 
     def process_ouster_device(self, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity=None,
-                              d_range=None, d_idx=None):
-        """Accumulator::process on Ouster LEGACY packets already in device memory (raw pointers); returns the points kept"""
+                              d_range=None, d_idx=None, profile=OUSTER_LEGACY):
+        """Accumulator::process on Ouster packets of a lidar UDP profile already in device memory (raw pointers); returns the points
+        kept"""
         m = C.c_int64(0)
-        _check(self.L.lv_process_ouster_device(self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal),
-                                               int(downsample_rate), float(min_dist), C.c_void_p(d_xyz), C.c_void_p(d_time),
-                                               C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx), C.byref(m)))
+        _check(self.L.lv_process_ouster_packets_device(self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal),
+                                                       int(profile), int(downsample_rate), float(min_dist), C.c_void_p(d_xyz),
+                                                       C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range),
+                                                       C.c_void_p(d_idx), C.byref(m)))
         return m.value
 
-    def process_ouster(self, packets, cal, downsample_rate, min_dist):
-        """Accumulator::process on Ouster LEGACY packets (their bytes): uploads them, returns (xyz, time, intensity, range, slot) of the
-        kept points in time order"""
+    def process_ouster(self, packets, cal, downsample_rate, min_dist, profile=OUSTER_LEGACY):
+        """Accumulator::process on Ouster packets of a lidar UDP profile (their bytes): uploads them, returns (xyz, time, intensity,
+        range, slot) of the kept points in time order"""
         raw = np.frombuffer(bytes(memoryview(packets)), np.uint8)
-        k = len(raw) // ouster_packet_bytes(cal.pixels_per_column)
+        k = len(raw) // ouster_packet_bytes(cal.pixels_per_column, profile)
         n = OUSTER_COLUMNS * cal.pixels_per_column * k
         out = (np.empty((n, 3), np.float32), np.empty(n, np.float64), np.empty(n, np.float32), np.empty(n, np.float32),
                np.empty(n, np.int32))
         bufs = [self.device_alloc(max(raw.nbytes, 1))] + [self.device_alloc(max(a.nbytes, 1)) for a in out]
         try:
             _check(self.L.lv_memcpy_h2d(self.h, bufs[0], raw.ctypes.data_as(C.c_void_p), raw.nbytes))
-            m = self.process_ouster_device(bufs[0], raw.nbytes, k, cal, downsample_rate, min_dist, *bufs[1:])
+            m = self.process_ouster_device(bufs[0], raw.nbytes, k, cal, downsample_rate, min_dist, *bufs[1:], profile=profile)
             return tuple(self.download(d, a[:m]) for a, d in zip(out, bufs[1:]))
         finally:
             for d in bufs:
@@ -978,11 +1003,11 @@ class Localizer:
             C.c_void_p(d_n_out)))
 
     def process_ouster_device_async(self, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_n_out,
-                                    d_intensity=None, d_range=None, d_idx=None):
-        """lv_process_ouster_device with the count of kept points written to d_n_out"""
-        return _check(self.L.lv_process_ouster_device_async(
-            self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal), int(downsample_rate), float(min_dist),
-            C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
+                                    d_intensity=None, d_range=None, d_idx=None, profile=OUSTER_LEGACY):
+        """lv_process_ouster_packets_device with the count of kept points written to d_n_out"""
+        return _check(self.L.lv_process_ouster_packets_device_async(
+            self.h, C.c_void_p(d_packets), int(data_bytes), int(n_packets), C.byref(cal), int(profile), int(downsample_rate),
+            float(min_dist), C.c_void_p(d_xyz), C.c_void_p(d_time), C.c_void_p(d_intensity), C.c_void_p(d_range), C.c_void_p(d_idx),
             C.c_void_p(d_n_out)))
 
     def compensate_device_async(self, path, Xt2, d_xyz, d_t, d_n, n_max, d_out):

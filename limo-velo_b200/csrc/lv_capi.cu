@@ -1801,8 +1801,8 @@ lv_status lv_process_velodyne_device_async(lv_handle h, const uint8_t* d_packets
                                  d_idx, &unused, d_n_out);
 }
 
-/* Ouster LEGACY packets (lv_wire.h): msg2points, then the decimator on the rank among its points.  The first call uploads the column
- * table, which the context keeps */
+/* Ouster packets of any UDP profile (lv_wire.h): msg2points through the profile's layout, then the decimator on the rank among its
+ * points.  The first call uploads the column table, which the context keeps */
 static cudaError_t ouster_table_ready(lv_handle h) {
     if (h->ouster_table_ok) return cudaSuccess;
     std::vector<float> t(2 * kOusterTable);
@@ -1814,40 +1814,58 @@ static cudaError_t ouster_table_ready(lv_handle h) {
     return e;
 }
 static lv_status process_ouster_impl(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
-                                     const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz,
-                                     double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out, int64_t* d_n_out) {
+                                     const lv_ouster_calibration* cal, lv_ouster_profile profile, int32_t downsample_rate, double min_dist,
+                                     float* d_xyz, double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out,
+                                     int64_t* d_n_out) {
     const CloudOut o{d_xyz, d_time, d_intensity, d_range, d_idx};
-    /* a calibration or n_packets out of range leaves n at 0 here, and the layout check names it */
+    /* a calibration, profile or n_packets out of range leaves n at 0 here, and the layout check names it */
     const bool cal_ok = cal && !ouster_calib_error(*cal);
     const int H = cal_ok ? cal->pixels_per_column : 0;
-    const int64_t n = cal_ok && n_packets >= 0 && n_packets <= ouster_max_packets(H) ? n_packets * kOusterColumns * H : 0;
+    OusterFormat fmt{};
+    const bool fmt_ok = cal_ok && ouster_format(profile, H, &fmt);
+    const int64_t n = fmt_ok && n_packets >= 0 && n_packets <= ouster_max_packets(H) ? n_packets * kOusterColumns * H : 0;
     return front_end_impl(
         h, "process ouster", !d_packets || !cal || !d_xyz || !d_time, "packets, cal, xyz, time or n_out", d_packets, data_bytes, n,
         downsample_rate, o, n_out, d_n_out,
         [&]() -> const char* {
             if (const char* why = ouster_calib_error(*cal)) return why;
-            return ouster_layout_error(n_packets, data_bytes, H);
+            if (!fmt_ok) return "profile is not an lv_ouster_profile";
+            return ouster_layout_error(fmt, n_packets, data_bytes, H);
         },
         [&](int* launches, uint32_t* err) {
             const cudaError_t e = ouster_table_ready(h);
             if (e != cudaSuccess) return e;
-            const OusterArgs a = {d_packets, n, h->d_ouster_table, ouster_calib(*cal), downsample_rate, min_dist};
+            const OusterArgs a = {d_packets, n, h->d_ouster_table, ouster_calib(*cal), fmt, downsample_rate, min_dist};
             return launch_process_ouster(h->ds, a, o, d_n_out, err, h->stream, launches);
         });
+}
+lv_status lv_process_ouster_packets_device(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                           const lv_ouster_calibration* cal, lv_ouster_profile profile, int32_t downsample_rate,
+                                           double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                           int32_t* d_idx, int64_t* n_out) {
+    return process_ouster_impl(h, d_packets, data_bytes, n_packets, cal, profile, downsample_rate, min_dist, d_xyz, d_time, d_intensity,
+                               d_range, d_idx, n_out, nullptr);
+}
+lv_status lv_process_ouster_packets_device_async(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
+                                                 const lv_ouster_calibration* cal, lv_ouster_profile profile, int32_t downsample_rate,
+                                                 double min_dist, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
+                                                 int32_t* d_idx, int64_t* d_n_out) {
+    int64_t unused = 0;                                           /* the count stays on the device */
+    if (!d_n_out) { set_error("process ouster: null packets, cal, xyz, time or n_out"); return LV_ERR_ARG; }
+    return process_ouster_impl(h, d_packets, data_bytes, n_packets, cal, profile, downsample_rate, min_dist, d_xyz, d_time, d_intensity,
+                               d_range, d_idx, &unused, d_n_out);
 }
 lv_status lv_process_ouster_device(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
                                    const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz, double* d_time,
                                    float* d_intensity, float* d_range, int32_t* d_idx, int64_t* n_out) {
-    return process_ouster_impl(h, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range, d_idx,
-                               n_out, nullptr);
+    return lv_process_ouster_packets_device(h, d_packets, data_bytes, n_packets, cal, LV_OUSTER_LEGACY, downsample_rate, min_dist, d_xyz,
+                                            d_time, d_intensity, d_range, d_idx, n_out);
 }
 lv_status lv_process_ouster_device_async(lv_handle h, const uint8_t* d_packets, int64_t data_bytes, int64_t n_packets,
                                          const lv_ouster_calibration* cal, int32_t downsample_rate, double min_dist, float* d_xyz,
                                          double* d_time, float* d_intensity, float* d_range, int32_t* d_idx, int64_t* d_n_out) {
-    int64_t unused = 0;                                           /* the count stays on the device */
-    if (!d_n_out) { set_error("process ouster: null packets, cal, xyz, time or n_out"); return LV_ERR_ARG; }
-    return process_ouster_impl(h, d_packets, data_bytes, n_packets, cal, downsample_rate, min_dist, d_xyz, d_time, d_intensity, d_range, d_idx,
-                               &unused, d_n_out);
+    return lv_process_ouster_packets_device_async(h, d_packets, data_bytes, n_packets, cal, LV_OUSTER_LEGACY, downsample_rate, min_dist,
+                                                  d_xyz, d_time, d_intensity, d_range, d_idx, d_n_out);
 }
 
 /* the deferred errors of the _async calls (AsyncWords::err) and the map's flags; clears the former */

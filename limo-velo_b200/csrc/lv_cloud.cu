@@ -14,8 +14,8 @@
  * and its select come first, and the rank is the position among the tag-kept points (Accumulator.cpp:143-151 decimates the list
  * msg2points returns).  velodyne_msgs/VelodyneScan likewise: a validity flag (return mode, block flags, distance) and its select
  * come first, and the key kernel also checks every packet for a dual return or a stamp that does not convert (the flag kernel
- * resets that word, so the first kernel cannot raise it).  Ouster LEGACY packets the same way: a validity flag (column status,
- * measurement id, range) and its select, with no per-packet check: a column's time always converts.  The bytes of a kept point are read twice (flag + key, gather), those
+ * resets that word, so the first kernel cannot raise it).  Ouster packets of every UDP profile the same way: a validity flag
+ * (column status, measurement id, range) and its select, with no per-packet check: a column's time always converts.  The bytes of a kept point are read twice (flag + key, gather), those
  * of a dropped point once.  Every value is assembled from single bytes (lv_wire.h): fields sit at any offset and the message at any address.  Byte offsets are
  * 64-bit: n < 2^31 points of up to 2^31 bytes each.
  *
@@ -88,7 +88,8 @@ struct VelodyneSource {
     }
 };
 
-/* ouster LEGACY packets: a point is a slot (its column and pixel), decoded through the column table and the beam terms */
+/* ouster packets of any UDP profile: a point is a slot (its column and pixel), decoded through the profile's layout, the column table
+ * and the beam terms */
 struct OusterSlot {
     const uint8_t* col;
     int p;
@@ -96,14 +97,14 @@ struct OusterSlot {
 struct OusterSource {
     OusterArgs a;
     __device__ __forceinline__ OusterSlot point(int64_t i) const {
-        return {ouster_column(a.data, i, a.cal.H), (int)(i % a.cal.H)};
+        return {ouster_column(a.fmt, a.data, i, a.cal.H), (int)(i % a.cal.H)};
     }
     __device__ __forceinline__ void xyz(const OusterSlot& p, float& x, float& y, float& z) const {
-        ouster_xyz(p.col, p.p, a.table, a.table + kOusterTable, a.cal, x, y, z);
+        ouster_xyz(a.fmt, p.col, p.p, a.table, a.table + kOusterTable, a.cal, x, y, z);
     }
     __device__ __forceinline__ double time(const OusterSlot& p) const { return ouster_time(p.col); }
-    __device__ __forceinline__ float intensity(const OusterSlot& p) const { return ouster_reflectivity(p.col, p.p); }
-    __device__ __forceinline__ float range(const OusterSlot& p, float, float, float) const { return ouster_range(p.col, p.p); }
+    __device__ __forceinline__ float intensity(const OusterSlot& p) const { return ouster_reflectivity(a.fmt, p.col, p.p); }
+    __device__ __forceinline__ float range(const OusterSlot& p, float, float, float) const { return ouster_range(a.fmt, p.col, p.p); }
     __device__ __forceinline__ void check(int64_t, int64_t, int*, uint32_t*) const {}
 };
 
@@ -140,7 +141,7 @@ __global__ void __launch_bounds__(256) lv_velodyne_valid_kernel(VelodyneArgs a, 
 __global__ void __launch_bounds__(256) lv_ouster_valid_kernel(OusterArgs a, uint8_t* __restrict__ keep) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n) return;
-    keep[i] = ouster_slot_valid(ouster_column(a.data, i, a.cal.H), (int)(i % a.cal.H), a.cal.W, a.cal.H) ? 1 : 0;
+    keep[i] = ouster_slot_valid(a.fmt, ouster_column(a.fmt, a.data, i, a.cal.H), (int)(i % a.cal.H), a.cal.W) ? 1 : 0;
 }
 
 /* msg2points' tag filter of a livox message */

@@ -272,13 +272,14 @@ struct VelodyneArgs {
 };
 cudaError_t launch_process_velodyne(DownsampleScratch& s, const VelodyneArgs& a, const CloudOut& o, int64_t* d_n_out, uint32_t* err,
                                     cudaStream_t st, int* launches);
-/* the same for Ouster LEGACY packets: msg2points (column status, measurement id, range), then the decimator on the rank among its
- * points (lv_wire.h).  No deferred error of its own: a column's time always converts */
+/* the same for Ouster packets of any UDP profile: msg2points (column status, measurement id, range), then the decimator on the rank
+ * among its points (lv_wire.h).  No deferred error of its own: a column's time always converts */
 struct OusterArgs {
     const uint8_t* data;       /* the packets (device, any alignment) */
     int64_t n;                 /* 16 H n_packets slots */
     const float* table;        /* C then S, kOusterTable floats each (ouster_table, device) */
     OusterCalib cal;           /* the beam terms, by value: the kernels read them from the parameter bank */
+    OusterFormat fmt;          /* where the profile keeps a column's fields (ouster_format), by value */
     int32_t rate;
     double min_dist;
 };

@@ -252,14 +252,23 @@ inline const char* velodyne_layout_error(int64_t n_packets, int64_t data_bytes) 
     return nullptr;
 }
 
-/* ---- ouster_ros/PacketMsg of an OS0 / OS1 / OS2 in the LEGACY profile (include/limovelo_b200.h, "Ouster packets"): packets of 16
- * columns of 20 + 12 H bytes
- *   uint64 timestamp (ns) | uint16 measurement_id m | uint16 frame_id | uint32 encoder (unused) | H x 12-byte pixels | uint32 status
- * pixel: uint32 range word (low 20 bits: range in mm) | uint16 reflectivity | 6 bytes of signal and noise (unused).
- * The packets are contiguous, so column g = k 16 + c of the message starts at packets + g (20 + 12 H), any alignment.
- * Slot i of the message: column g = i / H, pixel p = i % H. */
+/* ---- ouster_ros/PacketMsg of an OS0 / OS1 / OS2 (include/limovelo_b200.h, "Ouster packets"): packets of 16 columns in one of four
+ * UDP profiles.  What differs between the profiles is data, an OusterFormat built on the host (ouster_format); one decoder reads
+ * all four through it.
+ *   LEGACY   packet: 16 columns of 20 + 12 H bytes
+ *            column: uint64 timestamp (ns) | uint16 measurement_id m | uint16 frame_id | uint32 encoder | H x 12-byte pixels |
+ *                    uint32 status
+ *            pixel:  uint32 range word (low 20 bits: range in mm) | uint16 reflectivity | signal, noise
+ *   others   packet: 32-byte header | 16 columns of 12 + s H bytes | 32-byte footer (header and footer not read)
+ *            column: uint64 timestamp (ns) | uint16 measurement_id m | uint16 status | H x s-byte pixels
+ *            pixel:  RNG19_RFL8_SIG16_NIR16        s = 12  range = u32 @0 & 0x7FFFF          reflectivity = u8 @4
+ *                    RNG19_RFL8_SIG16_NIR16_DUAL   s = 16  range = u32 @0 & 0x7FFFF (first)  reflectivity = u8 @3 (first)
+ *                    RNG15_RFL8_NIR8 (low data)    s = 4   range = (u16 @0 & 0x7FFF) << 3    reflectivity = u8 @2
+ * Every profile keeps the timestamp at byte 0 and the measurement id at byte 8 of the column, and bit 0 of the status' first byte
+ * says the column is valid.  The low-data range is read as u32 @0 under the mask, which gives the same bits as u16 @0.  Packet k
+ * starts at packets + k packet bytes, any alignment.  Slot i of the message: column g = i / H (packet g / 16, column g % 16),
+ * pixel p = i % H. */
 enum { kOusterColumns = 16, kOusterMaxBeams = 128, kOusterTable = 2048 };
-constexpr uint32_t kOusterRangeMask = 0xFFFFFu;
 
 /* the calibration in the fp32 terms the point arithmetic reads (ouster_calib): per beam, cos / sin of the altitude and the azimuth */
 struct OusterCalib {
@@ -269,36 +278,54 @@ struct OusterCalib {
     int32_t W, H;                                     /* columns per frame, pixels per column */
 };
 
+/* where a UDP profile keeps a packet's fields, for one H (ouster_format) */
+struct OusterFormat {
+    int32_t packet;            /* bytes per packet                                                  */
+    int32_t header;            /* bytes before the first column (the packet header)                 */
+    int32_t column;            /* bytes per column                                                  */
+    int32_t pixels;            /* offset of pixel 0 in the column (the column header's bytes)       */
+    int32_t stride;            /* bytes per pixel                                                   */
+    int32_t status;            /* offset in the column of the status byte whose bit 0 is read       */
+    uint32_t range_mask;       /* range = (u32 at the pixel's byte 0 & range_mask) << range_shift   */
+    int32_t range_shift;
+    int32_t refl;              /* offset of the reflectivity in the pixel                           */
+    int32_t refl_bytes;        /* its width: 1 or 2                                                 */
+};
+
 LV_HD uint64_t wire_u64(const uint8_t* p) { return (uint64_t)wire_u32(p) | (uint64_t)wire_u32(p + 4) << 32; }
-LV_HD int64_t ouster_column_bytes(int H) { return 20 + 12 * (int64_t)H; }
-LV_HD int64_t ouster_packet_bytes(int H) { return kOusterColumns * ouster_column_bytes(H); }
 /* the column of slot i and its pixel p */
-LV_HD const uint8_t* ouster_column(const uint8_t* packets, int64_t i, int H) {
-    return packets + (uint64_t)(i / H) * (uint64_t)ouster_column_bytes(H);
+LV_HD const uint8_t* ouster_column(const OusterFormat& f, const uint8_t* packets, int64_t i, int H) {
+    const uint64_t g = (uint64_t)(i / H);
+    return packets + (g / kOusterColumns) * (uint64_t)f.packet + (uint64_t)f.header + (g % kOusterColumns) * (uint64_t)f.column;
 }
-LV_HD const uint8_t* ouster_pixel(const uint8_t* col, int p) { return col + 16 + 12 * p; }
+LV_HD const uint8_t* ouster_pixel(const OusterFormat& f, const uint8_t* col, int p) { return col + f.pixels + f.stride * p; }
 LV_HD uint32_t ouster_measurement_id(const uint8_t* col) { return wire_u16(col + 8); }
-LV_HD uint32_t ouster_status(const uint8_t* col, int H) { return wire_u32(col + 16 + 12 * H); }
-LV_HD uint32_t ouster_range_mm(const uint8_t* col, int p) { return wire_u32(ouster_pixel(col, p)) & kOusterRangeMask; }
+LV_HD uint32_t ouster_range_mm(const OusterFormat& f, const uint8_t* col, int p) {
+    return (wire_u32(ouster_pixel(f, col, p)) & f.range_mask) << f.range_shift;
+}
 
 /* msg2points: the column's status has bit 0 set, its measurement id is a column of the frame, and the pixel has a return */
-LV_HD bool ouster_slot_valid(const uint8_t* col, int p, int W, int H) {
-    return (ouster_status(col, H) & 1u) && ouster_measurement_id(col) < (uint32_t)W && ouster_range_mm(col, p) != 0;
+LV_HD bool ouster_slot_valid(const OusterFormat& f, const uint8_t* col, int p, int W) {
+    return (wire_u8(col + f.status) & 1u) && ouster_measurement_id(col) < (uint32_t)W && ouster_range_mm(f, col, p) != 0;
 }
 /* the point of pixel p of a valid column (C, S: the column table of ouster_table), in the LiDAR frame (os_lidar), fp32, each
  * product and sum rounded, in the order of the header */
-LV_HD void ouster_xyz(const uint8_t* col, int p, const float* C, const float* S, const OusterCalib& k, float& x, float& y, float& z) {
+LV_HD void ouster_xyz(const OusterFormat& f, const uint8_t* col, int p, const float* C, const float* S, const OusterCalib& k, float& x,
+                      float& y, float& z) {
     const int q = (int)ouster_measurement_id(col) * (kOusterTable / k.W);
     const float c = C[q], s = S[q];
-    const float e = fsub(fmul((float)ouster_range_mm(col, p), 0.001f), k.nf);
+    const float e = fsub(fmul((float)ouster_range_mm(f, col, p), 0.001f), k.nf);
     const float ch = fsub(fmul(c, k.ca[p]), fmul(s, k.sa[p])), sh = fadd(fmul(s, k.ca[p]), fmul(c, k.sa[p]));
     const float ee = fmul(e, k.ce[p]);
     x = fadd(fmul(ee, ch), fmul(k.nf, c));
     y = -fadd(fmul(ee, sh), fmul(k.nf, s));
     z = fmul(e, k.se[p]);
 }
-LV_HD float ouster_reflectivity(const uint8_t* col, int p) { return (float)wire_u16(ouster_pixel(col, p) + 4); }
-LV_HD float ouster_range(const uint8_t* col, int p) { return (float)ouster_range_mm(col, p); }
+LV_HD float ouster_reflectivity(const OusterFormat& f, const uint8_t* col, int p) {
+    const uint8_t* r = ouster_pixel(f, col, p) + f.refl;
+    return (float)(f.refl_bytes == 2 ? wire_u16(r) : wire_u8(r));
+}
+LV_HD float ouster_range(const OusterFormat& f, const uint8_t* col, int p) { return (float)ouster_range_mm(f, col, p); }
 /* the column's own timestamp, absolute */
 LV_HD double ouster_time(const uint8_t* col) { return wire_ns_to_sec(wire_u64(col)); }
 
@@ -338,11 +365,32 @@ inline OusterCalib ouster_calib(const lv_ouster_calibration& c) {
 /* the most packets whose slot indices fit an int32 */
 inline int64_t ouster_max_packets(int H) { return 0x7fffffff / (kOusterColumns * (int64_t)H); }
 
-/* NULL when n_packets is in range and its packets fit data_bytes (H from a calibration ouster_calib_error accepts), else what is wrong */
-inline const char* ouster_layout_error(int64_t n_packets, int64_t data_bytes, int H) {
+/* the layout of a profile for H pixels per column; false for a value outside lv_ouster_profile (*f is then left as it was) */
+inline bool ouster_format(int profile, int H, OusterFormat* f) {
+    if (profile == LV_OUSTER_LEGACY) {
+        const int32_t column = 20 + 12 * H;
+        *f = {kOusterColumns * column, 0, column, 16, 12, 16 + 12 * H, 0xFFFFFu, 0, 4, 2};
+        return true;
+    }
+    int32_t s, refl, shift = 0;
+    uint32_t mask;
+    switch (profile) {
+        case LV_OUSTER_RNG19_RFL8_SIG16_NIR16: s = 12; mask = 0x7FFFFu; refl = 4; break;
+        case LV_OUSTER_RNG19_RFL8_SIG16_NIR16_DUAL: s = 16; mask = 0x7FFFFu; refl = 3; break;
+        case LV_OUSTER_RNG15_RFL8_NIR8: s = 4; mask = 0x7FFFu; shift = 3; refl = 2; break;
+        default: return false;
+    }
+    const int32_t column = 12 + s * H;
+    *f = {32 + kOusterColumns * column + 32, 32, column, 12, s, 10, mask, shift, refl, 1};
+    return true;
+}
+
+/* NULL when n_packets is in range and its packets fit data_bytes (H from a calibration ouster_calib_error accepts, f its profile's
+ * layout), else what is wrong */
+inline const char* ouster_layout_error(const OusterFormat& f, int64_t n_packets, int64_t data_bytes, int H) {
     if (n_packets < 0 || data_bytes < 0) return "negative packet count or data length";
     if (n_packets > ouster_max_packets(H)) return "n_packets above (2^31 - 1) / (16 pixels_per_column) (slot indices are int32)";
-    if (n_packets > data_bytes / ouster_packet_bytes(H)) return "data_bytes is too short for n_packets packets of 16 (20 + 12 pixels_per_column) bytes";
+    if (n_packets > data_bytes / f.packet) return "data_bytes is too short for n_packets packets of the profile";
     return nullptr;
 }
 

@@ -306,24 +306,26 @@ class Accumulator {
             check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, 384 * m.n_packets),
                   "Accumulator::receive_velodyne_device_full");
     }
-    /* receive_lidar_device for Ouster LEGACY packets (lv_process_ouster_device_async: the packets decoded through the beam intrinsics,
-     * decimation on the rank among the points, time sort); the packets in device memory, e.g. the PacketMsgs of one frame batched
-     * into one upload.  The output buffers hold 16 H n_packets points (H = cal->pixels_per_column). */
+    /* receive_lidar_device for Ouster packets (lv_process_ouster_packets_device_async: the packets of the sensor's lidar UDP profile
+     * decoded through the beam intrinsics, decimation on the rank among the points, time sort); the packets in device memory, e.g. the
+     * PacketMsgs of one frame batched into one upload.  The output buffers hold 16 H n_packets points (H = cal->pixels_per_column).
+     * profile: the metadata's udp_profile_lidar (lv_ouster_sensor_from_json), LEGACY when left out. */
     struct DeviceOusterMessage {
         const uint8_t* d_packets; int64_t data_bytes, n_packets; const lv_ouster_calibration* cal; int32_t downsample_rate; double min_dist;
+        lv_ouster_profile profile = LV_OUSTER_LEGACY;
         int64_t slots() const { return 16 * (int64_t)cal->pixels_per_column * n_packets; }
     };
     void receive_ouster_device(const DeviceOusterMessage& m, float* d_xyz, double* d_time, int64_t* d_n) {
-        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
-                                             d_time, nullptr, nullptr, nullptr, d_n),
+        check(lv_process_ouster_packets_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.profile, m.downsample_rate,
+                                                     m.min_dist, d_xyz, d_time, nullptr, nullptr, nullptr, d_n),
               "Accumulator::receive_ouster_device");
         if (m.n_packets > 0) check(lv_lidar_push_device_async(ctx->h, d_xyz, d_time, d_n, m.slots()), "Accumulator::receive_ouster_device");
     }
     /* the same with whole Points: intensity = reflectivity, range = the range in mm */
     void receive_ouster_device_full(const DeviceOusterMessage& m, float* d_xyz, double* d_time, float* d_intensity, float* d_range,
                                     int64_t* d_n) {
-        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
-                                             d_time, d_intensity, d_range, nullptr, d_n),
+        check(lv_process_ouster_packets_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.profile, m.downsample_rate,
+                                                     m.min_dist, d_xyz, d_time, d_intensity, d_range, nullptr, d_n),
               "Accumulator::receive_ouster_device_full");
         if (m.n_packets > 0)
             check(lv_lidar_push_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.slots()),
@@ -381,16 +383,16 @@ class Accumulator {
                   "Accumulator::receive_velodyne_device_full");
     }
     void receive_ouster_device(const DeviceOusterMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, int64_t* d_n) {
-        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
-                                             d_time, nullptr, nullptr, nullptr, d_n),
+        check(lv_process_ouster_packets_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.profile, m.downsample_rate,
+                                                     m.min_dist, d_xyz, d_time, nullptr, nullptr, nullptr, d_n),
               "Accumulator::receive_ouster_device");
         if (m.n_packets > 0)
             check(lv_lidar_merge_device_async(ctx->h, d_xyz, d_time, d_n, m.slots(), L0_T_Lk), "Accumulator::receive_ouster_device");
     }
     void receive_ouster_device_full(const DeviceOusterMessage& m, const float* L0_T_Lk, float* d_xyz, double* d_time, float* d_intensity,
                                     float* d_range, int64_t* d_n) {
-        check(lv_process_ouster_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.downsample_rate, m.min_dist, d_xyz,
-                                             d_time, d_intensity, d_range, nullptr, d_n),
+        check(lv_process_ouster_packets_device_async(ctx->h, m.d_packets, m.data_bytes, m.n_packets, m.cal, m.profile, m.downsample_rate,
+                                                     m.min_dist, d_xyz, d_time, d_intensity, d_range, nullptr, d_n),
               "Accumulator::receive_ouster_device_full");
         if (m.n_packets > 0)
             check(lv_lidar_merge_full_device_async(ctx->h, d_xyz, d_time, d_intensity, d_range, d_n, m.slots(), L0_T_Lk),

@@ -234,13 +234,17 @@ bool lidar_mode_columns(const std::string& mode, int32_t* W) {
 
 }  // namespace
 
-extern "C" lv_status lv_ouster_calibration_from_json(const char* text, int64_t len, lv_ouster_calibration* out) {
-    if (!text || len < 0 || !out) return LV_ERR_ARG;
+/* the udp_profile_lidar strings the decoder reads, in lv_ouster_profile order */
+static const char* const kOusterProfiles[] = {"LEGACY", "RNG19_RFL8_SIG16_NIR16", "RNG19_RFL8_SIG16_NIR16_DUAL", "RNG15_RFL8_NIR8"};
+
+extern "C" lv_status lv_ouster_sensor_from_json(const char* text, int64_t len, lv_ouster_calibration* out, lv_ouster_profile* profile) {
+    if (!text || len < 0 || !out || !profile) return LV_ERR_ARG;
     memset(out, 0, sizeof(*out));
+    *profile = LV_OUSTER_LEGACY;
     const std::string t(text, (size_t)len);
     const JsonScan j(t);
     std::vector<double> alt, az;
-    std::string mode, profile;
+    std::string mode, name;
     int32_t W = 0;
     if (!j.numbers("beam_altitude_angles", &alt) || !j.numbers("beam_azimuth_angles", &az) || alt.size() != az.size() ||
         !j.str("lidar_mode", &mode) || !lidar_mode_columns(mode, &W))
@@ -250,7 +254,14 @@ extern "C" lv_status lv_ouster_calibration_from_json(const char* text, int64_t l
     double v = 0;
     if (j.has("pixels_per_column") && (!j.number("pixels_per_column", &v) || v != H)) return LV_ERR_ARG;
     if (j.has("columns_per_packet") && (!j.number("columns_per_packet", &v) || v != 16)) return LV_ERR_ARG;
-    if (j.has("udp_profile_lidar") && (!j.str("udp_profile_lidar", &profile) || profile != "LEGACY")) return LV_ERR_ARG;
+    int kind = LV_OUSTER_LEGACY;                                  /* firmware 1.x has no udp_profile_lidar: LEGACY */
+    if (j.has("udp_profile_lidar")) {
+        if (!j.str("udp_profile_lidar", &name)) return LV_ERR_ARG;
+        kind = -1;
+        for (int k = 0; k < 4; ++k)
+            if (name == kOusterProfiles[k]) kind = k;
+        if (kind < 0) return LV_ERR_ARG;
+    }
     double n = 0;
     if (j.has("lidar_origin_to_beam_origin_mm") && !j.number("lidar_origin_to_beam_origin_mm", &n)) return LV_ERR_ARG;
     out->columns_per_frame = W;
@@ -260,5 +271,17 @@ extern "C" lv_status lv_ouster_calibration_from_json(const char* text, int64_t l
         out->beam_azimuth_angles[p] = az[p];
     }
     out->lidar_origin_to_beam_origin_mm = n;
+    *profile = (lv_ouster_profile)kind;
+    return LV_OK;
+}
+
+extern "C" lv_status lv_ouster_calibration_from_json(const char* text, int64_t len, lv_ouster_calibration* out) {
+    lv_ouster_profile profile;
+    const lv_status st = lv_ouster_sensor_from_json(text, len, out, &profile);
+    if (st != LV_OK) return st;
+    if (profile != LV_OUSTER_LEGACY) {
+        memset(out, 0, sizeof(*out));
+        return LV_ERR_ARG;
+    }
     return LV_OK;
 }

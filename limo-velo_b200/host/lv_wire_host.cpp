@@ -7,7 +7,7 @@
  * One pass over the message bytes per sweep (a few MB); the per-point arithmetic is csrc/lv_wire.h, which
  * lv_process_cloud_device (csrc/lv_cloud.cu) runs on the device.  lv_livox_to_points is the same for a Livox CustomMsg
  * (lv_process_livox_device on the device), lv_velodyne_to_points for a VelodyneScan's packets (lv_process_velodyne_device),
- * lv_ouster_to_points for Ouster LEGACY packets (lv_process_ouster_device).
+ * lv_ouster_packets_to_points for Ouster packets of any UDP profile (lv_process_ouster_packets_device).
  */
 #include <math.h>
 
@@ -100,11 +100,13 @@ lv_status lv_velodyne_to_points(const uint8_t* packets, int64_t data_bytes, int6
     return LV_OK;
 }
 
-lv_status lv_ouster_to_points(const uint8_t* packets, int64_t data_bytes, int64_t n_packets, const lv_ouster_calibration* cal, float* xyz,
-                              double* time, float* intensity, float* range, int32_t* idx, int64_t* n_out) {
+lv_status lv_ouster_packets_to_points(const uint8_t* packets, int64_t data_bytes, int64_t n_packets, const lv_ouster_calibration* cal,
+                                      lv_ouster_profile profile, float* xyz, double* time, float* intensity, float* range, int32_t* idx,
+                                      int64_t* n_out) {
     if (n_out) *n_out = 0;
+    lv::OusterFormat f;
     if (!packets || !cal || !xyz || !time || !n_out || lv::ouster_calib_error(*cal) ||
-        lv::ouster_layout_error(n_packets, data_bytes, cal->pixels_per_column))
+        !lv::ouster_format(profile, cal->pixels_per_column, &f) || lv::ouster_layout_error(f, n_packets, data_bytes, cal->pixels_per_column))
         return LV_ERR_ARG;
     static const std::vector<float> table = [] {
         std::vector<float> t(2 * lv::kOusterTable);
@@ -115,20 +117,24 @@ lv_status lv_ouster_to_points(const uint8_t* packets, int64_t data_bytes, int64_
     const lv::OusterCalib k = lv::ouster_calib(*cal);
     int64_t m = 0;
     for (int64_t i = 0; i < n_packets * lv::kOusterColumns * k.H; ++i) {
-        const uint8_t* col = lv::ouster_column(packets, i, k.H);
+        const uint8_t* col = lv::ouster_column(f, packets, i, k.H);
         const int p = (int)(i % k.H);
-        if (!lv::ouster_slot_valid(col, p, k.W, k.H)) continue;
+        if (!lv::ouster_slot_valid(f, col, p, k.W)) continue;
         float x, y, z;
-        lv::ouster_xyz(col, p, C, S, k, x, y, z);
+        lv::ouster_xyz(f, col, p, C, S, k, x, y, z);
         xyz[3 * m] = x; xyz[3 * m + 1] = y; xyz[3 * m + 2] = z;
         time[m] = lv::ouster_time(col);
-        if (intensity) intensity[m] = lv::ouster_reflectivity(col, p);
-        if (range) range[m] = lv::ouster_range(col, p);
+        if (intensity) intensity[m] = lv::ouster_reflectivity(f, col, p);
+        if (range) range[m] = lv::ouster_range(f, col, p);
         if (idx) idx[m] = (int32_t)i;
         ++m;
     }
     *n_out = m;
     return LV_OK;
+}
+lv_status lv_ouster_to_points(const uint8_t* packets, int64_t data_bytes, int64_t n_packets, const lv_ouster_calibration* cal, float* xyz,
+                              double* time, float* intensity, float* range, int32_t* idx, int64_t* n_out) {
+    return lv_ouster_packets_to_points(packets, data_bytes, n_packets, cal, LV_OUSTER_LEGACY, xyz, time, intensity, range, idx, n_out);
 }
 
 lv_status lv_time_sort_indices(const double* time, int64_t n, int32_t* idx_out) {

@@ -152,3 +152,26 @@ for d in outs + [d_msg, d_n]:
     loc.device_free(d)
 loc.close()
 print("sanitize target: process ouster ok", flush=True)
+
+# the Ouster UDP profiles of firmware 2.2+ (lv_process_ouster_packets_device, both forms): packets at an odd device address, across
+# the frame wrap, with random packet headers and footers, flag bits above the range masks and a second return, against the restatement
+import ouster_profile_cases as OP
+loc = lv.Localizer(lv.default_params(max_points=1 << 14, max_map_points=1 << 13))
+outs = [loc.device_alloc(k * 16 * 32 * 12) for k in (12, 8, 4, 4, 4)]
+d_msg, d_n = loc.device_alloc(OP.profile_packet_bytes(OP.DUAL, 32) * 12 + 8), loc.device_alloc(8)
+for profile in OP.NEW_PROFILES:
+    for name, pk in (("frame", OP.profile_packets(rng, 12, 1024, 32, profile, m0=1000)),
+                     ("sparse", OP.profile_packets(rng, 5, 1024, 32, profile, invalid=0.3, bad_m=0.3))):
+        ref = OP.profile_process(pk, cal, profile, 2, 0.5)
+        raw = np.frombuffer(pk.tobytes(), np.uint8)
+        assert loc.L.lv_memcpy_h2d(loc.h, C.c_void_p(d_msg + 1), raw.ctypes.data_as(C.c_void_p), raw.nbytes) == 0
+        loc.process_ouster_device_async(d_msg + 1, raw.nbytes, len(pk), cal, 2, 0.5, outs[0], outs[1], d_n, *outs[2:], profile=profile)
+        m = int(loc.download(d_n, np.zeros(1, np.int64))[0])
+        got = [loc.download(d, np.empty_like(a)) for d, a in zip(outs, ref)]
+        assert m == len(ref[0]) and all(np.array_equal(a.view(np.uint8), b.view(np.uint8)) for a, b in zip(got, ref)), (profile, name)
+        assert loc.async_status()[0] == lv.OK, (profile, name)
+        assert loc.process_ouster_device(d_msg + 1, raw.nbytes, len(pk), cal, 2, 0.5, *outs, profile=profile) == len(ref[0])
+for d in outs + [d_msg, d_n]:
+    loc.device_free(d)
+loc.close()
+print("sanitize target: process ouster profiles ok", flush=True)
