@@ -22,6 +22,7 @@
 
 #include "../../limo-velo_b200/csrc/lv_ieskf.h"
 #include "../../limo-velo_b200/csrc/lv_voxel_search.h"
+#include "../gpu_shim/manifold_ops.h"
 
 using namespace lv;
 
@@ -350,6 +351,10 @@ int shim_step(const double* x_prop, const double* P_prop, const double* x_cur, c
     return st;
 }
 
+/* tests/gpu_shim's gs_manifold on the host: manifold_op (manifold_ops.h) over n rows */
+void shim_manifold(const int* op, const double* in, double* out, int n) {
+    for (int i = 0; i < n; ++i) manifold_op(op[i], in + (size_t)kManIn * i, out + (size_t)kManOut * i);
+}
 void shim_boxplus(double* x, const double* d) { state_boxplus(x, d); }
 void shim_boxminus(const double* x, const double* y, double* d) { state_boxminus(x, y, d); }
 void shim_plane_fit(const float* pts5, float thr, float* abcd, int* ok) {

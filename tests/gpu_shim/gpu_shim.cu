@@ -13,6 +13,7 @@
 
 #include "../../limo-velo_b200/csrc/lv_internal.h"
 #include "../../limo-velo_b200/csrc/lv_predict.h"
+#include "manifold_ops.h"
 
 using namespace lv;
 
@@ -48,6 +49,13 @@ __global__ void gs_fit_sets_kernel(const float* q_in, const float* g_in, const i
     dist_out[i] = dist;
     for (int k = 0; k < 12; ++k) row_out[13 * (size_t)i + k] = row[k];
     row_out[13 * (size_t)i + 12] = h;
+}
+
+/* manifold_op (manifold_ops.h) over n rows, one thread per row: the lv_manifold.h functions as the device build runs them */
+__global__ void gs_manifold_kernel(const int* op, const double* in, double* out, int n) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    manifold_op(op[i], in + (size_t)kManIn * i, out + (size_t)kManOut * i);
 }
 
 #define GS_CUDA(call)                             \
@@ -291,6 +299,25 @@ int gs_fit_sets(const float* q, const float* g, const int* id, const double* x, 
 out:
     cudaFree(dq); cudaFree(dg); cudaFree(did); cudaFree(dido); cudaFree(dabcd); cudaFree(dok); cudaFree(ddist); cudaFree(drows);
     cudaFree(dfr);
+    return rc;
+}
+
+/* gs_manifold_kernel on n rows (host arrays: op[n], in[n x kManIn], out[n x kManOut]); returns a cudaError_t */
+int gs_manifold(const int* op, const double* in, double* out, int n) {
+    int rc = 0;
+    int* dop = nullptr;
+    double *din = nullptr, *dout = nullptr;
+    GS_CUDA(cudaMalloc(&dop, sizeof(int) * (size_t)n));
+    GS_CUDA(cudaMalloc(&din, sizeof(double) * kManIn * (size_t)n));
+    GS_CUDA(cudaMalloc(&dout, sizeof(double) * kManOut * (size_t)n));
+    GS_CUDA(cudaMemcpy(dop, op, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice));
+    GS_CUDA(cudaMemcpy(din, in, sizeof(double) * kManIn * (size_t)n, cudaMemcpyHostToDevice));
+    GS_CUDA(cudaMemset(dout, 0, sizeof(double) * kManOut * (size_t)n));
+    gs_manifold_kernel<<<(unsigned)((n + 127) / 128), 128>>>(dop, din, dout, n);
+    GS_CUDA(cudaGetLastError());
+    GS_CUDA(cudaMemcpy(out, dout, sizeof(double) * kManOut * (size_t)n, cudaMemcpyDeviceToHost));
+out:
+    cudaFree(dop); cudaFree(din); cudaFree(dout);
     return rc;
 }
 

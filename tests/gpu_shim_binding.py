@@ -25,6 +25,7 @@ def lib():
         L.gs_map_dims.argtypes = [vp, vp, vp]
         L.gs_map_dump.argtypes = [vp, vp, vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32]
         L.gs_map_free.argtypes = [vp]
+        L.gs_manifold.argtypes = [vp, vp, vp, C.c_int]
         L.gs_fit_sets.argtypes = [vp, vp, vp, vp, C.c_float, C.c_int, C.c_int, vp, vp, vp, vp, vp]
         _lib = L
     return _lib
@@ -63,6 +64,17 @@ def predict(x, P, acc, gyro, dt, noise):
     rc = lib().gs_predict(_d(x), _d(P), _d(imu), len(dt), _d(_a(noise)))
     assert rc == 0, "CUDA error %d" % rc
     return x, P
+
+
+def manifold(ops, rows):
+    """the lv_manifold.h functions on the device, one thread per row (tests/gpu_shim/manifold_ops.h: ops[n] op codes,
+    rows n x 64 inputs); returns n x 32 outputs"""
+    ops = np.ascontiguousarray(ops, np.int32)
+    rows = np.ascontiguousarray(rows, np.float64).reshape(len(ops), 64)
+    out = np.zeros((len(ops), 32))
+    rc = lib().gs_manifold(ops.ctypes.data, rows.ctypes.data, out.ctypes.data, len(ops))
+    assert rc == 0, "CUDA error %d" % rc
+    return out
 
 
 class GsMap:

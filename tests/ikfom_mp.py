@@ -17,7 +17,9 @@ mp.dps = 50
 
 N = 23
 TOL = mpmath.mpf("1e-11")               # MTK::tolerance<double>() (mtkmath.hpp:122)
-S2_LEN = mpmath.mpf(98090) / 10000      # S2<double, 98090, 10000, 1>: length = den / num (S2.hpp:104)
+S2_LEN = mpmath.mpf(98090.0 / 10000.0)  # S2<double, 98090, 10000, 1>: length = scalar(den) / scalar(num) (S2.hpp:104), a
+                                        # double: 9.809 - 7.2e-16.  Near the chart's edge (v.x + length <= tol, S2.hpp:217) that
+                                        # rounding is a relative 1e-4 of the chart, so the restatement takes the reference's double
 SO3_IDX = (3, 6)
 S2_IDX = 21
 _Q = {3: 3, 6: 7}                       # error-state index -> flat index of the quaternion

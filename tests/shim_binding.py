@@ -82,6 +82,8 @@ def lib():
         L.shim_pg_extent.argtypes = [fp, i64, f, f, C.POINTER(C.c_uint32), i32p]
         L.shim_pg_top_level.argtypes = [i64, i64]
 
+        L.shim_manifold.argtypes = [vp, vp, vp, C.c_int]
+        L.shim_manifold.restype = None
         L.shim_buf_fail_at.argtypes = [i64]
         L.shim_buf_fail_at.restype = None
         L.shim_buf_counts.argtypes = [C.POINTER(i64)]
@@ -248,6 +250,15 @@ def boxminus(x, y):
     d = np.zeros(23)
     lib().shim_boxminus(_d(np.ascontiguousarray(x, np.float64)), _d(np.ascontiguousarray(y, np.float64)), _d(d))
     return d
+
+
+def manifold(ops, rows):
+    """tests/gpu_shim_binding.manifold on the host build: the lv_manifold.h functions over rows (manifold_ops.h)"""
+    ops = np.ascontiguousarray(ops, np.int32)
+    rows = np.ascontiguousarray(rows, np.float64).reshape(len(ops), 64)
+    out = np.zeros((len(ops), 32))
+    lib().shim_manifold(ops.ctypes.data, rows.ctypes.data, out.ctypes.data, len(ops))
+    return out
 
 
 def plane_fit(pts5, thr):
